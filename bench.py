@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py — the lens-warp benchmark (driver contract).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 metric   lens-warp Mpixels/s (output pixels, W*H per frame) on the headline workload of
          BASELINE.json: 3840x2160 screen, cube globe of 6x2048^2 8-bit faces, panini lens.
 step     one pass of the hot path over one batch of FRAMES distinct synthetic frames per GPU
          (one kernel launch).  The frames of a batch are 16 x 25 MB = 403 MB of faces, larger
-         than the 126 MB L2, so every step streams its faces from HBM; the lensmap (static per
+         than the H100's 50 MB L2, so every step streams its faces from HBM; the lensmap (static per
          lens, like the reference's) is reused by all frames and stays L2-resident.
 value    N = 1: throughput with inputs resident in HBM (CUDA events on the launch stream).  N > 1: frames are
          independent — rank r warps its own batch, no collective on the data path ("weak" scaling;
@@ -18,13 +18,16 @@ value    N = 1: throughput with inputs resident in HBM (CUDA events on the launc
          max over ranks.
 e2e      the same metric through the C ABI's host entry point blinky_warp_host: pinned host
          faces -> batched async copies -> warp -> copy back, all inside the timed region.
-roofline frac = SURVEY 8(d) algorithmic bytes / launch time / measured HBM peak; compulsory_frac = bytes the
-         launch cannot avoid (counted from the lensmap in this run); dram_frac = ncu-measured DRAM bytes of
-         this workload's launch (profiles/traffic_r2.json) / this run's launch time.
+roofline frac = SURVEY 8(d) algorithmic bytes / launch time / HBM peak; compulsory_frac = bytes the
+         launch cannot avoid (counted from the lensmap in this run).
 secondary  every other BASELINE configuration (C2, C3, the C4 lenses, C5 trism/cube): batched and single
          cold frame, same three fractions.
 --impl reference   the reference's own CPU loop (oracle/_ref = unmodified fisheye.c compiled
          headless; else the oracle port) on the host cores, same workload, bounded sample.
+--dump-outputs DIR after the timed steps, what the last one computed as float32 .npy files: the last frame
+         of the batch (frame_last.npy, [H, W]) and a fixed sample of the whole batch (frames_sample.npy: the
+         flat [F*H*W] output at DUMP_SAMPLE positions drawn with numpy's default_rng(DUMP_SEED)).  The
+         inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 The oracle (oracle/) is only ever the thing TIMED BESIDE or CHECKED AGAINST — never the
 product path, which raises if libblinky_b200.so is missing.
@@ -56,7 +59,9 @@ WORKLOADS = {
     "c1-640x480": (640, 480, 256, "cube", "panini", "f_fov 180", False),                  # configs[0]
 }
 OUT = sys.stdout
-FALLBACK_HBM_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md, used only if MEASURED_PEAKS.json is absent
+FALLBACK_HBM_GBS = 3350.0  # H100 SXM data sheet (3.35 TB/s HBM3), used only if MEASURED_PEAKS.json is absent
+DUMP_SAMPLE = 4 << 20      # sampled output pixels in frames_sample.npy (16 MB as float32)
+DUMP_SEED = 0
 
 
 def hbm_peak():
@@ -64,7 +69,7 @@ def hbm_peak():
     try:
         return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
     except Exception:  # noqa: BLE001
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+        return FALLBACK_HBM_GBS, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -308,7 +313,7 @@ def time_single_frame_stream(torch, fe, d_faces, d_out, stream, rounds=3):
     return e0.elapsed_time(e1) * 1e-3 / (rounds * F)
 
 
-def roofline_entry(fe, launch_s, frames, peak, traffic):
+def roofline_entry(fe, launch_s, frames, peak):
     npix, M = fe.width * fe.height, fe.mapped_pixels
     alg = (5 * npix + M) * frames  # SURVEY section 8d: 4 B lensmap entry + 1 B source (mapped) + 1 B output per pixel
     comp, face_sector_bytes = compulsory_bytes(fe, frames)
@@ -316,24 +321,17 @@ def roofline_entry(fe, launch_s, frames, peak, traffic):
            "algorithmic_bytes_per_launch": int(alg), "launch_us": round(launch_s * 1e6, 2),
            "compulsory_bytes_per_launch": comp, "compulsory_frac": round(comp / launch_s / 1e9 / peak, 4),
            "face_sector_bytes_per_frame": face_sector_bytes}
-    if traffic:
-        # the contract's `traffic`: dram__bytes_read.sum + dram__bytes_write.sum of this workload's launch (one ncu --set full capture)
-        out["traffic"] = int(traffic["dram_bytes_per_launch"])
-        out["traffic_detail"] = traffic
-        out["dram_frac"] = round(traffic["dram_bytes_per_launch"] / launch_s / 1e9 / peak, 4)
-    else:
-        out["traffic"] = None
-        out["dram_frac"] = None
     return out
 
 
-def load_traffic():
-    """measured DRAM bytes per launch (ncu, this round) per workload: profiles/traffic_r2.json, written by
-    scripts/ncu_traffic.py from the committed .ncu-rep summaries"""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic_r2.json")))
-    except Exception:  # noqa: BLE001
-        return {}
+def dump_outputs(torch, d_out, out_dir):
+    """--dump-outputs: the output of the last timed step as float32 .npy files (49 MB at most for a 4K batch)"""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "frame_last.npy"), d_out[-1].cpu().numpy().astype(np.float32))
+    flat = d_out.reshape(-1)
+    pos = np.sort(np.random.default_rng(DUMP_SEED).integers(0, flat.numel(), min(DUMP_SAMPLE, flat.numel())))
+    sample = flat[torch.from_numpy(pos).to(flat.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, "frames_sample.npy"), sample)
 
 
 def main():
@@ -352,7 +350,10 @@ def main():
     ap.add_argument("--gather-mode", default="best", choices=["best", "nccl", "peer_copy", "peer_store"],
                     help="N > 1: which transport's delivered rate is `value` (best = the fastest of the three measured)")
     ap.add_argument("--chunk", type=int, default=4, help="frames per gather chunk (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
 
@@ -388,7 +389,6 @@ def main():
     d_out = torch.zeros((F, H, W), dtype=torch.uint8, device="cuda")
     stream = torch.cuda.current_stream().cuda_stream
     peak, peak_src = hbm_peak()
-    traffic_db = load_traffic()
 
     def barrier():
         if world > 1:
@@ -421,6 +421,8 @@ def main():
     launches = fe.launch_count - launches0
     elapsed = max_over_ranks(e0.elapsed_time(e1) * 1e-3)
     kernel_name = fe.last_kernel
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, d_out, args.dump_outputs)
     # the timed region is a few milliseconds: keep the identical load running so that NVML
     # (which refreshes every few ms) actually sees the clocks this kernel runs at
     t_end = time.time() + 1.0
@@ -458,13 +460,12 @@ def main():
 
     if rank == 0:
         launch_s = elapsed / args.steps
-        roof = roofline_entry(fe, launch_s, F, peak, traffic_db.get(args.workload))
+        roof = roofline_entry(fe, launch_s, F, peak)
         roof.update({"bound": "hbm", "peak": peak, "unit": "GB/s", "peak_source": peak_src,
                      "kernels_per_step": int(launches // max(1, args.steps)),
                      "note": "frac = SURVEY 8(d) algorithmic bytes (5*W*H + M per frame) / CUDA-event launch time / peak; "
                              "compulsory_frac = bytes the launch cannot avoid (sampled 32-byte face sectors + output per frame, "
-                             "tile plan once per launch) / time / peak — computed in this run; dram_frac = DRAM bytes per launch "
-                             "measured by ncu this round (profiles/traffic_r2.json) / this run's launch time / peak"})
+                             "tile plan once per launch) / time / peak — computed in this run"})
         line = {
             "metric": "lens-warp Mpixels/s", "value": round(value, 1), "unit": "Mpixels/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": round(elapsed / args.steps * 1e3, 4), "higher_is_better": True, "scaling": "weak",
@@ -492,7 +493,7 @@ def main():
             line["ms_per_step"] = gather["ms"]
     # ---- the other BASELINE configurations (device-resident; every rank runs them, rank 0 reports) ----
     if world == 1 and not args.no_secondary:
-        secondary = run_secondary(args, torch, bb, fe, peak, traffic_db, stream)
+        secondary = run_secondary(args, torch, bb, fe, peak, stream)
         if rank == 0:
             line["secondary"] = secondary
     if rank == 0:
@@ -614,7 +615,7 @@ SECONDARY = ["1080p-cube-panini170", "4k-cube-quincuncial-rubix", "4k-cube-stere
              "4k-cube-fisheye1", "4k-trism-stereographic"]
 
 
-def run_secondary(args, torch, bb, fe, peak, traffic_db, stream):
+def run_secondary(args, torch, bb, fe, peak, stream):
     """every other BASELINE configuration, device-resident: batched launch (16 frames) and a single cold frame
     (L2 flushed before each launch — the in-engine shape), both fractions of the HBM roofline"""
     rows = []
@@ -632,15 +633,15 @@ def run_secondary(args, torch, bb, fe, peak, traffic_db, stream):
         if name != args.workload:
             t = time_device(torch, fe, d_faces, d_out, F, 10, 3, stream)
             row.update({"us_per_frame": round(t * 1e6 / F, 2), "value": round(W * H * F / t / 1e6, 1), "kernel": fe.last_kernel,
-                        "roofline": roofline_entry(fe, t, F, peak, traffic_db.get(name))})
+                        "roofline": roofline_entry(fe, t, F, peak)})
         tc = time_device(torch, fe, d_faces, d_out, 1, 7, 3, stream, flush=flush)
         row["single_frame_cold"] = {"us": round(tc * 1e6, 2), "value": round(W * H / tc / 1e6, 1),
-                                    "roofline": roofline_entry(fe, tc, 1, peak, None)}
+                                    "roofline": roofline_entry(fe, tc, 1, peak)}
         ts = time_single_frame_stream(torch, fe, d_faces, d_out, stream)
         row["single_frame_stream"] = {"us": round(ts * 1e6, 2), "value": round(W * H / ts / 1e6, 1),
-                                      "roofline": roofline_entry(fe, ts, 1, peak, None),
+                                      "roofline": roofline_entry(fe, ts, 1, peak),
                                       "how": "single-frame launches back to back, each on a different frame of the batch: the faces miss "
-                                             "L2 (F x 25 MB > 126 MB), the tile plan stays resident — the in-engine shape"}
+                                             "L2 (F x 25 MB > 50 MB), the tile plan stays resident — the in-engine shape"}
         rows.append(row)
         del d_faces, d_out
     return rows

@@ -1,13 +1,13 @@
-"""blinky_b200 — B200-native Blinky lens warp (globe faces -> lensmap gather -> screen).
+"""blinky_b200 — H100-native Blinky lens warp (globe faces -> lensmap gather -> screen).
 
 Python host-side mirror of the C ABI in ``include/blinky_b200.h``.  The product
-is the C-ABI shared library ``libblinky_b200.so`` (hand-written sm_100a CUDA
+is the C-ABI shared library ``libblinky_b200.so`` (hand-written sm_90a CUDA
 kernels + the host-side lensmap builder); this module only binds it with
 ``ctypes`` so tests and ``bench.py`` can drive it.  There is NO fallback: if the
 library is missing or a GPU entry point is called on a host-only context the
 call raises.
 
-Reference surface mirrored (all in /root/reference/engine/NQ/fisheye.c):
+Reference surface mirrored (all in the reference's engine/NQ/fisheye.c):
 console commands (:651-665) via :meth:`Fisheye.command`, ``F_WriteConfig``
 (:683-696) via :meth:`Fisheye.write_config`, the lensmap rebuild (:730-743,
 :2367-2397) via :meth:`Fisheye.build_lensmap`, and ``render_lensmap``

@@ -1,4 +1,4 @@
-// C ABI of the B200 lens-warp path (include/blinky_b200.h): a thin veneer over
+// C ABI of the H100 lens-warp path (include/blinky_b200.h): a thin veneer over
 // FisheyeHost (host-side scripts/console/lensmap build) and WarpDevice (CUDA).
 #include "../../include/blinky_b200.h"
 
@@ -124,7 +124,7 @@ int blinky_create(int device, blinky_ctx **out) {
 void blinky_destroy(blinky_ctx *ctx) { delete ctx; }
 
 const char *blinky_last_error(blinky_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
-const char *blinky_version(void) { return "blinky_b200 0.1 (sm_100a)"; }
+const char *blinky_version(void) { return "blinky_b200 0.1 (sm_90a)"; }
 
 void blinky_set_print_callback(blinky_ctx *ctx, blinky_print_fn fn, void *user) { ctx->host.set_print(fn, user); }
 void blinky_set_exec_callback(blinky_ctx *ctx, blinky_exec_fn fn, void *user) { ctx->host.set_exec(fn, user); }
@@ -331,7 +331,7 @@ int blinky_save_globe(blinky_ctx *ctx, const uint8_t *faces_host, const char *di
 #define NEED_DEVICE(ctx)                                                                                              \
     if (!(ctx)->dev)                                                                                                  \
         return set_err(ctx, BLINKY_E_NODEVICE,                                                                        \
-                       "this context has no GPU; the warp runs only as sm_100a CUDA kernels (no CPU fallback)")
+                       "this context has no GPU; the warp runs only as sm_90a CUDA kernels (no CPU fallback)")
 
 int blinky_set_kernel(blinky_ctx *ctx, int variant) {
     NEED_DEVICE(ctx);

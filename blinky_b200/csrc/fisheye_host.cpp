@@ -1,4 +1,4 @@
-// Host side of the B200 lens-warp path.  See fisheye_host.h.
+// Host side of the H100 lens-warp path.  See fisheye_host.h.
 //
 // Numeric contract (what makes the lensmap bit-identical to the reference's):
 // rays are float32 (`vec_t`, engine/include/mathlib.h:30) wherever the

@@ -1,4 +1,4 @@
-// Host side of the B200 lens-warp path: everything the reference's
+// Host side of the H100 lens-warp path: everything the reference's
 // engine/NQ/fisheye.c does BEFORE the per-frame gather — the Lua script
 // environment, globe/lens loading, the console command surface, zoom, the rubix
 // palette and the one-shot lensmap build — with the lensmap produced both in the
@@ -6,7 +6,7 @@
 // form the CUDA kernels read.  No CUDA in this file: it is usable (and tested)
 // on a machine without a GPU.
 //
-// Reference map (all /root/reference/engine/NQ/fisheye.c): state structs
+// Reference map (all the reference's engine/NQ/fisheye.c): state structs
 // :306-528, F_Init :642-676, console commands :916-1176, converters :1184-1214,
 // init_lua :1222-1265, zoom :1273-1386, Lua bridge :1494-1651, loaders
 // :1659-1913, setters :1922-2013, getters :2023-2066, builders :2084-2397.

@@ -290,7 +290,7 @@ bool LensDevice::compile(const std::string &lens_source, bool forward, std::vect
         return false;
     }
     // --fmad=false: the host computes with -ffp-contract=off; parity needs unfused arithmetic
-    const char *opts[] = {"--gpu-architecture=sm_100a", "--fmad=false", "--std=c++17", "--prec-div=true", "--prec-sqrt=true", "--ftz=false", "--disable-warnings"};
+    const char *opts[] = {"--gpu-architecture=sm_90a", "--fmad=false", "--std=c++17", "--prec-div=true", "--prec-sqrt=true", "--ftz=false", "--disable-warnings"};
     rc = n.CompileProgram(prog, static_cast<int>(sizeof(opts) / sizeof(opts[0])), opts);
     size_t logsz = 0;
     n.GetProgramLogSize(prog, &logsz);

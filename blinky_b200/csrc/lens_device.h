@@ -1,8 +1,8 @@
 // Device-side lensmap construction (SURVEY section 8f rank 1): the reference evaluates the
 // lens script once per screen pixel inside create_lensmap_inverse()
-// (/root/reference/engine/NQ/fisheye.c:2084-2124, ~1 us .. 10 us per pixel through the Lua
+// (the reference's engine/NQ/fisheye.c:2084-2124, ~1 us .. 10 us per pixel through the Lua
 // VM).  Here the script's lens_inverse is translated to CUDA C++ (lua_transpile.h),
-// compiled for sm_100a with NVRTC at lens-load time, and evaluated for all W*H pixels by
+// compiled for sm_90a with NVRTC at lens-load time, and evaluated for all W*H pixels by
 // one kernel; the ray -> plate -> texel -> rubix tint tail of the pixel pipeline
 // (fisheye.c:2023-2066, 1922-2013) runs in the same kernel with the host's exact float /
 // double operation order.

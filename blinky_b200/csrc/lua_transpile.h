@@ -6,7 +6,7 @@
 // upvalues and the globals it reads as they are RIGHT NOW).  Output: target-neutral
 // C++ source for the function and everything it calls, against the small prelude
 // returned by transpile_prelude().  The same source is compiled
-//   * by NVRTC for sm_100a (product: the lensmap is evaluated on the GPU), and
+//   * by NVRTC for sm_90a (product: the lensmap is evaluated on the GPU), and
 //   * by g++ in the CPU test-suite, where it must reproduce the interpreter bit for
 //     bit (same libm) — that is how the transpiler itself is pinned.
 //

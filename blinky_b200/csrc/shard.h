@@ -1,6 +1,6 @@
 // Sharded batches: independent frames split over N GPUs (one process per GPU), finished frames
 // gathered on rank 0 — the reference topology's last step is "frames reach the one display"
-// (/root/reference/engine/NQ/fisheye.c:802-803 writes vid.buffer).  The gather of chunk k overlaps the
+// (the reference's engine/NQ/fisheye.c:802-803 writes vid.buffer).  The gather of chunk k overlaps the
 // warp of chunk k+1 (compute stream + communication stream per rank).
 //   NCCL        ncclSend/ncclRecv of finished chunks (the north-star's "NCCL only for the final gather")
 //   PEER_COPY   copy engines push finished chunks into rank 0's buffer through CUDA-IPC peer memory (NVLink)

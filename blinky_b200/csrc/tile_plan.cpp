@@ -72,7 +72,7 @@ void plan_tile_row(const uint32_t *packed, int width, int height, int platesize,
         uint32_t bw = 0, bh = 0;
         if (box) {
             // TMA faults ("illegal instruction") unless the innermost coordinate is a multiple of
-            // 16 bytes (measured on B200, scripts/tma_probe.cu): start the box on a 16-texel
+            // 16 bytes (scripts/tma_probe.cu): start the box on a 16-texel
             // boundary.  The row coordinate is unconstrained.
             minx &= ~15u;
             bw = ((maxx - minx + 1) + 15) / 16 * 16;

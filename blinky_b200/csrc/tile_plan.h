@@ -15,7 +15,7 @@
 // and have fixed sizes, so a tile's block address is a function of its index alone.
 //
 // This replaces nothing in the reference (its lensmap is a flat array of pointers,
-// /root/reference/engine/NQ/fisheye.c:427-430); it is the B200 data layout for the same information.
+// the reference's engine/NQ/fisheye.c:427-430); it is the H100 data layout for the same information.
 #pragma once
 
 #include <cstdint>

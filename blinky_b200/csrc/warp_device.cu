@@ -1,6 +1,6 @@
-// Device side of the B200 lens-warp path — kernels, resident state, frame pipeline.
+// Device side of the H100 lens-warp path — kernels, resident state, frame pipeline.
 //
-// The reference's hot loop (/root/reference/engine/NQ/fisheye.c:2406-2424) is,
+// The reference's hot loop (the reference's engine/NQ/fisheye.c:2406-2424) is,
 // per screen pixel: load an 8-byte pointer, load the source byte through it,
 // optionally map it through a 256-entry tint LUT chosen by a second per-pixel
 // byte, store one byte.  Here one packed 32-bit lensmap entry per pixel
@@ -9,7 +9,7 @@
 // read-only path, and four output pixels are written per 32-bit store so that
 // every warp-level store instruction covers one full 128-byte line.
 //
-// sm_100a only.  HBM-bound byte work: no tensor cores on purpose.
+// sm_90a only.  HBM-bound byte work: no tensor cores on purpose.
 #include "warp_device.h"
 
 #include <cuda.h>  // CUtensorMap types only; the driver entry point is fetched at run time
@@ -181,16 +181,8 @@ __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams 
 //     its sequence as soon as the consumed bytes sit in registers, and writes the words with
 //     streaming stores.
 // There is no producer warp, no cross-warp barrier, no per-pixel entry traffic per frame, and no
-// global load on a scoreboard in the frame loop.  History, all measured (profiles/r2_c1*_sweep.jsonl):
-// round 1's kernel was bound by the serial per-item work of its producer thread; the first
-// self-feeding version spent 36 of 213 instructions per frame copying registers that an
-// uninitialised array in the GATHER path kept live around the unit loop, and the GATHER path's 130
-// registers capped the kernel at 160 registers per thread.  Now the frame loop is ~140
-// instructions at 100 registers.  What is left is not one bottleneck: with the 4K panini batch at
-// 4.4 us per frame (ring warps alone), removing the stores gives 3.2, removing the box loads 3.4,
-// both 2.6, conflict-free shared loads 4.4, 128-byte instead of 32-byte store segments 4.3 — DRAM
-// time (2.7 us for the 17.5 MB a frame moves) and issue time overlap only partly with 12 warps,
-// and more warps or deeper rings lose as much L2 locality as they gain latency hiding.
+// global load on a scoreboard in the frame loop.  More warps or deeper rings lose as much L2
+// locality on the halo sectors neighbouring tiles share as they gain latency hiding.
 // EMPTY tiles copy the background.  GATHER tiles (plate seams, singular points, boxes too large to
 // stage) are not the ring warps': see gather_item.
 // --------------------------------------------------------------------------
@@ -245,7 +237,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "r"(parity)
         : "memory");
 }
-// NB (measured on B200, scripts/tma_probe.cu): the innermost coordinate must be a
+// NB (scripts/tma_probe.cu): the innermost coordinate must be a
 // multiple of 16 bytes or the TMA unit raises "illegal instruction".
 __device__ __forceinline__ void tma_load_box(uint32_t smem_dst, const CUtensorMap *tmap, int x, int y, int plate, int frame, uint32_t bar) {
     asm volatile(
@@ -292,7 +284,7 @@ __device__ __forceinline__ uint32_t stage_dep(const uint32_t (&w)[8], uint32_t z
 // One TMA descriptor per box shape of the plan, passed in the kernel's parameter block
 // (__grid_constant__): descriptors in param space need no tensormap-proxy fence, unlike a table in
 // global memory written by cudaMemcpy (a per-unit fence there drains every outstanding load of the
-// warp and invalidates the SM's descriptor cache: measured 6 us per unit).
+// warp and invalidates the SM's descriptor cache).
 struct RingTmaps {
     CUtensorMap m[kMaxShapes];
 };
@@ -344,8 +336,7 @@ __device__ __forceinline__ void st_lab_u32x8(const uint64_t (&a)[8], const uint3
 // bound by load latency, so they get plain parallelism: one extra one-warp CTA per (tile, 8 of its rows, 4
 // frames) behind the ring CTAs in the same grid.  The launch leaves shared memory for two of them per SM next
 // to the resident ring warps, so this work runs beside the ring warps from the start and fills the slots they
-// vacate at the end — as a separate kernel behind the ring kernel it cost 0.7 us per 4K panini frame for 3.5 %
-// of the tiles.
+// vacate at the end.
 constexpr int kGatherRows = 8, kGatherFrames = 4;
 
 template <bool RUBIX, bool RGBA>
@@ -908,9 +899,9 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) throw std::runtime_error(std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e));
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on sm_90 only
         char buf[256];
-        snprintf(buf, sizeof buf, "blinky_b200 needs an sm_100 (B200) device; device %d is sm_%d%d (%s)", device, prop.major,
+        snprintf(buf, sizeof buf, "blinky_b200 needs an sm_90 (H100) device; device %d is sm_%d%d (%s)", device, prop.major,
                  prop.minor, prop.name);
         throw std::runtime_error(buf);
     }
@@ -1143,13 +1134,13 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
 // 116 with the rubix overlay).  How many ring warps are resident is decided in launch_ring.
 template <bool RUBIX>
 constexpr int ring_warps() { return 16; }
-// Resident ring warps per SM by default (BLINKY_RING_CTAS): measured on the 4K panini batch 12 / 14 / 16 warps give
-// 4.39 / 4.4 / 4.50 us per frame alone and 4.75 / 4.87 / 5.09 with the gather CTAs beside them — more warps only
-// spread the faces' L2 footprint; the registers left over go to the gather CTAs.
+// Resident ring warps per SM by default (BLINKY_RING_CTAS): measured on the 4K panini batch (bench.py, H100 80GB HBM3
+// at a 400 W power limit) 8 / 10 / 12 / 14 / 16 warps give 578 / 578 / 657 / 652 / 653 Gpixel/s — beyond 12, more
+// warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
 // GATHER tiles ride in the ring kernel's launch (gather_item) while they are at most this share of the plan; beyond
 // it (minifying lenses: thousands of GATHER tiles) the 256-thread gather kernel K3 in front of the ring kernel is
-// faster than tens of thousands of one-warp CTAs (measured: quincuncial 6.8 % -> 7.9 us serial vs 9.7 us merged).
+// faster than tens of thousands of one-warp CTAs.
 constexpr uint32_t kMergedGatherPercent = 5;
 
 template <bool RUBIX, bool RGBA>
@@ -1222,7 +1213,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     int want = std::min(kRingWarpsDefault, rubix ? ring_warps<true>() : ring_warps<false>());
     if (ring_ctas_cap_ > 0) want = std::min(ring_ctas_cap_, rubix ? ring_warps<true>() : ring_warps<false>());
     // ring size: twice the plan's largest box plus an entry block (two boxes of any size and the next unit's entries in
-    // flight; measured on the 4K panini plan, largest box 6.4 KB: 8 KB ring 5.2 us per frame, 12 KB 4.7), as far as `want`
+    // flight), as far as `want`
     // resident warps — plus two gather CTAs, which
     // carry the same allocation, when GATHER tiles ride along — leave room in the SM's shared memory
     uint32_t ring_bytes = 0;
@@ -1239,9 +1230,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
         return false;
     }
     p.ring_bytes = ring_bytes;
-    // items in flight per warp: two boxes and (at unit boundaries) the next entry block.  Measured: 2 / 3 / 4 the same on
-    // batches, and single-frame launches do not gain from running further ahead either (13.2 / 13.6 / 14.0 us with 2 / 4
-    // / 6) — they are bound by the ~480 instructions a unit costs, not by its loads (BLINKY_RING_BOXES overrides)
+    // items in flight per warp: two boxes and (at unit boundaries) the next entry block (BLINKY_RING_BOXES overrides)
     p.max_inflight = static_cast<uint32_t>(std::max(1, std::min(ring_boxes_ > 0 ? ring_boxes_ : 3, kRingBoxes)));
     const size_t smem = static_cast<size_t>(ring_bytes) + fixed;
     if (ring_ctas_per_sm_[vi] == 0 || ring_smem_[vi] != smem) {

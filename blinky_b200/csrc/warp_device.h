@@ -1,9 +1,9 @@
-// Device side of the B200 lens-warp path: resident lensmap / LUTs, the warp
+// Device side of the H100 lens-warp path: resident lensmap / LUTs, the warp
 // kernels and the host<->device frame pipeline.  CUDA types are kept out of
 // this header so that plain C++ translation units can include it.
 //
 // Replaces the reference's per-frame hot loop, render_lensmap()
-// (/root/reference/engine/NQ/fisheye.c:2406-2424).
+// (the reference's engine/NQ/fisheye.c:2406-2424).
 #pragma once
 
 #include <cstddef>
@@ -70,7 +70,7 @@ private:
     void finalize_slot(Slot &s);
 
     int device_ = 0;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     void *stream_ = nullptr;  // cudaStream_t
     bool upload_by_kernel_ = false, out_by_kernel_ = false;  // warp_host variants (BLINKY_E2E_UPLOAD / BLINKY_E2E_OUT)
     bool batch_copies_ = true;   // plate rectangles of a frame in one cudaMemcpy3DBatchAsync (BLINKY_E2E_BATCH=0: one 2-D copy each)

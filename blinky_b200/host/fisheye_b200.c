@@ -8,7 +8,7 @@
  * libblinky_b200.so (include/blinky_b200.h):
  *
  *   scripts / console / zoom / lensmap build  -> blinky_command, blinky_build_lensmap (host)
- *   render_lensmap() (fisheye.c:2406-2424)    -> blinky_warp_host (sm_100a CUDA kernels)
+ *   render_lensmap() (fisheye.c:2406-2424)    -> blinky_warp_host (sm_90a CUDA kernels)
  *
  * Build: compile this file instead of NQ/fisheye.c (engine/Makefile:645) with
  * the engine's include paths plus -I<repo>/include, and add -lblinky_b200 where

@@ -1,12 +1,12 @@
-/* blinky_b200 — C ABI of the B200-native Blinky lens-warp path.
+/* blinky_b200 — C ABI of the H100-native Blinky lens-warp path.
  *
  * This is the thin boundary a C host (TyrQuake's fisheye seams, or a headless
  * harness) calls into.  It replaces, for the lens-warp path only, what the
  * reference keeps inside one statically linked translation unit,
- * /root/reference/engine/NQ/fisheye.c (public surface: engine/include/fisheye.h:4-9).
+ * the reference's engine/NQ/fisheye.c (public surface: engine/include/fisheye.h:4-9).
  * Plain pointers and sizes only; no C++ or torch types.
  *
- * Mapping to the reference (file:line are in /root/reference/engine/NQ/fisheye.c):
+ * Mapping to the reference (file:line are in the reference's engine/NQ/fisheye.c):
  *
  *   blinky_create / blinky_destroy      F_Init :642-676 / F_Shutdown :678-681 (state + Lua VM)
  *   blinky_set_palette                  create_palmap :857-908 (from host_basepal)
@@ -122,7 +122,7 @@ int blinky_set_rubixgrid(blinky_ctx *ctx, int numcells, double cell_size, double
  *   threads  > 1  rows are split over that many cloned script states (requires
  *                 lens_inverse to be a pure function of x,y — true for every shipped lens);
  *   threads  < 0  as above with every CPU the process may use;
- *   threads == 0  GPU build: the lens function is translated to CUDA, compiled for sm_100a
+ *   threads == 0  GPU build: the lens function is translated to CUDA, compiled for sm_90a
  *                 with NVRTC and evaluated by one kernel — lens_inverse for every screen
  *                 pixel, or, for forward-only lenses, lens_forward for every plate grid point
  *                 followed by the quad rasterisation in the reference's writer order.

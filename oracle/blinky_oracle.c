@@ -1,6 +1,6 @@
 /* TEST INFRASTRUCTURE — parity oracle, not part of the product.  See blinky_oracle.h.
  *
- * Literal plain-C restatement of /root/reference/engine/NQ/fisheye.c for the
+ * Literal plain-C restatement of the reference's engine/NQ/fisheye.c for the
  * lens-warp path.  Float32/float64 truncation points are reproduced exactly:
  * `vec_t` is float (engine/include/mathlib.h:30), x86-64 evaluates float
  * expressions in float (FLT_EVAL_METHOD 0), and this file is compiled with

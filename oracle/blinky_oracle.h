@@ -1,7 +1,7 @@
 /* TEST INFRASTRUCTURE — parity oracle, not part of the product.
  *
  * Plain-C restatement of the reference's lens-warp path
- * (/root/reference/engine/NQ/fisheye.c), one function per reference function,
+ * (the reference's engine/NQ/fisheye.c), one function per reference function,
  * each citing the lines it follows.  Only tests/, __graft_entry__.smoke() and
  * bench.py's cpu_baseline / --impl reference legs may load this library; the
  * product (blinky_b200/) never links, imports or executes anything in oracle/.
@@ -9,13 +9,13 @@
  * Parity status: PINNED.  The reference has no tests or golden vectors of its
  * own (SURVEY.md section 4), so this restatement is pinned against the
  * reference ITSELF: oracle/_ref/libblinky_ref.so is the unmodified fisheye.c
- * compiled from /root/reference, and tests/test_oracle_vs_ref.py requires
+ * compiled from the original project, and tests/test_oracle_vs_ref.py requires
  * bit-identical lensmaps, tint maps, palette LUTs and rendered frames from
  * both on every shipped globe x lens combination; tests/golden/ holds vectors
  * generated from _ref by tests/golden/make_golden.py for boxes without
- * /root/reference.
+ * the original project.
  *
- * The one part of the path that is NOT in /root/reference is the Lua 5.2 VM
+ * The one part of the path that is NOT in the original project is the Lua 5.2 VM
  * (external liblua, engine/Makefile:834-841, BUILDING.md:19-27; no pinned patch
  * version, absent from the image).  Lens functions enter this oracle as C
  * callbacks; oracle_lenses.c holds literal C transcriptions of the BASELINE

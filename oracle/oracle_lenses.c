@@ -1,7 +1,7 @@
 /* TEST INFRASTRUCTURE — parity oracle, not part of the product.  See blinky_oracle.h.
  *
  * Literal C transcriptions of shipped Blinky lens and globe scripts
- * (/root/reference/game/lua-scripts/{lenses,globes}/<name>.lua).  A Lua 5.2 VM
+ * (the reference's game/lua-scripts/{lenses,globes}/<name>.lua).  A Lua 5.2 VM
  * executes those scripts as IEEE-double operations in source order with
  * libm for math.*; these functions perform the same operations in the same
  * order, so a correct Lua evaluator must reproduce their results BIT FOR BIT.

@@ -5,14 +5,17 @@ legs import this module; nothing under blinky_b200/ does.
 
 * :class:`RefOracle`   — oracle/_ref/libblinky_ref.so: the UNMODIFIED reference
   engine/NQ/fisheye.c compiled headless (needs a prebuilt .so; building it needs
-  /root/reference).  One per process (the reference keeps its state in statics).
+  the original project).  One per process (the reference keeps its state in statics).
 * :class:`Restatement` — oracle/liboracle.so: the plain-C restatement
   (blinky_oracle.c) + C transcriptions of shipped lenses/globes (oracle_lenses.c).
 """
 from __future__ import annotations
 
+import atexit
 import ctypes
 import os
+import shutil
+import tempfile
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_void_p
 
 import numpy as np
@@ -21,7 +24,17 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REF_SO = os.path.join(HERE, "_ref", "libblinky_ref.so")
 REF_FAST_SO = os.path.join(HERE, "_ref", "libblinky_ref_fastmath.so")
 RESTATE_SO = os.path.join(HERE, "liboracle.so")
-REFERENCE_GAME_DIR = "/root/reference/game"
+
+
+def _short_basedir(basedir: str) -> bytes:
+    """The reference formats script paths into a char[100] (fisheye.c:1665, 1758), which a checkout
+    under a long path overflows: it is handed a short link to `basedir` instead."""
+    tmp = tempfile.mkdtemp(prefix="blinky")
+    atexit.register(shutil.rmtree, tmp, True)
+    link = os.path.join(tmp, "b")
+    os.symlink(os.path.abspath(basedir), link)
+    return link.encode()
+
 
 ZOOM = {"f_fov": 1, "f_vfov": 2, "f_cover": 3, "f_contain": 4}
 
@@ -60,13 +73,13 @@ class RefOracle:
         L.ref_lens_inverse.argtypes = [c_double, c_double, c_void_p]
         L.ref_lens_forward.argtypes = [c_void_p, POINTER(c_double), POINTER(c_double)]
         self.palette = np.ascontiguousarray(palette, np.uint8).reshape(768)
-        rc = L.ref_init(basedir.encode(), _p(self.palette))
+        rc = L.ref_init(_short_basedir(basedir), _p(self.palette))
         if rc != 0:
             raise RuntimeError("ref_init failed (already initialised in this process?)")
         self.W = self.H = 0
 
     def set_basedir(self, basedir: str):
-        self.lib.ref_set_basedir(basedir.encode())
+        self.lib.ref_set_basedir(_short_basedir(basedir))
 
     def command(self, text: str):
         self.lib.ref_command(text.encode())

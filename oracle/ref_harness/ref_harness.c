@@ -2,7 +2,7 @@
  *
  * Headless harness around the UNMODIFIED reference fisheye layer.  The
  * reference source is pulled in where it lies (`#include "fisheye.c"` resolves
- * through -I/root/reference/engine/NQ, see ../Makefile); nothing is copied into
+ * through -Ithe reference's engine/NQ, see ../Makefile); nothing is copied into
  * this repository.  Including it in this translation unit gives the harness
  * access to the file-static `lens`, `globe`, `zoom`, `rubix` structures
  * (engine/NQ/fisheye.c:334-528) so the lensmap can be exported as indices.

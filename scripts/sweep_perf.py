@@ -1,4 +1,4 @@
-"""Developer sweep (run under gpurun): one process, many (environment knob, workload) combinations of the
+"""Developer sweep (run on the GPU machine): one process, many (environment knob, workload) combinations of the
 device-resident warp; prints one line per combination.  Knobs are read when the context is created /
 the lensmap is planned, so each combination gets a fresh context."""
 import json

@@ -1,7 +1,7 @@
 // Lab: how fast can one SM be FED with small source boxes?  Measures, per box shape, the rate at which
 // per-warp rings of TMA tensor loads (mode 0), TMA loads + a 2 KB bulk copy (mode 1) or warp-issued
 // 16-byte cp.async copies (mode 2) complete, with nothing consuming the data.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/tma_lab.bin scripts/tma_lab.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/tma_lab.bin scripts/tma_lab.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>

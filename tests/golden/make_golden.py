@@ -1,6 +1,6 @@
 """Generates the committed golden vectors from the COMPILED REFERENCE (oracle/_ref,
-i.e. the unmodified /root/reference/engine/NQ/fisheye.c) driving the repo's own
-script set.  Run here (needs oracle/_ref built):
+i.e. the unmodified engine/NQ/fisheye.c of the original project) driving the repo's own
+script set.  Needs oracle/_ref, built by build() with BLINKY_REFERENCE set:
 
     python tests/golden/make_golden.py
 
@@ -15,7 +15,7 @@ Outputs (all under tests/golden/):
   palmaps.npz          the six rubix LUTs for the seeded palette
   config.txt           F_WriteConfig output
 
-The GPU box has no /root/reference: tests there compare against these files.
+The tests compare against these files; they do not need the reference.
 """
 import hashlib
 import json

@@ -30,8 +30,8 @@ def test_library_is_in_tree_and_native(bb):
     assert os.path.dirname(bb.LIB_PATH) == os.path.join(ROOT, "blinky_b200")
     data = open(bb.LIB_PATH, "rb").read()
     assert data[:4] == b"\x7fELF"
-    # the kernels are really in there, compiled for sm_100a
-    assert b"warp_gather_kernel" in data and b"sm_100a" in data
+    # the kernels are really in there, compiled for sm_90a
+    assert b"warp_gather_kernel" in data and b"sm_90a" in data
 
 
 def test_host_only_context_refuses_the_hot_path(bb, host):

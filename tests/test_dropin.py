@@ -12,7 +12,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "oracle", "_ref", "libdropin_b200.so")
 
-needs_so = pytest.mark.skipif(not os.path.exists(SO), reason="oracle/_ref/libdropin_b200.so not built (needs /root/reference headers)")
+needs_so = pytest.mark.skipif(not os.path.exists(SO), reason="oracle/_ref/libdropin_b200.so not built (needs the original engine's headers: BLINKY_REFERENCE)")
 
 
 @needs_so

@@ -3,7 +3,7 @@ lensmap builder built on it (SURVEY section 8f rank 1).
 
 CPU suite: the translated lens is compiled with g++ (same libm as the interpreter) and must
 reproduce the interpreter's lens_inverse BIT FOR BIT; that pins the translator.  The CUDA
-flavour of the same source must compile for sm_100a with NVRTC (no GPU needed for that).
+flavour of the same source must compile for sm_90a with NVRTC (no GPU needed for that).
 
 GPU suite: blinky_build_lensmap(threads=0) evaluates the lens on the GPU; the finished
 lensmap must equal the all-interpreter build for every translatable lens."""
@@ -177,7 +177,7 @@ def test_script_level_state_is_per_pixel(host, tmp_path):
         assert struct.pack("3d", *want) == struct.pack("3d", out[0], out[1], out[2])
 
 
-def test_cuda_flavour_of_every_lens_compiles_for_sm100a(bb, host):
+def test_cuda_flavour_of_every_lens_compiles_for_sm90a(bb, host):
     """NVRTC cross-compiles without a GPU; a missing libnvrtc is a skip, a compile error is a failure"""
     host.command("f_globe cube")
     compiled = 0
