@@ -516,17 +516,21 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
         const uint32_t n = c_entry ? static_cast<uint32_t>(kBoxBlockBytes) : c_bytes;
         if (inflight == 0) ipos = cpos = 0;   // (an empty ring restarts at the front: keeps "everything in flight lies behind cpos" true)
         if (ipos + n > R) ipos = 0;
-#ifdef BLINKY_LAB
-        if (lane == 0 && (c_entry || !(p.lab & 16u))) {
-#else
         if (lane == 0) {
-#endif
             const uint32_t bar = bars + 8 * is;
+#ifdef BLINKY_LAB
+            // no box load: the barrier still completes its phase (an arrive without bytes), so the slot's parity
+            // bookkeeping stays right for the entry blocks that use the slot later
+            if (!c_entry && (p.lab & 16u)) {
+                mbar_expect_tx(bar, 0);
+            } else {
+                mbar_expect_tx(bar, n);
+                if (c_entry) bulk_load(ring + ipos + dep, p.entries + static_cast<size_t>(c_tile) * kBoxBlockBytes, n, bar);
+                else tma_load_box(ring + ipos + dep, reinterpret_cast<const CUtensorMap *>(c_tmap), c_bx, c_by, c_plate, (p.lab & 8u) ? 0 : static_cast<int>(c_frame), bar);
+            }
+#else
             mbar_expect_tx(bar, n);
             if (c_entry) bulk_load(ring + ipos + dep, p.entries + static_cast<size_t>(c_tile) * kBoxBlockBytes, n, bar);
-#ifdef BLINKY_LAB
-            else tma_load_box(ring + ipos + dep, reinterpret_cast<const CUtensorMap *>(c_tmap), c_bx, c_by, c_plate, (p.lab & 8u) ? 0 : static_cast<int>(c_frame), bar);
-#else
             else tma_load_box(ring + ipos + dep, reinterpret_cast<const CUtensorMap *>(c_tmap), c_bx, c_by, c_plate, static_cast<int>(c_frame), bar);
 #endif
         }
@@ -583,7 +587,7 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
 #ifdef BLINKY_LAB
             if (p.lab & 2u) {
 #pragma unroll
-                for (int i = 0; i < 32; ++i) off[i] = (lane * 4u + (i & 3) + (i >> 2) * 128u) & 1023u;
+                for (int i = 0; i < 32; ++i) off[i] = ((lane * 4u + (i & 3) + (i >> 2) * 128u) & 1023u) % a_bytes;   // inside the box
             }
 #endif
             // the block's bytes may be overwritten once they sit in registers (same reasoning as stage_dep)
@@ -615,9 +619,6 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
 
             // one frame: wait for its box, 32 byte loads from shared memory, pack, hand the stage on
             auto gather_frame = [&](uint32_t (&w)[8]) {
-#ifdef BLINKY_LAB
-                if (!(p.lab & 16u))
-#endif
                 mbar_wait(bars + 8 * cs, (phases >> cs) & 1u);
                 if (cpos + a_bytes > R) cpos = 0;
                 const uint32_t base = ring + cpos;
@@ -739,9 +740,9 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
 }
 
 // --------------------------------------------------------------------------
-// K3: the GATHER tiles of plans in which they are many (more than kMergedGatherPercent of the tiles:
-// minifying lenses, where a tile's texels do not fit a box), launched in front of the ring kernel; with
-// few GATHER tiles they ride in the ring kernel's launch instead (gather_item).  Those tiles are bound
+// K3: the GATHER tiles (plate seams, singular points; thousands of them with minifying lenses, where a tile's
+// texels do not fit a box), launched in front of the ring kernel; in short launches with few GATHER items
+// they ride in the ring kernel's launch instead (gather_item).  Those tiles are bound
 // by global-load latency and, at 32-byte sectors scattered over DRAM pages, by DRAM itself (ncu, 4K fisheye1:
 // 4.6 TB/s = 70 % of the measured copy peak with about one useful byte in 20 fetched); they get plain parallelism: grid = (tiles, groups of 4 frames), 256 threads, a warp owns 4 tile rows and lane l is
 // column l (one warp-level load = 32 consecutive screen pixels of one row).  The tile's entries are
@@ -1138,10 +1139,6 @@ constexpr int ring_warps() { return 16; }
 // at a 400 W power limit) 8 / 10 / 12 / 14 / 16 warps give 578 / 578 / 657 / 652 / 653 Gpixel/s — beyond 12, more
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
-// GATHER tiles ride in the ring kernel's launch (gather_item) while they are at most this share of the plan; beyond
-// it (minifying lenses: thousands of GATHER tiles) the 256-thread gather kernel K3 in front of the ring kernel is
-// faster than tens of thousands of one-warp CTAs.
-constexpr uint32_t kMergedGatherPercent = 5;
 
 template <bool RUBIX, bool RGBA>
 static cudaError_t ring_config(size_t smem, int *ctas_per_sm) {
@@ -1206,10 +1203,15 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     // largest box would not fit such a ring.
     const size_t fixed = kRingBarBytes + (rubix ? 6 * 256 : 0) + (rgba ? 1024 : 0);
     const uint32_t max_box = std::max<uint32_t>(static_cast<uint32_t>(stage_bytes_ > 0 ? stage_bytes_ : 128), kBoxBlockBytes);  // largest ring item
-    // (few gather items in absolute terms — short launches — also ride along: a second kernel launch costs more than they do)
+    // GATHER tiles ride in the ring kernel's launch (gather_item) only in launches of at most kMergedFramesMax frames
+    // with few GATHER items, where a second kernel launch costs more than they do; otherwise the gather kernel K3 goes
+    // in front.  Measured on the H100 (80GB HBM3, 400 W): riding along is 2-20 % faster for 1-8 frames of 4K panini and
+    // trism, but with 16 frames K3 in front is faster by 1.5-10 % (panini, stereographic, trism, 1080p panini; the
+    // 1080p batch prefers K3 from 8 frames on, by 10 %, and keeps riding along there).
+    constexpr int kMergedFramesMax = 8;
     const uint32_t all_gather_items = ngather_tiles_ * (kTileH / kGatherRows) * static_cast<uint32_t>((nframes + kGatherFrames - 1) / kGatherFrames);
-    const bool merged_gather = !serial_gather_ && ngather_tiles_ > 0 &&
-                               (ngather_tiles_ * 100u <= ntiles_ * kMergedGatherPercent || all_gather_items <= static_cast<uint32_t>(merged_items_max_));
+    const bool merged_gather = !serial_gather_ && ngather_tiles_ > 0 && nframes <= kMergedFramesMax &&
+                               all_gather_items <= static_cast<uint32_t>(merged_items_max_);
     int want = std::min(kRingWarpsDefault, rubix ? ring_warps<true>() : ring_warps<false>());
     if (ring_ctas_cap_ > 0) want = std::min(ring_ctas_cap_, rubix ? ring_warps<true>() : ring_warps<false>());
     // ring size: twice the plan's largest box plus an entry block (two boxes of any size and the next unit's entries in
@@ -1246,15 +1248,18 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     }
     int ctas = std::min(ring_ctas_per_sm_[vi], want);
     uint32_t grid = static_cast<uint32_t>(sm_count_ * ctas);
-    // frames per unit: a unit pays a fixed cost (entry unpack, ring refill across the boundary: ~0.8 frame
+    // frames per unit: a unit pays a fixed cost (entry unpack, ring refill across the boundary: ~kUnitCost frame
     // times) and the launch ends with a tail of about one unit; pick the chunk that minimises
-    // units-per-warp x (chunk + 0.8) + chunk
+    // units-per-warp x (chunk + kUnitCost) + chunk.  kUnitCost = 2 fits the H100 (80GB HBM3, 400 W): 16-frame units
+    // beat 8-frame ones by 4-7 % on the 4K batches of ~7900 ring tiles (panini, stereographic, quincuncial, trism),
+    // and lose 1-3 % on those of ~5000 (hammer, fisheye1), which keep 8.
+    constexpr double kUnitCost = 2.0;
     uint32_t fchunk = fchunk_ > 0 ? static_cast<uint32_t>(fchunk_) : 1;
     if (fchunk_ <= 0) {
         double best = 0;
         for (uint32_t c = 1; c <= std::min<uint32_t>(p.nframes, 16u); ++c) {
             const double units = static_cast<double>(ring_tiles) * ((p.nframes + c - 1) / c);
-            const double cost = std::max(1.0, units / grid) * (c + 0.8) + c;
+            const double cost = std::max(1.0, units / grid) * (c + kUnitCost) + c;
             if (c == 1 || cost < best) best = cost, fchunk = c;
         }
     }

@@ -110,7 +110,7 @@ private:
     int l2_promotion_ = 0;               // CUtensorMapL2promotion of the box descriptors (BLINKY_L2_PROMOTION)
     bool serial_gather_ = false;         // BLINKY_SERIAL_GATHER=1: GATHER tiles in their own kernel instead of as extra CTAs of the ring kernel's launch
     int ring_bytes_override_ = 0, ring_ctas_cap_ = 0, fchunk_ = 0;  // tuning overrides (BLINKY_RING_BYTES / _CTAS, BLINKY_FCHUNK); 0 = automatic
-    int merged_items_max_ = 4096;        // gather items up to which GATHER tiles ride in the ring kernel's launch whatever their share (BLINKY_MERGED_ITEMS)
+    int merged_items_max_ = 4096;        // gather items up to which GATHER tiles ride in the ring kernel's launch of <= 8 frames (BLINKY_MERGED_ITEMS)
     int ring_boxes_ = 0;                 // boxes a warp keeps in flight at most (BLINKY_RING_BOXES)
     size_t smem_per_sm_ = 233472;
     std::vector<uint16_t> shapes_;
