@@ -138,13 +138,12 @@ def load_library() -> ctypes.CDLL:
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("BLINKY_B200_LIB", LIB_PATH)  # (developer builds: make lab)
-    if not os.path.exists(path):
+    if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build the CUDA extension first (make -C blinky_b200, or "
             f"__graft_entry__.build()).  blinky_b200 has no CPU fallback for the warp."
         )
-    lib = ctypes.CDLL(path)
+    lib = ctypes.CDLL(LIB_PATH)
     for name, restype, argtypes in _SIGNATURES:
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.restype = restype

@@ -210,10 +210,6 @@ struct RingParams {
     uint32_t ring_grid;     // CTAs [0, ring_grid) are ring warps, the CTAs behind them take one gather item each
     int width, height;
     uint32_t zero;  // always 0, but only the host knows: see stage_dep()
-    uint32_t lab_bytes;  // (lab bit 5) bytes of box shape 0
-    uint32_t lab;   // BLINKY_LAB builds only (make lab): bit 0 no stores, bit 1 bank-conflict-free gather offsets,
-                    // bit 2 each warp-level store covers 128 contiguous bytes, bit 3 every frame reads frame 0's
-                    // faces (L2-resident), bit 4 no box loads at all — wrong pixels, timing experiments
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -314,22 +310,6 @@ __device__ __forceinline__ void st_stream_u32x8(const uint64_t (&a)[8], const ui
         : "memory");
 }
 
-#ifdef BLINKY_LAB
-#define LAB_ST8(POL)                                                                                                        \
-    asm volatile("st.global" POL ".u32 [%0], %8;\n\tst.global" POL ".u32 [%1], %9;\n\tst.global" POL ".u32 [%2], %10;\n\t"    \
-                 "st.global" POL ".u32 [%3], %11;\n\tst.global" POL ".u32 [%4], %12;\n\tst.global" POL ".u32 [%5], %13;\n\t"  \
-                 "st.global" POL ".u32 [%6], %14;\n\tst.global" POL ".u32 [%7], %15;"                                        \
-                 ::"l"(a[0]), "l"(a[1]), "l"(a[2]), "l"(a[3]), "l"(a[4]), "l"(a[5]), "l"(a[6]), "l"(a[7]), "r"(w[0]), "r"(w[1]), \
-                   "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory")
-// store cache policy experiment: 0 .cs (shipped), 1 default (.wb), 2 .cg, 3 .wt
-__device__ __forceinline__ void st_lab_u32x8(const uint64_t (&a)[8], const uint32_t (&w)[8], uint32_t pol) {
-    if (pol == 1) LAB_ST8("");
-    else if (pol == 2) LAB_ST8(".cg");
-    else if (pol == 3) LAB_ST8(".wt");
-    else LAB_ST8(".cs");
-}
-#endif
-
 // ---- gather role of the ring kernel's launch ---------------------------------------------------------------
 // GATHER tiles (plate seams, singular points, boxes too large to stage) read the globe directly: 32-bit
 // entries, lane = column, so one warp-level load covers 32 consecutive screen pixels of one row.  They are
@@ -385,9 +365,13 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
     }
 }
 
-// MINB: CTAs per SM the register allocation is sized for (ring warps plus the gather CTAs beside them)
-template <bool RUBIX, bool RGBA, int MINB>
-__global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm) {
+// CTAs per SM the ring kernel's register allocation is sized for, ring warps plus the gather CTAs beside them:
+// 128 registers per thread (the BOX path uses 96, 116 with the rubix overlay).  How many ring warps are resident is
+// decided in launch_ring.
+constexpr int kRingMinBlocks = 16;
+
+template <bool RUBIX, bool RGBA>
+__global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // XOR with a parameter that is always zero: keeps ptxas from re-reading the special register
     // (S2R, tens of cycles) at every `lane == 0` test instead of holding the lane number in a register
@@ -500,12 +484,6 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
                 c_by = static_cast<int16_t>(dy >> 16);
                 c_plate = static_cast<int>(dz & 7u);
                 c_bytes = ((dz >> 16) & 0xffu) * (dz >> 24) * 128u;
-#ifdef BLINKY_LAB
-                if (p.lab & 32u) {   // every box through ONE descriptor (shape 0): is the TMA unit's descriptor cache the limit?
-                    c_tmap = reinterpret_cast<uint64_t>(&tm.m[0]);
-                    c_bytes = p.lab_bytes;
-                }
-#endif
             } else {
                 ++c_unit;  // GATHER / EMPTY / no unit: nothing to stage
             }
@@ -518,21 +496,9 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
         if (ipos + n > R) ipos = 0;
         if (lane == 0) {
             const uint32_t bar = bars + 8 * is;
-#ifdef BLINKY_LAB
-            // no box load: the barrier still completes its phase (an arrive without bytes), so the slot's parity
-            // bookkeeping stays right for the entry blocks that use the slot later
-            if (!c_entry && (p.lab & 16u)) {
-                mbar_expect_tx(bar, 0);
-            } else {
-                mbar_expect_tx(bar, n);
-                if (c_entry) bulk_load(ring + ipos + dep, p.entries + static_cast<size_t>(c_tile) * kBoxBlockBytes, n, bar);
-                else tma_load_box(ring + ipos + dep, reinterpret_cast<const CUtensorMap *>(c_tmap), c_bx, c_by, c_plate, (p.lab & 8u) ? 0 : static_cast<int>(c_frame), bar);
-            }
-#else
             mbar_expect_tx(bar, n);
             if (c_entry) bulk_load(ring + ipos + dep, p.entries + static_cast<size_t>(c_tile) * kBoxBlockBytes, n, bar);
             else tma_load_box(ring + ipos + dep, reinterpret_cast<const CUtensorMap *>(c_tmap), c_bx, c_by, c_plate, static_cast<int>(c_frame), bar);
-#endif
         }
         ipos += n;
         is = is + 1 == kRingBoxes ? 0 : is + 1;
@@ -557,10 +523,7 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
         seat();
         if (A.tile < p.nbox) {
             while (can_issue()) issue(0);
-            uint32_t a_bytes = ((A.dz >> 16) & 0xffu) * (A.dz >> 24) * 128u;   // size of this unit's boxes
-#ifdef BLINKY_LAB
-            if (p.lab & 32u) a_bytes = p.lab_bytes;
-#endif
+            const uint32_t a_bytes = ((A.dz >> 16) & 0xffu) * (A.dz >> 24) * 128u;   // size of this unit's boxes
             // ---- the lane's 32 entries, out of the ring into registers once for all frames of the unit
             mbar_wait(bars + 8 * cs, (phases >> cs) & 1u);
             if (cpos + kBoxBlockBytes > R) cpos = 0;
@@ -584,12 +547,6 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
                     off[8 * k + 2 * j + 1] = (w4[j] >> 16) & kBoxOffsetMask;
                 }
             }
-#ifdef BLINKY_LAB
-            if (p.lab & 2u) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) off[i] = ((lane * 4u + (i & 3) + (i >> 2) * 128u) & 1023u) % a_bytes;   // inside the box
-            }
-#endif
             // the block's bytes may be overwritten once they sit in registers (same reasoning as stage_dep)
             {
                 uint32_t dep = 0;
@@ -659,15 +616,6 @@ __global__ void __launch_bounds__(32, MINB) warp_ring_kernel(const __grid_consta
                         uint64_t a[8];
 #pragma unroll
                         for (int q = 0; q < 8; ++q) a[q] = reinterpret_cast<uint64_t>(o) + static_cast<uint64_t>(static_cast<uint32_t>(q) * row4);
-#ifdef BLINKY_LAB
-                        if (p.lab & 4u) {
-                            uint8_t *fb = static_cast<uint8_t *>(p.out) + static_cast<size_t>(A.f0 + f) * p.out_stride + static_cast<size_t>(A.tile) * 1024u;
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) a[q] = reinterpret_cast<uint64_t>(fb + q * 128 + lane * 4u);
-                        }
-                        if ((p.lab >> 8) & 3u) st_lab_u32x8(a, w, (p.lab >> 8) & 3u);
-                        else if (!(p.lab & 1u) || w[0] == 0x12345679u)
-#endif
                         st_stream_u32x8(a, w);
                     }
                     o += p.out_stride;
@@ -827,34 +775,8 @@ inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 }  // namespace
 
 // ---------------------------------------------------------------------------
-// frame pipeline slot
+// frame pipeline slot: one frame of blinky_warp_host in flight
 // ---------------------------------------------------------------------------
-// ---- host -> device plate upload without the copy engine --------------------------------------
-// The rectangles a lens samples are strided (e.g. half a plate wide); 2-D DMA copies of them reach
-// ~35 GB/s here while the link does 45-48.  Pinned host memory is mapped into the device address
-// space (UVA), so the SMs can pull exactly those bytes themselves, 16 bytes per thread.
-struct UploadRects {
-    int n;
-    uint32_t off[6];     // byte offset of the rectangle's first 16-byte column in the frame
-    uint32_t vec_w[6];   // rectangle width in 16-byte vectors
-    uint32_t rows[6];
-    uint32_t first[7];   // prefix sum of vec_w * rows
-    uint32_t pitch;      // platesize
-};
-
-__global__ void __launch_bounds__(256) upload_rects_kernel(const uint8_t *__restrict__ host_src, uint8_t *__restrict__ dst, const __grid_constant__ UploadRects R) {
-    const uint32_t total = R.first[R.n];
-    for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < total; v += gridDim.x * blockDim.x) {
-        int k = 0;
-        while (v >= R.first[k + 1]) ++k;
-        const uint32_t local = v - R.first[k];
-        const uint32_t row = local / R.vec_w[k], col = local - row * R.vec_w[k];
-        const size_t at = static_cast<size_t>(R.off[k]) + static_cast<size_t>(row) * R.pitch + static_cast<size_t>(col) * 16;
-        const uint4 x = __ldcs(reinterpret_cast<const uint4 *>(host_src + at));
-        *reinterpret_cast<uint4 *>(dst + at) = x;
-    }
-}
-
 struct WarpDevice::Slot {
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
@@ -862,9 +784,7 @@ struct WarpDevice::Slot {
     uint8_t *h_faces = nullptr, *h_out = nullptr;  // pinned staging
     bool busy = false;
     // finalize info
-    uint8_t *dst = nullptr;          // first frame of the group
-    size_t dst_frame_stride = 0;
-    int nf = 0;                      // frames in the slot
+    uint8_t *dst = nullptr;          // the caller's frame
     int dst_rowbytes = 0, x0 = 0, y0 = 0;
     bool keep_unmapped = false, direct = false;
 };
@@ -908,9 +828,6 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     }
     sm_count_ = prop.multiProcessorCount;
     smem_per_sm_ = prop.sharedMemPerMultiprocessor;
-    if (const char *e = getenv("BLINKY_E2E_UPLOAD")) upload_by_kernel_ = strcmp(e, "kernel") == 0;
-    if (const char *e = getenv("BLINKY_E2E_OUT")) out_by_kernel_ = strcmp(e, "direct") == 0;
-    if (const char *e = getenv("BLINKY_E2E_BATCH")) batch_copies_ = atoi(e) != 0;
     if (const char *e = getenv("BLINKY_RING_BYTES")) ring_bytes_override_ = atoi(e);
     if (const char *e = getenv("BLINKY_RING_BOXES")) ring_boxes_ = atoi(e);
     if (const char *e = getenv("BLINKY_MERGED_ITEMS")) merged_items_max_ = atoi(e);
@@ -918,7 +835,6 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     if (const char *e = getenv("BLINKY_FCHUNK")) fchunk_ = atoi(e);
     if (const char *e = getenv("BLINKY_SERIAL_GATHER")) serial_gather_ = atoi(e) != 0;  // GATHER tiles in their own kernel before the ring kernel (A/B)
     if (const char *e = getenv("BLINKY_STATIC_PCT")) static_pct_ = std::max(0, std::min(100, atoi(e)));
-    if (const char *e = getenv("BLINKY_L2_PROMOTION")) l2_promotion_ = atoi(e) & 3;  // 0 none, 1 64 B, 2 128 B, 3 256 B
     cudaStream_t s;
     e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
     if (e != cudaSuccess) throw std::runtime_error(std::string("cudaStreamCreate: ") + cudaGetErrorString(e));
@@ -1109,17 +1025,10 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
     const cuuint32_t estr[4] = {1, 1, 1, 1};
     for (size_t si = 0; si < shapes_.size() && si < static_cast<size_t>(kMaxShapes); ++si) {
         const uint32_t w16 = shapes_[si] >> 8, h8 = shapes_[si] & 0xff;
-        cuuint32_t box[4] = {w16 * 16, h8 * 8, 1, 1};
-#ifdef BLINKY_LAB
-        // timing experiment: the same bytes as wider, flatter boxes (fewer TMA rows; wrong texels)
-        if (const char *e = getenv("BLINKY_LAB_FLAT")) {
-            for (int k = atoi(e); k > 1; k /= 2)
-                if (box[0] * 2 <= 256 && box[1] % 2 == 0) box[0] *= 2, box[1] /= 2;
-        }
-#endif
+        const cuuint32_t box[4] = {w16 * 16, h8 * 8, 1, 1};
         CUresult r = reinterpret_cast<EncodeTiledFn>(encode_fn_)(
             &t->table.m[si], CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void *>(d_faces), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, static_cast<CUtensorMapL2promotion>(l2_promotion_), CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             char buf[160];
             snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(box %ux%u, ps %d) failed with CUresult %d", w16 * 16, h8 * 8, platesize_, static_cast<int>(r));
@@ -1131,10 +1040,6 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
     return t;
 }
 
-// CTAs per SM the ring kernel's register allocation is sized for: 16 (128 registers per thread; the BOX path uses 96,
-// 116 with the rubix overlay).  How many ring warps are resident is decided in launch_ring.
-template <bool RUBIX>
-constexpr int ring_warps() { return 16; }
 // Resident ring warps per SM by default (BLINKY_RING_CTAS): measured on the 4K panini batch (bench.py, H100 80GB HBM3
 // at a 400 W power limit) 8 / 10 / 12 / 14 / 16 warps give 578 / 578 / 657 / 652 / 653 Gpixel/s — beyond 12, more
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
@@ -1142,9 +1047,9 @@ constexpr int kRingWarpsDefault = 12;
 
 template <bool RUBIX, bool RGBA>
 static cudaError_t ring_config(size_t smem, int *ctas_per_sm) {
-    cudaError_t e = cudaFuncSetAttribute(warp_ring_kernel<RUBIX, RGBA, ring_warps<RUBIX>()>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    cudaError_t e = cudaFuncSetAttribute(warp_ring_kernel<RUBIX, RGBA>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, warp_ring_kernel<RUBIX, RGBA, ring_warps<RUBIX>()>, 32, smem);
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, warp_ring_kernel<RUBIX, RGBA>, 32, smem);
 }
 
 static cudaError_t ring_config_v(bool rubix, bool rgba, size_t smem, int *n) {
@@ -1155,10 +1060,10 @@ static cudaError_t ring_config_v(bool rubix, bool rgba, size_t smem, int *n) {
 }
 
 static void ring_launch_v(bool rubix, bool rgba, uint32_t grid, size_t smem, cudaStream_t st, const RingParams &p, const RingTmaps &tm) {
-    if (rubix && rgba) warp_ring_kernel<true, true, ring_warps<true>()><<<grid, 32, smem, st>>>(p, tm);
-    else if (rubix) warp_ring_kernel<true, false, ring_warps<true>()><<<grid, 32, smem, st>>>(p, tm);
-    else if (rgba) warp_ring_kernel<false, true, ring_warps<false>()><<<grid, 32, smem, st>>>(p, tm);
-    else warp_ring_kernel<false, false, ring_warps<false>()><<<grid, 32, smem, st>>>(p, tm);
+    if (rubix && rgba) warp_ring_kernel<true, true><<<grid, 32, smem, st>>>(p, tm);
+    else if (rubix) warp_ring_kernel<true, false><<<grid, 32, smem, st>>>(p, tm);
+    else if (rgba) warp_ring_kernel<false, true><<<grid, 32, smem, st>>>(p, tm);
+    else warp_ring_kernel<false, false><<<grid, 32, smem, st>>>(p, tm);
 }
 
 bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes,
@@ -1188,9 +1093,6 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.width = width_;
     p.height = height_;
     p.zero = 0;
-    p.lab = 0;
-    if (const char *e = getenv("BLINKY_LAB")) p.lab = static_cast<uint32_t>(atoi(e));
-    p.lab_bytes = shapes_.empty() ? 128u : static_cast<uint32_t>((shapes_[0] >> 8) * (shapes_[0] & 0xff) * 128);
     const bool rubix = rubix_;
     const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0);
     // The ring kernel takes the BOX tiles [0, nbox) and the EMPTY tiles; the GATHER tiles in between go to the
@@ -1209,11 +1111,10 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     // trism, but with 16 frames K3 in front is faster by 1.5-10 % (panini, stereographic, trism, 1080p panini; the
     // 1080p batch prefers K3 from 8 frames on, by 10 %, and keeps riding along there).
     constexpr int kMergedFramesMax = 8;
-    const uint32_t all_gather_items = ngather_tiles_ * (kTileH / kGatherRows) * static_cast<uint32_t>((nframes + kGatherFrames - 1) / kGatherFrames);
+    const uint32_t gather_items = ngather_tiles_ * (kTileH / kGatherRows) * static_cast<uint32_t>((nframes + kGatherFrames - 1) / kGatherFrames);
     const bool merged_gather = !serial_gather_ && ngather_tiles_ > 0 && nframes <= kMergedFramesMax &&
-                               all_gather_items <= static_cast<uint32_t>(merged_items_max_);
-    int want = std::min(kRingWarpsDefault, rubix ? ring_warps<true>() : ring_warps<false>());
-    if (ring_ctas_cap_ > 0) want = std::min(ring_ctas_cap_, rubix ? ring_warps<true>() : ring_warps<false>());
+                               gather_items <= static_cast<uint32_t>(merged_items_max_);
+    int want = ring_ctas_cap_ > 0 ? std::min(ring_ctas_cap_, kRingMinBlocks) : kRingWarpsDefault;
     // ring size: twice the plan's largest box plus an entry block (two boxes of any size and the next unit's entries in
     // flight), as far as `want`
     // resident warps — plus two gather CTAs, which
@@ -1272,14 +1173,9 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     int nbuf = 0;
     // GATHER tiles: one-warp CTAs behind the ring warps in the same grid (see gather_item); only a plan without BOX and
     // EMPTY tiles launches the stand-alone gather kernel.
-    uint32_t ngather = ngather_tiles_;
-#ifdef BLINKY_LAB
-    if (getenv("BLINKY_LAB_NOK3")) ngather = 0;  // time the ring warps alone
-#endif
-    const uint32_t gather_items = ngather * (kTileH / kGatherRows) * static_cast<uint32_t>((nframes + kGatherFrames - 1) / kGatherFrames);
     buf[0] = 0;
-    if (ngather > 0 && (grid == 0 || !merged_gather)) {
-        dim3 g2(ngather, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
+    if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
+        dim3 g2(ngather_tiles_, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
         if (rubix && rgba) warp_tile_gather_kernel<true, true><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
         else if (rubix) warp_tile_gather_kernel<true, false><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
         else if (rgba) warp_tile_gather_kernel<false, true><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
@@ -1386,19 +1282,8 @@ bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_ou
 
 bool WarpDevice::ensure_slots() {
     if (!slots_.empty()) return true;
-    int kSlots = 3;
-    if (const char *e = getenv("BLINKY_HOST_SLOTS")) {  // pipeline depth of blinky_warp_host (experiments)
-        const int v = atoi(e);
-        if (v >= 1 && v <= 16) kSlots = v;
-    }
-    // A slot can hold a GROUP of frames (one batched upload, one launch, one copy back per group; BLINKY_HOST_GROUP).
-    // Measured with 16-frame calls: 1 / 2 / 4 / 8 frames per group give 28.4 / 26.6 / 25.9 / 25.0 Gpx/s — fewer, larger
-    // copies do not make the link faster, and the coarser pipeline overlaps less — so the default is one frame per slot.
-    host_group_ = 1;
-    if (const char *e = getenv("BLINKY_HOST_GROUP")) {
-        const int v = atoi(e);
-        if (v >= 1 && v <= kMaxHostGroup) host_group_ = v;
-    }
+    // three frames in flight overlap upload, warp and copy back; 2-8 measured the same
+    constexpr int kSlots = 3;
     slot_face_bytes_ = static_cast<size_t>(numplates_) * platesize_ * platesize_;
     slot_out_bytes_ = round_up(npix_, 16);
     for (int i = 0; i < kSlots; ++i) {
@@ -1406,9 +1291,9 @@ bool WarpDevice::ensure_slots() {
         slots_.push_back(s);
         CK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
-        CK(cudaMalloc(&s->d_faces, slot_face_bytes_ * host_group_));
-        CK(cudaMemset(s->d_faces, 0, slot_face_bytes_ * host_group_));
-        CK(cudaMalloc(&s->d_out, slot_out_bytes_ * host_group_));
+        CK(cudaMalloc(&s->d_faces, slot_face_bytes_));
+        CK(cudaMemset(s->d_faces, 0, slot_face_bytes_));
+        CK(cudaMalloc(&s->d_out, slot_out_bytes_));
         // (pinned staging for callers whose buffers are not pinned: allocated when first needed)
     }
     return true;
@@ -1420,24 +1305,21 @@ void WarpDevice::finalize_slot(Slot &s) {
     s.busy = false;
     if (s.direct) return;  // the copy engine already wrote the caller's buffer
     const int W = width_, H = height_;
-    for (int k = 0; k < s.nf; ++k) {
-        uint8_t *dst = s.dst + static_cast<size_t>(k) * s.dst_frame_stride + static_cast<size_t>(s.y0) * s.dst_rowbytes + s.x0;
-        const uint8_t *frame = s.h_out + static_cast<size_t>(k) * slot_out_bytes_;
-        if (s.keep_unmapped) {
-            // only mapped pixels are written, like `if (*lmap)` in render_lensmap (:2413)
-            for (int y = 0; y < H; ++y) {
-                const uint8_t *src = frame + static_cast<size_t>(y) * W;
-                uint8_t *row = dst + static_cast<size_t>(y) * s.dst_rowbytes;
-                for (int32_t j = span_off_[static_cast<size_t>(y)]; j < span_off_[static_cast<size_t>(y) + 1]; ++j) {
-                    const int32_t a = spans_[static_cast<size_t>(j) * 2], b = spans_[static_cast<size_t>(j) * 2 + 1];
-                    memcpy(row + a, src + a, static_cast<size_t>(b - a));
-                }
+    uint8_t *dst = s.dst + static_cast<size_t>(s.y0) * s.dst_rowbytes + s.x0;
+    if (s.keep_unmapped) {
+        // only mapped pixels are written, like `if (*lmap)` in render_lensmap (:2413)
+        for (int y = 0; y < H; ++y) {
+            const uint8_t *src = s.h_out + static_cast<size_t>(y) * W;
+            uint8_t *row = dst + static_cast<size_t>(y) * s.dst_rowbytes;
+            for (int32_t j = span_off_[static_cast<size_t>(y)]; j < span_off_[static_cast<size_t>(y) + 1]; ++j) {
+                const int32_t a = spans_[static_cast<size_t>(j) * 2], b = spans_[static_cast<size_t>(j) * 2 + 1];
+                memcpy(row + a, src + a, static_cast<size_t>(b - a));
             }
-        } else if (s.dst_rowbytes == W) {
-            memcpy(dst, frame, static_cast<size_t>(W) * H);
-        } else {
-            for (int y = 0; y < H; ++y) memcpy(dst + static_cast<size_t>(y) * s.dst_rowbytes, frame + static_cast<size_t>(y) * W, static_cast<size_t>(W));
         }
+    } else if (s.dst_rowbytes == W) {
+        memcpy(dst, s.h_out, static_cast<size_t>(W) * H);
+    } else {
+        for (int y = 0; y < H; ++y) memcpy(dst + static_cast<size_t>(y) * s.dst_rowbytes, s.h_out + static_cast<size_t>(y) * W, static_cast<size_t>(W));
     }
 }
 
@@ -1465,134 +1347,81 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
     if (dst_host != pin_dst_ptr_) pin_dst_ptr_ = dst_host, pin_dst_ = is_pinned(dst_host);
     const bool src_pinned = pin_src_, dst_pinned = pin_dst_;
     const int W = width_, H = height_;
+    const bool direct = dst_pinned && !keep_unmapped;  // the copy engine writes the caller's buffer, no staging
+    const size_t frame = static_cast<size_t>(W) * H;
     bool ok = true;
-    const int G = std::max(1, std::min(host_group_, kMaxHostGroup));
-    int group = 0;
-    for (int f0 = 0; f0 < nframes && ok; ++group) {
-        const int g = std::min(G, nframes - f0);
-        Slot &s = *slots_[static_cast<size_t>(group) % slots_.size()];
-        finalize_slot(s);  // frees the slot (waits for the group that used it last)
-        const bool direct = dst_pinned && !keep_unmapped;
-        if (!src_pinned && !s.h_faces) CK(cudaMallocHost(&s.h_faces, slot_face_bytes_ * G));
-        if (!direct && !s.h_out) CK(cudaMallocHost(&s.h_out, slot_out_bytes_ * G));
+    int f = 0;
+    for (; f < nframes; ++f) {
+        Slot &s = *slots_[static_cast<size_t>(f) % slots_.size()];
+        finalize_slot(s);  // frees the slot (waits for the frame that used it last)
+        if (!src_pinned && !s.h_faces) CK(cudaMallocHost(&s.h_faces, slot_face_bytes_));
+        if (!direct && !s.h_out) CK(cudaMallocHost(&s.h_out, slot_out_bytes_));
         // Only what the lens looks at is uploaded: plates with display != 0 (:764-766), and of
         // those only the texel rectangle the lensmap samples.  (TMA boxes may overhang the
         // rectangle; those texels are staged but never referenced by an entry.)
-        cudaMemcpy3DBatchOp ops[BLINKY_MAX_PLATES * kMaxHostGroup];
+        const uint8_t *src = faces_host + static_cast<size_t>(f) * face_stride;
+        cudaMemcpy3DBatchOp ops[BLINKY_MAX_PLATES];
         size_t nops = 0;
-        for (int k = 0; k < g && ok; ++k) {
-            const uint8_t *src = faces_host + static_cast<size_t>(f0 + k) * face_stride;
-            uint8_t *d_frame = s.d_faces + static_cast<size_t>(k) * slot_face_bytes_;
-            UploadRects ur;
-            ur.n = 0;
-            ur.first[0] = 0;
-            ur.pitch = static_cast<uint32_t>(platesize_);
-            const bool by_kernel = upload_by_kernel_ && platesize_ % 16 == 0 && reinterpret_cast<uintptr_t>(src) % 16 == 0 && face_stride % 16 == 0;
-            for (int pl = 0; pl < numplates_; ++pl) {
-                if (!display_[pl]) continue;
-                const int *r = plate_rect_[pl];
-                if (r[0] > r[2] || r[1] > r[3]) continue;
-                if (by_kernel && src_pinned) {
-                    const int xa = r[0] & ~15, xb = (r[2] + 16) & ~15;  // 16-byte columns covering [r0, r2]
-                    ur.off[ur.n] = static_cast<uint32_t>(pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + xa);
-                    ur.vec_w[ur.n] = static_cast<uint32_t>((xb - xa) / 16);
-                    ur.rows[ur.n] = static_cast<uint32_t>(r[3] - r[1] + 1);
-                    ur.first[ur.n + 1] = ur.first[ur.n] + ur.vec_w[ur.n] * ur.rows[ur.n];
-                    ++ur.n;
-                    continue;
-                }
-                const size_t rw = static_cast<size_t>(r[2] - r[0] + 1), rh = static_cast<size_t>(r[3] - r[1] + 1);
-                const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + r[0];
-                const uint8_t *from = src + off;
-                if (!src_pinned) {
-                    uint8_t *stage = s.h_faces + static_cast<size_t>(k) * slot_face_bytes_ + off;
-                    for (size_t y = 0; y < rh; ++y) memcpy(stage + y * platesize_, from + y * platesize_, rw);
-                    from = stage;
-                }
-                // a full-width rectangle is one contiguous run: copy it as such
-                const bool contiguous = rw == static_cast<size_t>(platesize_);
-                if (batch_copies_) {  // all rectangles of the group in ONE driver call (no gap between the DMA operations)
-                    cudaMemcpy3DBatchOp &op = ops[nops++];
-                    memset(&op, 0, sizeof op);
-                    const size_t row = contiguous ? rw * rh : static_cast<size_t>(platesize_), rows = contiguous ? 1 : rh;
-                    op.src.type = cudaMemcpyOperandTypePointer;
-                    op.src.op.ptr.ptr = const_cast<uint8_t *>(from);
-                    op.src.op.ptr.rowLength = row;
-                    op.src.op.ptr.layerHeight = rows;
-                    op.dst.type = cudaMemcpyOperandTypePointer;
-                    op.dst.op.ptr.ptr = d_frame + off;
-                    op.dst.op.ptr.rowLength = row;
-                    op.dst.op.ptr.layerHeight = rows;
-                    op.extent = make_cudaExtent(contiguous ? rw * rh : rw, rows, 1);
-                    op.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
-                    continue;
-                }
-                cudaError_t e = contiguous ? cudaMemcpyAsync(d_frame + off, from, rw * rh, cudaMemcpyHostToDevice, s.stream)
-                                           : cudaMemcpy2DAsync(d_frame + off, static_cast<size_t>(platesize_), from, static_cast<size_t>(platesize_), rw, rh,
-                                                               cudaMemcpyHostToDevice, s.stream);
-                if (e != cudaSuccess) { ok = fail("cudaMemcpy2DAsync(H2D faces)", e); break; }
+        for (int pl = 0; pl < numplates_; ++pl) {
+            if (!display_[pl]) continue;
+            const int *r = plate_rect_[pl];
+            if (r[0] > r[2] || r[1] > r[3]) continue;
+            const size_t rw = static_cast<size_t>(r[2] - r[0] + 1), rh = static_cast<size_t>(r[3] - r[1] + 1);
+            const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + r[0];
+            const uint8_t *from = src + off;
+            if (!src_pinned) {
+                uint8_t *stage = s.h_faces + off;
+                for (size_t y = 0; y < rh; ++y) memcpy(stage + y * platesize_, from + y * platesize_, rw);
+                from = stage;
             }
-            if (ok && ur.n > 0) {
-                const uint32_t total = ur.first[ur.n];
-                const unsigned blocks = std::min<unsigned>((total + 255) / 256, static_cast<unsigned>(sm_count_) * 8u);
-                upload_rects_kernel<<<blocks, 256, 0, s.stream>>>(src, d_frame, ur);
-                ++launches_;
-            }
+            // a full-width rectangle is one contiguous run: copy it as such
+            const bool contiguous = rw == static_cast<size_t>(platesize_);
+            const size_t row = contiguous ? rw * rh : static_cast<size_t>(platesize_), rows = contiguous ? 1 : rh;
+            cudaMemcpy3DBatchOp &op = ops[nops++];
+            memset(&op, 0, sizeof op);
+            op.src.type = cudaMemcpyOperandTypePointer;
+            op.src.op.ptr.ptr = const_cast<uint8_t *>(from);
+            op.src.op.ptr.rowLength = row;
+            op.src.op.ptr.layerHeight = rows;
+            op.dst.type = cudaMemcpyOperandTypePointer;
+            op.dst.op.ptr.ptr = s.d_faces + off;
+            op.dst.op.ptr.rowLength = row;
+            op.dst.op.ptr.layerHeight = rows;
+            op.extent = make_cudaExtent(contiguous ? rw * rh : rw, rows, 1);
+            op.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
         }
-        if (ok && nops > 0) {
-            size_t fail_idx = 0;
-            cudaError_t e = cudaMemcpy3DBatchAsync(nops, ops, &fail_idx, 0, s.stream);
-            if (e != cudaSuccess) {
-                // not available on this driver: fall back to one copy per rectangle, from now on
-                cudaGetLastError();
-                batch_copies_ = false;
-                for (size_t k = 0; k < nops && ok; ++k) {
-                    e = cudaMemcpy2DAsync(ops[k].dst.op.ptr.ptr, ops[k].dst.op.ptr.rowLength, ops[k].src.op.ptr.ptr, ops[k].src.op.ptr.rowLength,
-                                          ops[k].extent.width, ops[k].extent.height, cudaMemcpyHostToDevice, s.stream);
-                    if (e != cudaSuccess) ok = fail("cudaMemcpy2DAsync(H2D faces)", e);
-                }
-            }
+        // all rectangles of the frame in ONE driver call (no gap between the DMA operations)
+        size_t fail_idx = 0;
+        if (nops > 0 && batch_copies_ && cudaMemcpy3DBatchAsync(nops, ops, &fail_idx, 0, s.stream) != cudaSuccess) {
+            cudaGetLastError();  // not available on this driver: one copy per rectangle, from now on
+            batch_copies_ = false;
+        }
+        for (size_t k = 0; !batch_copies_ && k < nops && ok; ++k) {
+            const cudaError_t e = cudaMemcpy2DAsync(ops[k].dst.op.ptr.ptr, ops[k].dst.op.ptr.rowLength, ops[k].src.op.ptr.ptr, ops[k].src.op.ptr.rowLength,
+                                                    ops[k].extent.width, ops[k].extent.height, cudaMemcpyHostToDevice, s.stream);
+            if (e != cudaSuccess) ok = fail("cudaMemcpy2DAsync(H2D faces)", e);
         }
         if (!ok) break;
-        s.dst = dst_host + static_cast<size_t>(f0) * dst_frame_stride;
-        s.dst_frame_stride = dst_frame_stride;
-        s.nf = g;
-        // the warp kernel can store straight into the caller's pinned frames (posted PCIe writes, no
-        // staging copy) when they are tightly packed
-        const bool zero_copy_out = out_by_kernel_ && direct && dst_rowbytes == W && x0 == 0 && y0 == 0 &&
-                                   reinterpret_cast<uintptr_t>(s.dst) % 16 == 0 && (g == 1 || dst_frame_stride % 16 == 0);
-        if (!warp(s.d_faces, slot_face_bytes_, zero_copy_out ? s.dst : s.d_out, zero_copy_out ? dst_frame_stride : slot_out_bytes_, g, s.stream, false)) { ok = false; break; }
+        s.dst = dst_host + static_cast<size_t>(f) * dst_frame_stride;
+        if (!warp(s.d_faces, slot_face_bytes_, s.d_out, slot_out_bytes_, 1, s.stream, false)) { ok = false; break; }
         s.dst_rowbytes = dst_rowbytes;
         s.x0 = x0;
         s.y0 = y0;
         s.keep_unmapped = keep_unmapped;
         s.direct = direct;
-        cudaError_t e = cudaSuccess;
-        const size_t frame = static_cast<size_t>(W) * H;
-        if (zero_copy_out) {
-        } else if (direct && dst_rowbytes == W && (g == 1 || (dst_frame_stride == frame && slot_out_bytes_ == frame))) {
-            // tightly packed destination frames: the whole group is one contiguous run
-            e = cudaMemcpyAsync(s.dst + static_cast<size_t>(y0) * dst_rowbytes + x0, s.d_out, frame * g, cudaMemcpyDeviceToHost, s.stream);
-        } else if (direct) {
-            for (int k = 0; k < g && e == cudaSuccess; ++k) {
-                uint8_t *to = s.dst + static_cast<size_t>(k) * dst_frame_stride + static_cast<size_t>(y0) * dst_rowbytes + x0;
-                const uint8_t *from = s.d_out + static_cast<size_t>(k) * slot_out_bytes_;
-                e = dst_rowbytes == W ? cudaMemcpyAsync(to, from, frame, cudaMemcpyDeviceToHost, s.stream)
-                                      : cudaMemcpy2DAsync(to, static_cast<size_t>(dst_rowbytes), from, static_cast<size_t>(W), static_cast<size_t>(W),
-                                                          static_cast<size_t>(H), cudaMemcpyDeviceToHost, s.stream);
-            }
-        } else {
-            e = cudaMemcpyAsync(s.h_out, s.d_out, slot_out_bytes_ * (g - 1) + frame, cudaMemcpyDeviceToHost, s.stream);
-        }
+        uint8_t *to = s.dst + static_cast<size_t>(y0) * dst_rowbytes + x0;
+        cudaError_t e = !direct              ? cudaMemcpyAsync(s.h_out, s.d_out, frame, cudaMemcpyDeviceToHost, s.stream)
+                        : dst_rowbytes == W ? cudaMemcpyAsync(to, s.d_out, frame, cudaMemcpyDeviceToHost, s.stream)
+                                            : cudaMemcpy2DAsync(to, static_cast<size_t>(dst_rowbytes), s.d_out, static_cast<size_t>(W),
+                                                                static_cast<size_t>(W), static_cast<size_t>(H), cudaMemcpyDeviceToHost, s.stream);
         if (e != cudaSuccess) { ok = fail("cudaMemcpyAsync(D2H frame)", e); break; }
         e = cudaEventRecord(s.done, s.stream);
         if (e != cudaSuccess) { ok = fail("cudaEventRecord", e); break; }
         s.busy = true;
-        f0 += g;
     }
     // drain in submission order
     for (size_t k = 0; k < slots_.size(); ++k) {
-        Slot &s = *slots_[(static_cast<size_t>(group) + k) % slots_.size()];
+        Slot &s = *slots_[(static_cast<size_t>(f) + k) % slots_.size()];
         finalize_slot(s);
     }
     if (ok) {

@@ -72,8 +72,7 @@ private:
     int device_ = 0;
     int sm_count_ = 132;
     void *stream_ = nullptr;  // cudaStream_t
-    bool upload_by_kernel_ = false, out_by_kernel_ = false;  // warp_host variants (BLINKY_E2E_UPLOAD / BLINKY_E2E_OUT)
-    bool batch_copies_ = true;   // plate rectangles of a frame in one cudaMemcpy3DBatchAsync (BLINKY_E2E_BATCH=0: one 2-D copy each)
+    bool batch_copies_ = true;   // plate rectangles of a frame in one cudaMemcpy3DBatchAsync (false once the driver refused it)
     const void *pin_src_ptr_ = nullptr, *pin_dst_ptr_ = nullptr;  // last buffers warp_host saw and whether they are pinned
     bool pin_src_ = false, pin_dst_ = false;
     std::string err_;
@@ -107,7 +106,6 @@ private:
     uint32_t ntiles_ = 0, nbox_tiles_ = 0, ngather_tiles_ = 0;
     int stage_bytes_ = 0;                // largest staged box of the plan
     int static_pct_ = 85;                // share of the ring kernel's units scheduled statically (BLINKY_STATIC_PCT)
-    int l2_promotion_ = 0;               // CUtensorMapL2promotion of the box descriptors (BLINKY_L2_PROMOTION)
     bool serial_gather_ = false;         // BLINKY_SERIAL_GATHER=1: GATHER tiles in their own kernel instead of as extra CTAs of the ring kernel's launch
     int ring_bytes_override_ = 0, ring_ctas_cap_ = 0, fchunk_ = 0;  // tuning overrides (BLINKY_RING_BYTES / _CTAS, BLINKY_FCHUNK); 0 = automatic
     int merged_items_max_ = 4096;        // gather items up to which GATHER tiles ride in the ring kernel's launch of <= 8 frames (BLINKY_MERGED_ITEMS)
@@ -133,8 +131,6 @@ private:
     // e2e pipeline
     std::vector<Slot *> slots_;
     size_t slot_face_bytes_ = 0, slot_out_bytes_ = 0;
-    static constexpr int kMaxHostGroup = 8;
-    int host_group_ = 1;                 // frames per slot of the blinky_warp_host pipeline (BLINKY_HOST_GROUP)
 
     int64_t launches_ = 0;
     std::string last_kernel_;

@@ -261,15 +261,20 @@ def test_pinned_host_buffers(bb, fe, restate, palette):
     idx, tint = fe.lensmap()
     pm = restate.palmaps(palette)
     src = fe.alloc_pinned(N * 6 * PS * PS)
-    dst = fe.alloc_pinned(N * W * H)
     faces = np.stack([bb.synthetic_faces(6, PS, 20 + f) for f in range(N)])
     src[:] = faces.reshape(-1)
-    dst[:] = 0
-    fe.warp_host(src, dst.reshape(N, H, W))
     want = np.stack([restate.render(idx, tint, faces[f], pm, False) for f in range(N)])
-    assert np.array_equal(dst.reshape(N, H, W), want)
+    # the frame fills the pinned screen, or is a view rectangle of a wider one (rows copied at the screen's pitch)
+    for SW, SH, x0, y0 in [(W, H, 0, 0), (W + 24, H + 10, 8, 6)]:
+        dst = fe.alloc_pinned(N * SW * SH)
+        dst[:] = 77
+        screen = dst.reshape(N, SH, SW)
+        fe.warp_host(src, screen, x0=x0, y0=y0)
+        expect = np.full((N, SH, SW), 77, np.uint8)
+        expect[:, y0:y0 + H, x0:x0 + W] = want
+        assert np.array_equal(screen, expect), (SW, SH, x0, y0)
+        fe.free_pinned(dst)
     fe.free_pinned(src)
-    fe.free_pinned(dst)
 
 
 def test_rgba_expansion(bb, fe, restate, palette, torch_mod):
