@@ -97,6 +97,8 @@ _SIGNATURES = [
     ("blinky_set_kernel", c_int, [_CTX, c_int]),
     ("blinky_set_background", c_int, [_CTX, c_void_p]),
     ("blinky_warp_device", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p]),
+    ("blinky_warp_device_view", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    ("blinky_warp_device_view_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     ("blinky_warp_host", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int]),
     ("blinky_upload_bytes_per_frame", c_int64, [_CTX]),
     ("blinky_alloc_pinned", c_int, [_CTX, c_size_t, POINTER(c_void_p)]),
@@ -396,6 +398,25 @@ class Fisheye:
             out_stride = self.width * self.height * (4 if rgba else 1)
         fn = self._lib.blinky_warp_device_rgba if rgba else self._lib.blinky_warp_device
         self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_out), out_stride, nframes, stream))
+
+    def warp_view(self, d_faces, d_screen, x0: int = 0, y0: int = 0, rowbytes: int | None = None, nframes: int = 1,
+                  keep_unmapped: bool = False, rgba: bool = False, face_stride: int | None = None,
+                  screen_stride: int | None = None, stream: int | None = None):
+        """device-resident batch into the view rectangle at pixel (x0, y0) of device screens (blinky_warp_device_view).
+        d_screen: a torch CUDA tensor [N, SH, SW] (or [SH, SW]), whose row pitch and frame stride give rowbytes and
+        screen_stride, or a raw device address.  keep_unmapped: only mapped pixels are written."""
+        if face_stride is None:
+            face_stride = self.numplates * self.platesize * self.platesize
+        bpp = 4 if rgba else 1
+        shape = getattr(d_screen, "shape", None)
+        if rowbytes is None:
+            rowbytes = d_screen.stride(-2) * d_screen.element_size() if shape is not None and len(shape) >= 2 else (x0 + self.width) * bpp
+        if screen_stride is None:
+            screen_stride = (d_screen.stride(-3) * d_screen.element_size() if shape is not None and len(shape) >= 3
+                             else (y0 + self.height) * rowbytes)
+        fn = self._lib.blinky_warp_device_view_rgba if rgba else self._lib.blinky_warp_device_view
+        self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_screen), screen_stride, rowbytes, x0, y0, nframes,
+                       1 if keep_unmapped else 0, stream))
 
     def warp_host(self, faces: np.ndarray, dst: np.ndarray | None = None, keep_unmapped: bool = False, x0: int = 0,
                   y0: int = 0, nframes: int | None = None, dst_rowbytes: int | None = None,

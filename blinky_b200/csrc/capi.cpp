@@ -346,12 +346,56 @@ int blinky_set_background(blinky_ctx *ctx, const uint8_t *bg) {
     return ctx->dev->set_background(bg) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
 }
 
+}  // extern "C"
+
+namespace {
+
+// The one way into the device-resident warp: frames land in the view rectangle at (x0, y0) of screens with rows of
+// `rowbytes` bytes.  The dense entry points are the rectangle that is the whole screen.
+int warp_into_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
+                   int rowbytes, int x0, int y0, int nframes, bool keep_unmapped, void *stream, bool rgba) {
+    const size_t bpp = rgba ? 4 : 1;
+    uint8_t *origin = static_cast<uint8_t *>(d_screen) + static_cast<size_t>(y0) * static_cast<size_t>(rowbytes) + static_cast<size_t>(x0) * bpp;
+    return ctx->dev->warp(d_faces, face_stride, origin, screen_frame_stride, nframes, stream, rgba, static_cast<size_t>(rowbytes), keep_unmapped)
+               ? BLINKY_OK
+               : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+}
+
+int warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
+                     int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream, bool rgba) {
+    NEED_DEVICE(ctx);
+    const char *name = rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
+    auto invalid = [&](const char *why) { return set_err(ctx, BLINKY_E_INVALID, std::string(name) + ": " + why); };
+    const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = rgba ? 4 : 1;
+    if (!d_faces || !d_screen) return invalid("NULL buffer");
+    if (x0 < 0 || y0 < 0) return invalid("the view origin (x0, y0) must not be negative");
+    if (static_cast<int64_t>(rowbytes) < (x0 + W) * bpp) return invalid("rowbytes too small for the view rectangle");
+    if (nframes > 1 && static_cast<uint64_t>(screen_frame_stride) < static_cast<uint64_t>((y0 + H) * rowbytes))
+        return invalid("screen_frame_stride too small for the view rectangle");
+    if (rgba && ((reinterpret_cast<uintptr_t>(d_screen) + static_cast<uintptr_t>(y0) * static_cast<uintptr_t>(rowbytes)) % 4 != 0 || rowbytes % 4 != 0 ||
+                 (nframes > 1 && screen_frame_stride % 4 != 0)))
+        return invalid("the RGBA view origin, rowbytes and screen_frame_stride must be 4-byte aligned");
+    return warp_into_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped != 0, stream, rgba);
+}
+
+}  // namespace
+
+extern "C" {
+
 int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                        int nframes, void *stream) {
     NEED_DEVICE(ctx);
-    return ctx->dev->warp(d_faces, face_stride, d_out, out_stride, nframes, stream, false)
-               ? BLINKY_OK
-               : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+    return warp_into_view(ctx, d_faces, face_stride, d_out, out_stride, ctx->dev->width(), 0, 0, nframes, false, stream, false);
+}
+
+int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
+                            int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
+    return warp_device_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream, false);
+}
+
+int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
+                                 int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
+    return warp_device_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream, true);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,
@@ -415,9 +459,7 @@ int blinky_set_rgba_table(blinky_ctx *ctx, const uint32_t table[256]) {
 int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                             int nframes, void *stream) {
     NEED_DEVICE(ctx);
-    return ctx->dev->warp(d_faces, face_stride, d_out, out_stride, nframes, stream, true)
-               ? BLINKY_OK
-               : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+    return warp_into_view(ctx, d_faces, face_stride, d_out, out_stride, ctx->dev->width() * 4, 0, 0, nframes, false, stream, true);
 }
 
 int64_t blinky_launch_count(blinky_ctx *ctx) { return ctx->dev ? ctx->dev->launches() : 0; }

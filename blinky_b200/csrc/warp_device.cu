@@ -19,6 +19,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <stdexcept>
+#include <type_traits>
 
 #include "../../include/blinky_b200.h"
 #include "tile_plan.h"
@@ -39,10 +40,13 @@ struct WarpParams {
     const uint32_t *bg32;       // background, 4 pixels per element (padded like the lensmap)
     const uint8_t *lut;         // [6][256] rubix tint LUTs
     const uint32_t *rgba;       // [256] palette expansion table (RGBA mode)
-    void *out;                  // frame 0
+    void *out;                  // view origin of frame 0
     size_t out_stride;          // bytes between frames
     uint32_t nquads;            // ceil(W*H / 4)
     uint32_t npix;              // W*H
+    uint32_t width;             // W
+    uint32_t out_pitch;         // bytes between output rows
+    bool pitched;               // out_pitch != W * bytes per pixel: rows are addressed one by one
 };
 
 __device__ __forceinline__ uint4 ld_lensmap(const uint4 *p) {
@@ -69,13 +73,40 @@ __device__ __forceinline__ void st_stream_v4(uint4 *p, uint4 v) {
     asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
+__device__ __forceinline__ void st_stream_u8(uint8_t *p, uint32_t v) {
+    asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// keep_unmapped: the mapped pixels of a partly mapped quad, one store each (a byte, or an RGBA word), so the
+// caller's other pixels are never read or rewritten — another writer may own them (neighbouring view rectangles
+// of one screen, warped concurrently).  px: the four output values, valid4: bit k = pixel k is mapped.
+template <bool RGBA>
+__device__ __forceinline__ void st_quad_masked(uint8_t *dst, const uint32_t (&px)[4], uint32_t valid4) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (!((valid4 >> k) & 1u)) continue;
+        if (RGBA) st_stream_u32(reinterpret_cast<uint32_t *>(dst + 4 * k), px[k]);
+        else st_stream_u8(dst + k, px[k]);
+    }
+}
+
+// byte offset of pixel `pix` (dense index y*W + x) in a frame of the output
+__device__ __forceinline__ size_t out_offset(const WarpParams &p, uint32_t pix, uint32_t opx) {
+    if (!p.pitched) return static_cast<size_t>(pix) * opx;
+    const uint32_t y = pix / p.width;
+    return static_cast<size_t>(y) * p.out_pitch + static_cast<size_t>(pix - y * p.width) * opx;
+}
+
 // --------------------------------------------------------------------------
 // K1: direct gather.  grid = (ceil(nquads/1024), nframes), block = 256.
 // Thread t of CTA b owns quads b*1024 + c*256 + t, c = 0..3, so each of the
 // four 128-bit lensmap loads of a warp covers 512 contiguous bytes and each
-// 32-bit output store of a warp covers 128 contiguous bytes.
+// 32-bit output store of a warp covers 128 contiguous bytes.  A pitched output
+// needs W % 4 == 0, so that no quad straddles two rows.
+// KEEP (keep_unmapped): unmapped pixels are not written and the background is
+// never read; a partly mapped quad is stored pixel by pixel.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA>
+template <bool RUBIX, bool RGBA, bool KEEP>
 __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams p) {
     __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
     __shared__ uint32_t s_rgba[RGBA ? 256 : 1];
@@ -113,8 +144,10 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
         if (q >= p.nquads) continue;
         const uint32_t ent[4] = {e[c].x, e[c].y, e[c].z, e[c].w};
         const uint32_t all_valid = ent[0] & ent[1] & ent[2] & ent[3] & BLINKY_LM_VALID;
+        const uint32_t valid4 = (ent[0] >> 31) | ((ent[1] >> 31) << 1) | ((ent[2] >> 31) << 2) | ((ent[3] >> 31) << 3);
+        if (KEEP && valid4 == 0) continue;
         uint32_t bgw = 0;
-        if (!all_valid) bgw = __ldg(p.bg32 + q);
+        if (!KEEP && !all_valid) bgw = __ldg(p.bg32 + q);
         uint32_t px[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -126,28 +159,33 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
             if (!(ent[k] & BLINKY_LM_VALID)) b = (bgw >> (8 * k)) & 0xffu;
             px[k] = b;
         }
+        uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride + out_offset(p, 4 * q, RGBA ? 4 : 1);
         if (RGBA) {
-            uint4 w = make_uint4(s_rgba[px[0]], s_rgba[px[1]], s_rgba[px[2]], s_rgba[px[3]]);
-            uint4 *o = reinterpret_cast<uint4 *>(static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride);
-            st_stream_v4(o + q, w);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) px[k] = s_rgba[px[k]];
+        }
+        if (KEEP && !all_valid) {
+            st_quad_masked<RGBA>(o, px, valid4);
+        } else if (RGBA) {
+            st_stream_v4(reinterpret_cast<uint4 *>(o), make_uint4(px[0], px[1], px[2], px[3]));
         } else {
-            uint32_t w = px[0] | (px[1] << 8) | (px[2] << 16) | (px[3] << 24);
-            uint32_t *o = reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride);
-            st_stream_u32(o + q, w);
+            st_stream_u32(reinterpret_cast<uint32_t *>(o), px[0] | (px[1] << 8) | (px[2] << 16) | (px[3] << 24));
         }
     }
 }
 
 // --------------------------------------------------------------------------
 // K0: scalar kernel, one pixel per thread, byte stores.  Used only when the
-// frame size or the caller's pointers rule out 32-bit stores (W*H % 4 != 0 or
-// unaligned strides) — a correctness path for ragged sizes, not a fast path.
+// frame size or the caller's pointers rule out 32-bit stores (W*H % 4 != 0,
+// unaligned strides, or a view rectangle whose origin or pitch is not a
+// multiple of 4 pixels) — a correctness path for ragged sizes, not a fast path.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA>
+template <bool RUBIX, bool RGBA, bool KEEP>
 __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams p) {
     const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
     if (i >= p.npix) return;
     const uint32_t ent = __ldg(reinterpret_cast<const uint32_t *>(p.lensmap4) + i);
+    if (KEEP && !(ent & BLINKY_LM_VALID)) return;
     const uint8_t *faces = p.faces + static_cast<size_t>(blockIdx.y) * p.face_stride;
     uint32_t b;
     if (ent & BLINKY_LM_VALID) {
@@ -159,9 +197,9 @@ __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams 
     } else {
         b = __ldg(reinterpret_cast<const uint8_t *>(p.bg32) + i);
     }
-    uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride;
-    if (RGBA) reinterpret_cast<uint32_t *>(o)[i] = __ldg(p.rgba + b);
-    else o[i] = static_cast<uint8_t>(b);
+    uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride + out_offset(p, i, RGBA ? 4 : 1);
+    if (RGBA) *reinterpret_cast<uint32_t *>(o) = __ldg(p.rgba + b);
+    else *o = static_cast<uint8_t>(b);
 }
 
 
@@ -198,8 +236,9 @@ struct RingParams {
     const uint8_t *bg;
     const uint8_t *lut;
     const uint32_t *rgba;
-    void *out;
-    size_t out_stride;
+    void *out;              // view origin of frame 0
+    size_t out_stride;      // bytes between frames
+    uint32_t out_pitch;     // PIXELS between output rows (the background and the lensmap stay dense: W per row)
     uint32_t *ticket;       // monotonic counter (never reset: see launch_ring)
     uint32_t ticket_base;   // its value when this launch starts
     uint32_t nstatic;       // units per warp that are assigned statically (warp w owns w, w+NW, ...) before it draws tickets
@@ -319,7 +358,7 @@ __device__ __forceinline__ void st_stream_u32x8(const uint64_t (&a)[8], const ui
 // vacate at the end.
 constexpr int kGatherRows = 8, kGatherFrames = 4;
 
-template <bool RUBIX, bool RGBA>
+template <bool RUBIX, bool RGBA, bool KEEP>
 __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, uint32_t lane) {
     const uint32_t nfg = (p.nframes + kGatherFrames - 1) / kGatherFrames;
     const uint32_t fg = item % nfg, rest = item / nfg;
@@ -349,7 +388,9 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
     for (int j = 0; j < kGatherRows; ++j) {
         const uint32_t y = tile_y + j;
         if (y >= height) break;
-        const size_t pix = static_cast<size_t>(y) * width + x;
+        if (KEEP && !(e[j] & BLINKY_LM_VALID)) continue;
+        const size_t pix = static_cast<size_t>(y) * width + x;         // background index
+        const size_t opix = static_cast<size_t>(y) * p.out_pitch + x;  // output index
         uint32_t bgv = 0, t = BLINKY_LM_TINT_NONE;
         if (!(e[j] & BLINKY_LM_VALID)) bgv = __ldg(p.bg + pix);
         else if (RUBIX) t = (e[j] >> BLINKY_LM_TINT_SHIFT) & 7u;
@@ -359,8 +400,8 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
             uint32_t b = v[g][j] & 0x100u ? bgv : v[g][j];
             if (RUBIX && t != BLINKY_LM_TINT_NONE) b = __ldg(p.lut + t * 256 + b);
             uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(f0 + g) * p.out_stride;
-            if (RGBA) reinterpret_cast<uint32_t *>(o)[pix] = __ldg(p.rgba + b);
-            else o[pix] = static_cast<uint8_t>(b);
+            if (RGBA) reinterpret_cast<uint32_t *>(o)[opix] = __ldg(p.rgba + b);
+            else o[opix] = static_cast<uint8_t>(b);
         }
     }
 }
@@ -370,14 +411,16 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
 // decided in launch_ring.
 constexpr int kRingMinBlocks = 16;
 
-template <bool RUBIX, bool RGBA>
+// KEEP (keep_unmapped): only mapped pixels are written.  The host gives this instance the BOX tiles alone (EMPTY tiles
+// have nothing to write); a partly mapped quad is stored pixel by pixel and the background is never read.
+template <bool RUBIX, bool RGBA, bool KEEP>
 __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // XOR with a parameter that is always zero: keeps ptxas from re-reading the special register
     // (S2R, tens of cycles) at every `lane == 0` test instead of holding the lane number in a register
     const uint32_t lane = threadIdx.x ^ p.zero;
     if (blockIdx.x >= p.ring_grid) {   // the CTAs behind the ring warps: one gather item each
-        gather_item<RUBIX, RGBA>(p, blockIdx.x - p.ring_grid, lane);
+        gather_item<RUBIX, RGBA, KEEP>(p, blockIdx.x - p.ring_grid, lane);
         return;
     }
     const uint32_t R = p.ring_bytes;
@@ -571,8 +614,8 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
             // pixels of quad q (0..7): row (lane>>3) + 4q, columns 4*(lane&7) .. +3
             const uint32_t qx = tile_x + 4u * (lane & 7u), qy = tile_y + (lane >> 3);
             const size_t opx = RGBA ? 4 : 1;
-            uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(A.f0) * p.out_stride + (static_cast<size_t>(qy) * width + qx) * opx;
-            const uint32_t row4 = width * 4u * static_cast<uint32_t>(opx);   // four screen rows, bytes
+            uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(A.f0) * p.out_stride + (static_cast<size_t>(qy) * p.out_pitch + qx) * opx;
+            const uint32_t row4 = p.out_pitch * 4u * static_cast<uint32_t>(opx);   // four screen rows, bytes
 
             // one frame: wait for its box, 32 byte loads from shared memory, pack, hand the stage on
             auto gather_frame = [&](uint32_t (&w)[8]) {
@@ -636,9 +679,9 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                     vmask[q] = m;
                     const uint32_t y = qy + 4u * q;
                     bgw[q] = 0;
-                    if (qx < width && y < height) {
+                    if (qx < width && y < height && (!KEEP || m != 0)) {   // (KEEP: an unmapped quad is skipped)
                         store_mask |= 1u << q;
-                        if (m != 0xffffffffu) bgw[q] = __ldg(reinterpret_cast<const uint32_t *>(p.bg + static_cast<size_t>(y) * width + qx)) & ~m;
+                        if (!KEEP && m != 0xffffffffu) bgw[q] = __ldg(reinterpret_cast<const uint32_t *>(p.bg + static_cast<size_t>(y) * width + qx)) & ~m;
                     }
                 }
                 for (uint32_t f = 0; f < A.nf; ++f) {
@@ -647,15 +690,24 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
 #pragma unroll
                     for (int q = 0; q < 8; ++q) {
                         if (!((store_mask >> q) & 1u)) continue;
-                        const uint32_t v = (w[q] & vmask[q]) | bgw[q];
                         uint8_t *dst = o + static_cast<size_t>(static_cast<uint32_t>(q) * row4);
+                        if (KEEP && vmask[q] != 0xffffffffu) {
+                            // partly mapped quad: its mapped pixels one by one
+                            uint32_t px[4];
+#pragma unroll
+                            for (int k = 0; k < 4; ++k) px[k] = RGBA ? s_rgba[(w[q] >> (8 * k)) & 0xffu] : (w[q] >> (8 * k)) & 0xffu;
+                            const uint32_t m = vmask[q];
+                            st_quad_masked<RGBA>(dst, px, (m & 1u) | ((m >> 7) & 2u) | ((m >> 14) & 4u) | ((m >> 21) & 8u));
+                            continue;
+                        }
+                        const uint32_t v = (w[q] & vmask[q]) | bgw[q];
                         if (RGBA) store_rgba(dst, v);
                         else st_stream_u32(reinterpret_cast<uint32_t *>(dst), v);
                     }
                     o += p.out_stride;
                 }
             }
-        } else {
+        } else if (!KEEP) {
             // ---- EMPTY: background only (quad layout)
             const uint32_t qx = tile_x + 4u * (lane & 7u), qy = tile_y + (lane >> 3);
             if (qx < width) {
@@ -665,11 +717,12 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                     if (y >= height) break;
                     const size_t pix = static_cast<size_t>(y) * width + qx;
                     const uint32_t v = __ldg(reinterpret_cast<const uint32_t *>(p.bg + pix));
+                    const size_t opix = static_cast<size_t>(y) * p.out_pitch + qx;
                     for (uint32_t f = 0; f < A.nf; ++f) {
                         uint8_t *out_frame = static_cast<uint8_t *>(p.out) + static_cast<size_t>(A.f0 + f) * p.out_stride;
-                        if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(out_frame) + (pix >> 2),
+                        if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(out_frame) + (opix >> 2),
                                                make_uint4(s_rgba[v & 0xffu], s_rgba[(v >> 8) & 0xffu], s_rgba[(v >> 16) & 0xffu], s_rgba[v >> 24]));
-                        else st_stream_u32(reinterpret_cast<uint32_t *>(out_frame) + (pix >> 2), v);
+                        else st_stream_u32(reinterpret_cast<uint32_t *>(out_frame) + (opix >> 2), v);
                     }
                 }
             }
@@ -699,7 +752,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
 // --------------------------------------------------------------------------
 constexpr int kGatherFramesPerCta = 4;
 
-template <bool RUBIX, bool RGBA>
+template <bool RUBIX, bool RGBA, bool KEEP>
 __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid_constant__ RingParams p, const uint32_t first_tile) {
     const uint32_t tid = threadIdx.x;
     const uint4 d = __ldg(reinterpret_cast<const uint4 *>(p.tiles + first_tile + blockIdx.x));
@@ -710,16 +763,18 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
     const uint32_t f1 = min(f0 + kGatherFramesPerCta, p.nframes);
 
     if (type == TILE_EMPTY) {
+        if (KEEP) return;   // nothing mapped, nothing to write
         // quad layout: thread t copies 4 background pixels of row t/8
         const uint32_t x = tile_x + (tid & 7u) * 4u, y = tile_y + (tid >> 3);
         if (x >= width || y >= height) return;
         const size_t pix = static_cast<size_t>(y) * width + x;
         const uint32_t bgw = __ldg(reinterpret_cast<const uint32_t *>(p.bg + pix));
         const uint32_t px[4] = {bgw & 0xffu, (bgw >> 8) & 0xffu, (bgw >> 16) & 0xffu, bgw >> 24};
+        const size_t opix = static_cast<size_t>(y) * p.out_pitch + x;
         for (uint32_t f = f0; f < f1; ++f) {
             uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(f) * p.out_stride;
-            if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(o) + (pix >> 2), make_uint4(__ldg(p.rgba + px[0]), __ldg(p.rgba + px[1]), __ldg(p.rgba + px[2]), __ldg(p.rgba + px[3])));
-            else st_stream_u32(reinterpret_cast<uint32_t *>(o) + (pix >> 2), bgw);
+            if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(o) + (opix >> 2), make_uint4(__ldg(p.rgba + px[0]), __ldg(p.rgba + px[1]), __ldg(p.rgba + px[2]), __ldg(p.rgba + px[3])));
+            else st_stream_u32(reinterpret_cast<uint32_t *>(o) + (opix >> 2), bgw);
         }
         return;
     }
@@ -735,7 +790,7 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
     for (int j = 0; j < 4; ++j) {
         const uint32_t y = tile_y + warp * 4 + j;
         bgv[j] = 0;
-        if (!(e[j] & BLINKY_LM_VALID) && y < height) bgv[j] = __ldg(p.bg + static_cast<size_t>(y) * width + x);
+        if (!KEEP && !(e[j] & BLINKY_LM_VALID) && y < height) bgv[j] = __ldg(p.bg + static_cast<size_t>(y) * width + x);
     }
     uint32_t v[kGatherFramesPerCta][4];
 #pragma unroll
@@ -756,13 +811,13 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const uint32_t y = tile_y + warp * 4 + j;
-            if (y < height) {
+            if (y < height && (!KEEP || (e[j] & BLINKY_LM_VALID))) {
                 uint32_t b = v[g][j];
                 if (RUBIX && (e[j] & BLINKY_LM_VALID)) {
                     const uint32_t t = (e[j] >> BLINKY_LM_TINT_SHIFT) & 7u;
                     if (t != BLINKY_LM_TINT_NONE) b = __ldg(p.lut + t * 256 + b);
                 }
-                const size_t pix = static_cast<size_t>(y) * width + x;
+                const size_t pix = static_cast<size_t>(y) * p.out_pitch + x;
                 if (RGBA) reinterpret_cast<uint32_t *>(o)[pix] = __ldg(p.rgba + b);
                 else o[pix] = static_cast<uint8_t>(b);
             }
@@ -963,7 +1018,7 @@ bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
 }
 
 bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                      bool rgba) {
+                      bool rgba, size_t out_pitch, bool keep_unmapped) {
     if (!have_lensmap_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
         return false;
@@ -974,16 +1029,24 @@ bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size
         return false;
     }
     const size_t opx = rgba ? 4 : 1;
-    if (rgba && (reinterpret_cast<uintptr_t>(d_out) % 4 != 0 || (nframes > 1 && out_stride % 4 != 0))) {
-        err_ = "warp (RGBA): the output buffer and the frame stride must be 4-byte aligned";
+    if (rgba && (reinterpret_cast<uintptr_t>(d_out) % 4 != 0 || out_pitch % 4 != 0 || (nframes > 1 && out_stride % 4 != 0))) {
+        err_ = "warp (RGBA): the output buffer, the row pitch and the frame stride must be 4-byte aligned";
         return false;
     }
-    // the tiled kernel writes 4-pixel words at (y*W + x): needs W % 4 == 0 and aligned frames
-    const bool tiled_ok = have_plan_ && (width_ % 4 == 0) && (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) &&
-                          (out_stride % (4 * opx) == 0 || nframes == 1) &&
+    const size_t pitch = out_pitch ? out_pitch : static_cast<size_t>(width_) * opx;
+    if (pitch < static_cast<size_t>(width_) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
+        err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
+        return false;
+    }
+    // 4-pixel words (the ring kernel, the flat kernel's vector stores): W % 4 == 0 and the view's origin, pitch and frame
+    // stride aligned to 4 pixels
+    const bool vec_ok = (width_ % 4 == 0) && (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (pitch % (4 * opx) == 0) &&
+                        (out_stride % (4 * opx) == 0 || nframes == 1);
+    const bool tiled_ok = have_plan_ && vec_ok &&
                           (!plan_has_box_ || (reinterpret_cast<uintptr_t>(d_faces) % 16 == 0 && (face_stride % 16 == 0 || nframes == 1)));
-    if (variant_ == BLINKY_KERNEL_GATHER || !tiled_ok) return launch_flat(d_faces, face_stride, d_out, out_stride, nframes, stream, rgba);
-    return launch_ring(d_faces, face_stride, d_out, out_stride, nframes, stream, rgba);
+    if (variant_ == BLINKY_KERNEL_GATHER || !tiled_ok)
+        return launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped);
+    return launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped);
 }
 
 WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stride, int nframes) {
@@ -1045,29 +1108,31 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
 
-template <bool RUBIX, bool RGBA>
-static cudaError_t ring_config(size_t smem, int *ctas_per_sm) {
-    cudaError_t e = cudaFuncSetAttribute(warp_ring_kernel<RUBIX, RGBA>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, warp_ring_kernel<RUBIX, RGBA>, 32, smem);
+// Calls f(R, C, K) with std::bool_constant arguments for (rubix, rgba, keep): one place turns the run-time flags into
+// the kernels' template arguments.
+template <typename F>
+static auto with_variant(bool rubix, bool rgba, bool keep, F &&f) {
+    using T = std::true_type;
+    using N = std::false_type;
+    if (rubix) {
+        if (rgba) return keep ? f(T{}, T{}, T{}) : f(T{}, T{}, N{});
+        return keep ? f(T{}, N{}, T{}) : f(T{}, N{}, N{});
+    }
+    if (rgba) return keep ? f(N{}, T{}, T{}) : f(N{}, T{}, N{});
+    return keep ? f(N{}, N{}, T{}) : f(N{}, N{}, N{});
 }
 
-static cudaError_t ring_config_v(bool rubix, bool rgba, size_t smem, int *n) {
-    return rubix && rgba ? ring_config<true, true>(smem, n)
-           : rubix       ? ring_config<true, false>(smem, n)
-           : rgba        ? ring_config<false, true>(smem, n)
-                         : ring_config<false, false>(smem, n);
+static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, size_t smem, int *n) {
+    return with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
+        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value>;
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+        if (e != cudaSuccess) return e;
+        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(n, kernel, 32, smem);
+    });
 }
 
-static void ring_launch_v(bool rubix, bool rgba, uint32_t grid, size_t smem, cudaStream_t st, const RingParams &p, const RingTmaps &tm) {
-    if (rubix && rgba) warp_ring_kernel<true, true><<<grid, 32, smem, st>>>(p, tm);
-    else if (rubix) warp_ring_kernel<true, false><<<grid, 32, smem, st>>>(p, tm);
-    else if (rgba) warp_ring_kernel<false, true><<<grid, 32, smem, st>>>(p, tm);
-    else warp_ring_kernel<false, false><<<grid, 32, smem, st>>>(p, tm);
-}
-
-bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes,
-                             void *stream, bool rgba) {
+bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
+                             void *stream, bool rgba, bool keep) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     RingParams p;
     p.tiles = static_cast<const TileDesc *>(d_tiles_);
@@ -1086,6 +1151,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.rgba = d_rgba_;
     p.out = d_out;
     p.out_stride = out_stride;
+    p.out_pitch = out_pitch / (rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
     p.nbox = nbox_tiles_;
     p.ngather = ngather_tiles_;
     p.ntiles = ntiles_;
@@ -1094,12 +1160,13 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.height = height_;
     p.zero = 0;
     const bool rubix = rubix_;
-    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0);
+    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0);
     // The ring kernel takes the BOX tiles [0, nbox) and the EMPTY tiles; the GATHER tiles in between go to the
     // gather kernel K3 on the context's side stream (forked from and joined to the caller's stream), so the two
-    // kernels share the GPU instead of queueing behind each other.
+    // kernels share the GPU instead of queueing behind each other.  With keep_unmapped an EMPTY tile has nothing
+    // to write: the ring kernel's units are the BOX tiles alone.
     const uint32_t nempty = ntiles_ - nbox_tiles_ - ngather_tiles_;
-    const uint32_t ring_tiles = nbox_tiles_ + nempty;
+    const uint32_t ring_tiles = nbox_tiles_ + (keep ? 0u : nempty);
     // Ring geometry: as many warps per SM as the registers allow (or BLINKY_RING_CTAS), each with the largest
     // staging ring that still lets that many CTAs share the SM's shared memory; fewer warps if the plan's
     // largest box would not fit such a ring.
@@ -1138,7 +1205,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     const size_t smem = static_cast<size_t>(ring_bytes) + fixed;
     if (ring_ctas_per_sm_[vi] == 0 || ring_smem_[vi] != smem) {
         int n = 0;
-        cudaError_t e = ring_config_v(rubix, rgba, smem, &n);
+        cudaError_t e = ring_config_v(rubix, rgba, keep, smem, &n);
         if (e != cudaSuccess) return fail("ring kernel configuration (shared memory / occupancy)", e);
         if (n < 1) {
             err_ = "ring kernel does not fit on an SM";
@@ -1171,17 +1238,17 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     if (grid > p.nunits) grid = p.nunits;
     char buf[640];
     int nbuf = 0;
+    const char *keep_tag = keep ? ",keep=1" : "";
     // GATHER tiles: one-warp CTAs behind the ring warps in the same grid (see gather_item); only a plan without BOX and
-    // EMPTY tiles launches the stand-alone gather kernel.
-    buf[0] = 0;
+    // EMPTY tiles (with keep_unmapped: without BOX tiles) launches the stand-alone gather kernel.
+    snprintf(buf, sizeof buf, "%s", ngather_tiles_ == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
     if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
         dim3 g2(ngather_tiles_, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
-        if (rubix && rgba) warp_tile_gather_kernel<true, true><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
-        else if (rubix) warp_tile_gather_kernel<true, false><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
-        else if (rgba) warp_tile_gather_kernel<false, true><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
-        else warp_tile_gather_kernel<false, false><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
+        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
+            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
+        });
         ++launches_;
-        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d> grid=(%u,%u) block=%d", rubix, rgba, g2.x, g2.y, kThreads);
+        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, g2.x, g2.y, kThreads);
     }
     if (grid > 0) {
         // ticket counter of this stream (launches on one stream are serialised; the counter is never reset:
@@ -1222,21 +1289,23 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
 
         p.ring_grid = grid;
         const uint32_t extra = merged_gather ? gather_items : 0u;
-        ring_launch_v(rubix, rgba, grid + extra, smem, st, p, *tm);
+        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
+            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid + extra, 32, smem, st>>>(p, *tm);
+        });
         ++launches_;
         nbuf = static_cast<int>(strlen(buf));
         snprintf(buf + nbuf, sizeof buf - static_cast<size_t>(nbuf),
-                 "%swarp_ring_kernel<rubix=%d,rgba=%d> grid=%u+%u block=32 (%d ring warps/SM, TMA box ring of %u B, <=%u boxes in flight, %u frames/unit, %u units; "
+                 "%swarp_ring_kernel<rubix=%d,rgba=%d%s> grid=%u+%u block=32 (%d ring warps/SM, TMA box ring of %u B, <=%u boxes in flight, %u frames/unit, %u units; "
                  "%u gather CTAs of %dx32 px x %d frames)",
-                 nbuf ? " + " : "", rubix, rgba, grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows, kGatherFrames);
+                 nbuf ? " + " : "", rubix, rgba, keep_tag, grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows, kGatherFrames);
     }
     last_kernel_ = buf;
     CK(cudaGetLastError());
     return true;
 }
 
-bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                             bool rgba) {
+bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
+                             void *stream, bool rgba, bool keep) {
     // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out
     // unless the caller made its own) — NOT this context's private stream.
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1251,30 +1320,31 @@ bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_ou
     p.out_stride = out_stride;
     p.nquads = static_cast<uint32_t>((npix_ + 3) / 4);
     p.npix = static_cast<uint32_t>(npix_);
+    p.width = static_cast<uint32_t>(width_);
+    p.out_pitch = out_pitch;
 
     const size_t opx = rgba ? 4 : 1;  // output bytes per pixel
-    const bool vector_ok = (npix_ % 4 == 0) && (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) &&
-                           (out_stride % (4 * opx) == 0 || nframes == 1);
+    p.pitched = out_pitch != static_cast<size_t>(width_) * opx;
+    // 4-pixel words: dense frames need W*H % 4 == 0, pitched ones W % 4 == 0 (no quad straddles two rows)
+    const bool vector_ok = (p.pitched ? width_ % 4 == 0 && out_pitch % (4 * opx) == 0 : npix_ % 4 == 0) &&
+                           (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (out_stride % (4 * opx) == 0 || nframes == 1);
     const bool rubix = rubix_;
+    const char *keep_tag = keep ? ",keep=1" : "";
+    char buf[160];
     if (vector_ok) {
         dim3 grid(static_cast<unsigned>(npix_pad_ / kPixelsPerBlock), static_cast<unsigned>(nframes));
-        if (rubix && rgba) warp_gather_kernel<true, true><<<grid, kThreads, 0, st>>>(p);
-        else if (rubix) warp_gather_kernel<true, false><<<grid, kThreads, 0, st>>>(p);
-        else if (rgba) warp_gather_kernel<false, true><<<grid, kThreads, 0, st>>>(p);
-        else warp_gather_kernel<false, false><<<grid, kThreads, 0, st>>>(p);
-        char buf[160];
-        snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d> grid=(%u,%u) block=%d", rubix, rgba, grid.x, grid.y, kThreads);
-        last_kernel_ = buf;
+        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
+            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid, kThreads, 0, st>>>(p);
+        });
+        snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, grid.x, grid.y, kThreads);
     } else {
         dim3 grid(static_cast<unsigned>((npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(nframes));
-        if (rubix && rgba) warp_scalar_kernel<true, true><<<grid, kThreads, 0, st>>>(p);
-        else if (rubix) warp_scalar_kernel<true, false><<<grid, kThreads, 0, st>>>(p);
-        else if (rgba) warp_scalar_kernel<false, true><<<grid, kThreads, 0, st>>>(p);
-        else warp_scalar_kernel<false, false><<<grid, kThreads, 0, st>>>(p);
-        char buf[160];
-        snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d> grid=(%u,%u) block=%d", rubix, rgba, grid.x, grid.y, kThreads);
-        last_kernel_ = buf;
+        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
+            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid, kThreads, 0, st>>>(p);
+        });
+        snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, grid.x, grid.y, kThreads);
     }
+    last_kernel_ = buf;
     ++launches_;
     CK(cudaGetLastError());
     return true;

@@ -43,9 +43,15 @@ public:
     bool set_rgba_table(const uint32_t table[256]);
     void set_kernel(int variant) { variant_ = variant; }
 
-    // device-resident batch (asynchronous on `stream`, nullptr = CUDA default stream)
+    // size of the resident lensmap's view (0 before the first upload)
+    int width() const { return width_; }
+    int height() const { return height_; }
+
+    // device-resident batch (asynchronous on `stream`, nullptr = CUDA default stream).  d_out is the view origin of
+    // frame 0; rows are out_pitch bytes apart (0: dense, W * bytes per pixel).  keep_unmapped: only mapped pixels
+    // are written, the others keep what the caller's buffer holds.
     bool warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-              bool rgba);
+              bool rgba, size_t out_pitch = 0, bool keep_unmapped = false);
     // end to end from host buffers (synchronous)
     bool warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
                    int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped);
@@ -116,13 +122,13 @@ private:
     uint64_t tmap_tick_ = 0;
     std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
-    int ring_ctas_per_sm_[4] = {0, 0, 0, 0};
-    size_t ring_smem_[4] = {0, 0, 0, 0};
+    int ring_ctas_per_sm_[8] = {};       // per ring kernel instance: rubix | rgba << 1 | keep << 2
+    size_t ring_smem_[8] = {};
     TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes);
-    bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                     bool rgba);
-    bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                     bool rgba);
+    bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
+                     void *stream, bool rgba, bool keep);
+    bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
+                     void *stream, bool rgba, bool keep);
     std::string plan_summary_;
 public:
     const std::string &plan_summary() const { return plan_summary_; }

@@ -207,6 +207,24 @@ int blinky_set_background(blinky_ctx *ctx, const uint8_t *background_host);
 int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                        int nframes, void *stream);
 
+/* Device-resident batch into a view rectangle of a device framebuffer (scr_vrect, VBUFFER :634).
+ * d_screen: nframes screens, frame stride screen_frame_stride bytes, rows of rowbytes bytes; the
+ * width x height view starts at pixel (x0, y0).  keep_unmapped != 0: only mapped pixels are written
+ * (:2413); otherwise unmapped pixels of the rectangle get the background.  Nothing outside the
+ * rectangle is written, and no pixel is read back and rewritten: unmapped pixels are skipped with
+ * byte (RGBA: 32-bit) stores, so other writers may fill neighbouring rectangles of the same screen at
+ * the same time, from other contexts and streams.  Asynchronous on `stream`, like blinky_warp_device.
+ * Fails with BLINKY_E_INVALID, launching nothing, for a NULL buffer, x0 < 0 or y0 < 0,
+ * rowbytes < (x0 + width) * bytes per pixel, or nframes > 1 with
+ * screen_frame_stride < (y0 + height) * rowbytes.  Views whose width, origin, rowbytes and frame
+ * stride are multiples of 4 pixels take the fast kernels; any other view is warped pixel by pixel.
+ * Known limitation, shared with every blinky_warp_device* call: not capturable in a CUDA graph.  The
+ * ring kernel draws work tickets from a per-stream counter that is never reset, and each launch is
+ * given the counter's value at its start; a replayed graph would reuse a stale value. */
+int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen,
+                            size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                            int keep_unmapped, void *stream);
+
 /* End to end from HOST buffers: pinned-staged cudaMemcpyAsync of each frame's
  * displayed plates, the warp, and the copy back, software-pipelined over
  * internal streams.  faces_host: nframes x [numplates][ps][ps].  dst_host: nframes
@@ -275,6 +293,12 @@ int blinky_shard_close(blinky_ctx *ctx);
 int blinky_set_rgba_table(blinky_ctx *ctx, const uint32_t table[256]);
 int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out_rgba,
                             size_t out_stride, int nframes, void *stream);
+/* blinky_warp_device_view with one uint32 per pixel through the blinky_set_rgba_table table: rowbytes
+ * and screen_frame_stride in bytes, x0 in pixels.  The view origin, rowbytes and (nframes > 1) the
+ * frame stride must be 4-byte aligned, else BLINKY_E_INVALID. */
+int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen_rgba,
+                                 size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                                 int keep_unmapped, void *stream);
 
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
