@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import sys
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint8, c_uint32, c_void_p
 
 import numpy as np
@@ -109,6 +110,7 @@ _SIGNATURES = [
     ("blinky_ipc_open", c_int, [_CTX, c_void_p, POINTER(c_void_p)]),
     ("blinky_ipc_close", c_int, [_CTX, c_void_p]),
     ("blinky_sync", c_int, [_CTX]),
+    ("blinky_release_captures", c_int, [_CTX]),
     ("blinky_set_rgba_table", c_int, [_CTX, c_void_p]),
     ("blinky_warp_device_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p]),
     ("blinky_plan_summary", c_char_p, [_CTX]),
@@ -165,6 +167,16 @@ def _ptr(a) -> int:
     if hasattr(a, "data_ptr"):
         return a.data_ptr()
     raise TypeError(f"cannot take the address of {type(a)}")
+
+
+def _warp_stream(stream):
+    """stream=None is CUDA's legacy default stream, which cannot be captured: while torch captures on its current
+    stream (torch.cuda.graph), a warp goes to that stream instead"""
+    if stream is None:
+        torch = sys.modules.get("torch")
+        if torch is not None and torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():
+            return torch.cuda.current_stream().cuda_stream
+    return stream
 
 
 class Fisheye:
@@ -390,14 +402,15 @@ class Fisheye:
 
     def warp(self, d_faces, d_out, nframes: int = 1, face_stride: int | None = None, out_stride: int | None = None,
              stream: int | None = None, rgba: bool = False):
-        """device-resident batch; d_faces/d_out are torch CUDA tensors (or raw device addresses)."""
+        """device-resident batch; d_faces/d_out are torch CUDA tensors (or raw device addresses).  May be captured
+        into a CUDA graph (torch.cuda.graph; see release_captures)."""
         ps2 = self.platesize * self.platesize
         if face_stride is None:
             face_stride = self.numplates * ps2
         if out_stride is None:
             out_stride = self.width * self.height * (4 if rgba else 1)
         fn = self._lib.blinky_warp_device_rgba if rgba else self._lib.blinky_warp_device
-        self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_out), out_stride, nframes, stream))
+        self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_out), out_stride, nframes, _warp_stream(stream)))
 
     def warp_view(self, d_faces, d_screen, x0: int = 0, y0: int = 0, rowbytes: int | None = None, nframes: int = 1,
                   keep_unmapped: bool = False, rgba: bool = False, face_stride: int | None = None,
@@ -416,7 +429,12 @@ class Fisheye:
                              else (y0 + self.height) * rowbytes)
         fn = self._lib.blinky_warp_device_view_rgba if rgba else self._lib.blinky_warp_device_view
         self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_screen), screen_stride, rowbytes, x0, y0, nframes,
-                       1 if keep_unmapped else 0, stream))
+                       1 if keep_unmapped else 0, _warp_stream(stream)))
+
+    def release_captures(self):
+        """No CUDA graph that captured a warp of this context will run again (blinky_release_captures): frees the
+        lensmap buffers rebuilds kept for such graphs and returns their work counters.  Synchronises the device."""
+        self._check(self._lib.blinky_release_captures(self._ctx))
 
     def warp_host(self, faces: np.ndarray, dst: np.ndarray | None = None, keep_unmapped: bool = False, x0: int = 0,
                   y0: int = 0, nframes: int | None = None, dst_rowbytes: int | None = None,

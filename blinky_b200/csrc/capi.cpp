@@ -358,7 +358,7 @@ int warp_into_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, voi
     uint8_t *origin = static_cast<uint8_t *>(d_screen) + static_cast<size_t>(y0) * static_cast<size_t>(rowbytes) + static_cast<size_t>(x0) * bpp;
     return ctx->dev->warp(d_faces, face_stride, origin, screen_frame_stride, nframes, stream, rgba, static_cast<size_t>(rowbytes), keep_unmapped)
                ? BLINKY_OK
-               : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+               : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
@@ -449,6 +449,10 @@ int blinky_ipc_close(blinky_ctx *ctx, void *peer_ptr) {
 int blinky_sync(blinky_ctx *ctx) {
     NEED_DEVICE(ctx);
     return ctx->dev->sync() ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+}
+int blinky_release_captures(blinky_ctx *ctx) {
+    NEED_DEVICE(ctx);
+    return ctx->dev->release_captures() ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int blinky_set_rgba_table(blinky_ctx *ctx, const uint32_t table[256]) {

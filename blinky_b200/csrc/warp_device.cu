@@ -239,8 +239,8 @@ struct RingParams {
     void *out;              // view origin of frame 0
     size_t out_stride;      // bytes between frames
     uint32_t out_pitch;     // PIXELS between output rows (the background and the lensmap stay dense: W per row)
-    uint32_t *ticket;       // monotonic counter (never reset: see launch_ring)
-    uint32_t ticket_base;   // its value when this launch starts
+    uint32_t *ticket;       // work counter: 0 when the launch starts, set back to 0 by its last draw (see ticket_drawn)
+    uint32_t ndraws;        // counter draws the launch makes (see launch_ring)
     uint32_t nstatic;       // units per warp that are assigned statically (warp w owns w, w+NW, ...) before it draws tickets
     uint32_t nbox, ngather, ntiles;
     uint32_t nframes, fchunk, nchunks, nunits;
@@ -406,6 +406,15 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
     }
 }
 
+// A dynamic ticket has been drawn: `d` is the counter value the warp received (warp-uniform).  Draws on one address
+// are totally ordered and a launch makes exactly p.ndraws of them from 0, so the warp that receives ndraws - 1 makes
+// the launch's last draw, and it stores 0: the next launch on the counter (stream order, or the next replay of a
+// graph) starts from 0 without the host knowing what the counter holds.  Returns the unit index.
+__device__ __forceinline__ uint32_t ticket_drawn(const RingParams &p, uint32_t d, uint32_t nw, uint32_t lane) {
+    if (d == p.ndraws - 1u && lane == 0) asm volatile("st.relaxed.gpu.global.u32 [%0], 0;" ::"l"(p.ticket) : "memory");
+    return p.nstatic * nw + d;
+}
+
 // CTAs per SM the ring kernel's register allocation is sized for, ring warps plus the gather CTAs beside them:
 // 128 registers per thread (the BOX path uses 96, 116 with the rubix overlay).  How many ring warps are resident is
 // decided in launch_ring.
@@ -468,7 +477,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
     // launch is handed out through the ticket counter.  Mostly static because one counter serves the
     // whole GPU and same-address atomics serialise; the dynamic tail evens out the finish.
     // A warp draws only while its last known ticket was good, so that the number of draws per launch is
-    // a function of the launch alone (the host advances ticket_base by it).
+    // a function of the launch alone (the host passes it as ndraws).
     uint32_t k_next = 0;        // index of the next ticket of this warp
     bool last_good = true;
     auto draw_now = [&]() {     // the k_next-th ticket, waiting for the counter if it is a dynamic one
@@ -478,7 +487,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
         } else if (last_good) {
             uint32_t d = 0;
             if (lane == 0) asm volatile("atom.global.add.u32 %0, [%1], 1;" : "=r"(d) : "l"(p.ticket) : "memory");
-            t = p.nstatic * NW + (__shfl_sync(0xffffffffu, d, 0) - p.ticket_base);
+            t = ticket_drawn(p, __shfl_sync(0xffffffffu, d, 0), NW, lane);
         }
         ++k_next;
         last_good = t < p.nunits;
@@ -730,7 +739,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
         // rotate: A <- B <- C <- the ticket drawn above; the cursor moves with its unit
         uint32_t next_ticket = 0xffffffffu;
         if (k_next < p.nstatic) next_ticket = blockIdx.x + k_next * NW;
-        else if (draw_dynamic) next_ticket = p.nstatic * NW + (__shfl_sync(0xffffffffu, drawn, 0) - p.ticket_base);
+        else if (draw_dynamic) next_ticket = ticket_drawn(p, __shfl_sync(0xffffffffu, drawn, 0), NW, lane);
         ++k_next;
         last_good = next_ticket < p.nunits;
         A = B;
@@ -827,6 +836,8 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
+constexpr uint32_t kCaptureSlots = 4096;   // work counters for captured ring launches (see WarpDevice::CaptureStream)
+
 }  // namespace
 
 // ---------------------------------------------------------------------------
@@ -898,6 +909,9 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     if (e == cudaSuccess) e = cudaMemset(d_lut_, 0, 6 * 256);
     if (e == cudaSuccess) e = cudaMalloc(&d_rgba_, 256 * 4);
     if (e == cudaSuccess) e = cudaMemset(d_rgba_, 0, 256 * 4);
+    // (here, not on first use: a capture may allocate nothing)
+    if (e == cudaSuccess) e = cudaMalloc(&d_capture_slots_, kCaptureSlots * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMemset(d_capture_slots_, 0, kCaptureSlots * sizeof(uint32_t));
     if (e != cudaSuccess) throw std::runtime_error(std::string("cudaMalloc: ") + cudaGetErrorString(e));
 }
 
@@ -921,6 +935,8 @@ WarpDevice::~WarpDevice() {
     cudaFree(d_entries_);
     for (TmapSet *t : tmap_sets_) delete t;
     for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
+    cudaFree(d_capture_slots_);
+    for (void *p : retired_) cudaFree(p);
     if (stream_) cudaStreamDestroy(static_cast<cudaStream_t>(stream_));
 }
 
@@ -929,17 +945,25 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
     CK(cudaDeviceSynchronize());  // nothing may still be reading the old map
     const size_t npix = static_cast<size_t>(lm.width) * lm.height;
     const size_t npad = round_up(npix, kPixelsPerBlock);
-    if (npad != npix_pad_) {
-        cudaFree(d_lensmap_);
-        cudaFree(d_bg_);
-        d_lensmap_ = nullptr;
-        d_bg_ = nullptr;
+    // A graph captured since the last upload keeps rendering the lensmap and plan it was captured with: their buffers
+    // are retired instead of freed or rewritten.  The background stays shared while the view size stays the same, so
+    // it is retired when it is replaced and any graph captured since it was allocated reads it.
+    auto drop = [&](auto *&p, bool retire) {
+        if (p && retire) retired_.push_back(p);
+        else cudaFree(p);
+        p = nullptr;
+    };
+    const bool resize = npad != npix_pad_, new_view = resize || lm.width != width_ || lm.height != height_;
+    if (resize || captured_) {
+        drop(d_lensmap_, captured_);
         CK(cudaMalloc(&d_lensmap_, npad * sizeof(uint32_t)));
-        CK(cudaMalloc(&d_bg_, npad));
-        CK(cudaMemset(d_bg_, 0, npad));
-    } else if (lm.width != width_ || lm.height != height_) {
-        CK(cudaMemset(d_bg_, 0, npad));
     }
+    if (resize || (bg_captured_ && new_view)) {
+        drop(d_bg_, bg_captured_);
+        bg_captured_ = false;
+        CK(cudaMalloc(&d_bg_, npad));
+    }
+    if (new_view) CK(cudaMemset(d_bg_, 0, npad));
     // padding entries are "unmapped"
     CK(cudaMemset(d_lensmap_, 0, npad * sizeof(uint32_t)));
     CK(cudaMemcpy(d_lensmap_, lm.packed, npix * sizeof(uint32_t), cudaMemcpyHostToDevice));
@@ -959,10 +983,9 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
     // tiled layout
     have_plan_ = false;
     plan_has_box_ = false;
-    cudaFree(d_tiles_);
-    cudaFree(d_entries_);
-    d_tiles_ = nullptr;
-    d_entries_ = nullptr;
+    drop(d_tiles_, captured_);
+    drop(d_entries_, captured_);
+    captured_ = false;
     for (TmapSet *t : tmap_sets_) delete t;
     tmap_sets_.clear();
     if (lm.plan && !lm.plan->tiles.empty()) {
@@ -1019,6 +1042,7 @@ bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
 
 bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
                       bool rgba, size_t out_pitch, bool keep_unmapped) {
+    err_code_ = BLINKY_E_CUDA;
     if (!have_lensmap_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
         return false;
@@ -1044,9 +1068,52 @@ bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size
                         (out_stride % (4 * opx) == 0 || nframes == 1);
     const bool tiled_ok = have_plan_ && vec_ok &&
                           (!plan_has_box_ || (reinterpret_cast<uintptr_t>(d_faces) % 16 == 0 && (face_stride % 16 == 0 || nframes == 1)));
-    if (variant_ == BLINKY_KERNEL_GATHER || !tiled_ok)
-        return launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped);
-    return launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped);
+    // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    unsigned long long cap_id = 0;
+    if (stream != nullptr && static_cast<cudaStream_t>(stream) != cudaStreamLegacy)
+        CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(stream), &cap, &cap_id));
+    const bool capturing = cap != cudaStreamCaptureStatusNone;
+    const bool ok = variant_ == BLINKY_KERNEL_GATHER || !tiled_ok
+                        ? launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped)
+                        : launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
+                                      capturing);
+    if (capturing) {
+        captured_ = bg_captured_ = true;
+        bool known = false;
+        for (CaptureStream &c : capture_streams_)
+            if (c.stream == stream) c.id = cap_id, known = true;
+        if (!known) capture_streams_.push_back({stream, cap_id});
+    }
+    return ok;
+}
+
+bool WarpDevice::release_captures() {
+    err_code_ = BLINKY_E_CUDA;
+    // a capture that holds a warp of this object and is still open: synchronising now would invalidate it
+    for (const CaptureStream &c : capture_streams_) {
+        cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+        unsigned long long id = 0;
+        if (cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(c.stream), &s, &id) == cudaSuccess && s != cudaStreamCaptureStatusNone &&
+            id == c.id) {
+            err_code_ = BLINKY_E_INVALID;
+            err_ = "release_captures: a stream is still capturing a warp of this context (end the capture first)";
+            return false;
+        }
+    }
+    CK(cudaSetDevice(device_));
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaErrorStreamCaptureUnsupported || e == cudaErrorStreamCaptureImplicit) {
+        err_code_ = BLINKY_E_INVALID;
+        return fail("release_captures: cudaDeviceSynchronize while a stream is capturing", e);
+    }
+    if (e != cudaSuccess) return fail("release_captures: cudaDeviceSynchronize", e);
+    for (void *p : retired_) cudaFree(p);
+    retired_.clear();
+    capture_streams_.clear();
+    capture_slots_used_ = 0;
+    captured_ = bg_captured_ = false;
+    return true;
 }
 
 WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stride, int nframes) {
@@ -1132,7 +1199,7 @@ static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, size_t smem, 
 }
 
 bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep) {
+                             void *stream, bool rgba, bool keep, bool capturing) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     RingParams p;
     p.tiles = static_cast<const TileDesc *>(d_tiles_);
@@ -1236,6 +1303,36 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.nchunks = (p.nframes + fchunk - 1) / fchunk;
     p.nunits = ring_tiles * p.nchunks;
     if (grid > p.nunits) grid = p.nunits;
+    // The ring kernel's work counter, 0 before and after every launch (ticket_drawn).  Eager launches on one stream
+    // run one after the other and share the stream's counter; a captured launch gets a pool slot of its own.  Taken
+    // before anything is launched, so that a capture refused for want of slots launches nothing.
+    if (grid > 0 && capturing) {
+        if (capture_slots_used_ == kCaptureSlots) {
+            err_code_ = BLINKY_E_STATE;
+            err_ = "warp: all 4096 work counters for captured ring kernel launches are in use; call blinky_release_captures "
+                   "once the graphs holding them will not run again";
+            return false;
+        }
+        p.ticket = d_capture_slots_ + capture_slots_used_++;
+    } else if (grid > 0) {
+        TicketCounter *tc = nullptr;
+        for (TicketCounter &c : tickets_)
+            if (c.stream == stream) tc = &c;
+        if (!tc) {
+            if (tickets_.size() >= 64) {  // streams come and go: start over
+                CK(cudaDeviceSynchronize());
+                for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
+                tickets_.clear();
+            }
+            TicketCounter c;
+            c.stream = stream;
+            CK(cudaMalloc(&c.d_counter, sizeof(uint32_t)));
+            CK(cudaMemsetAsync(c.d_counter, 0, sizeof(uint32_t), st));
+            tickets_.push_back(c);
+            tc = &tickets_.back();
+        }
+        p.ticket = tc->d_counter;
+    }
     char buf[640];
     int nbuf = 0;
     const char *keep_tag = keep ? ",keep=1" : "";
@@ -1251,27 +1348,6 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
         snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, g2.x, g2.y, kThreads);
     }
     if (grid > 0) {
-        // ticket counter of this stream (launches on one stream are serialised; the counter is never reset:
-        // the kernel subtracts the value it had when the launch started)
-        TicketCounter *tc = nullptr;
-        for (TicketCounter &c : tickets_)
-            if (c.stream == stream) tc = &c;
-        if (!tc) {
-            if (tickets_.size() >= 64) {  // streams come and go: start over
-                CK(cudaDeviceSynchronize());
-                for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
-                tickets_.clear();
-            }
-            TicketCounter c;
-            c.stream = stream;
-            c.base = 0;
-            CK(cudaMalloc(&c.d_counter, sizeof(uint32_t)));
-            CK(cudaMemsetAsync(c.d_counter, 0, sizeof(uint32_t), st));
-            tickets_.push_back(c);
-            tc = &tickets_.back();
-        }
-        p.ticket = tc->d_counter;
-        p.ticket_base = tc->base;
         // static share of the schedule (see the kernel): static_pct_ percent of the units, whole rounds
         uint32_t nstatic = static_cast<uint32_t>(static_cast<uint64_t>(p.nunits) * static_cast<uint64_t>(static_pct_) / 100u / grid);
         p.nstatic = nstatic;
@@ -1285,7 +1361,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
             const uint64_t before_last = static_cast<uint64_t>(nstatic - 1) * grid;
             drawers = p.nunits > before_last ? static_cast<uint32_t>(std::min<uint64_t>(p.nunits - before_last, grid)) : 0u;
         }
-        tc->base += good + drawers;
+        p.ndraws = good + drawers;
 
         p.ring_grid = grid;
         const uint32_t extra = merged_gather ? gather_items : 0u;

@@ -49,9 +49,15 @@ public:
 
     // device-resident batch (asynchronous on `stream`, nullptr = CUDA default stream).  d_out is the view origin of
     // frame 0; rows are out_pitch bytes apart (0: dense, W * bytes per pixel).  keep_unmapped: only mapped pixels
-    // are written, the others keep what the caller's buffer holds.
+    // are written, the others keep what the caller's buffer holds.  May be captured into a CUDA graph: see
+    // release_captures.
     bool warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
               bool rgba, size_t out_pitch = 0, bool keep_unmapped = false);
+    // The caller will not run again any graph that captured a warp of this object: synchronises the device, frees
+    // the buffers upload_lensmap retired for such graphs and returns every capture counter slot to the pool.
+    bool release_captures();
+    // BLINKY_E_* code of the last failure (BLINKY_E_CUDA unless the call was refused for another reason)
+    int last_error_code() const { return err_code_; }
     // end to end from host buffers (synchronous)
     bool warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
                    int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped);
@@ -82,6 +88,7 @@ private:
     const void *pin_src_ptr_ = nullptr, *pin_dst_ptr_ = nullptr;  // last buffers warp_host saw and whether they are pinned
     bool pin_src_ = false, pin_dst_ = false;
     std::string err_;
+    int err_code_ = 0;
 
     // resident lensmap
     int width_ = 0, height_ = 0, platesize_ = 0, numplates_ = 0;
@@ -102,8 +109,7 @@ private:
     struct TmapSet;
     struct TicketCounter {
         void *stream = nullptr;
-        uint32_t *d_counter = nullptr;
-        uint32_t base = 0;  // value the counter will have when the next launch on this stream starts
+        uint32_t *d_counter = nullptr;  // 0 between launches: each launch sets it back
     };
     bool have_plan_ = false;
     bool plan_has_box_ = false;
@@ -120,15 +126,30 @@ private:
     std::vector<uint16_t> shapes_;
     std::vector<TmapSet *> tmap_sets_;   // small cache keyed by (faces ptr, stride, nframes)
     uint64_t tmap_tick_ = 0;
-    std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on
+    std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on (eagerly)
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
     int ring_ctas_per_sm_[8] = {};       // per ring kernel instance: rubix | rgba << 1 | keep << 2
     size_t ring_smem_[8] = {};
     TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes);
     bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep);
+                     void *stream, bool rgba, bool keep, bool capturing);
     bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
                      void *stream, bool rgba, bool keep);
+
+    // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
+    // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are
+    // handed out in order and come back all at once (release_captures).  Buffers a captured launch reads are not
+    // freed by the next upload_lensmap but retired, until release_captures.
+    struct CaptureStream {
+        void *stream;
+        unsigned long long id;  // capture sequence a warp was captured into
+    };
+    uint32_t *d_capture_slots_ = nullptr;
+    uint32_t capture_slots_used_ = 0;
+    bool captured_ = false;               // a launch was captured since the last upload_lensmap
+    bool bg_captured_ = false;            // a launch was captured since d_bg_ was allocated
+    std::vector<void *> retired_;         // device buffers that captured graphs may still read
+    std::vector<CaptureStream> capture_streams_;  // where warps were captured (release_captures refuses while one is open)
     std::string plan_summary_;
 public:
     const std::string &plan_summary() const { return plan_summary_; }

@@ -49,7 +49,7 @@ enum {
     BLINKY_E_NODEVICE = -4,  /* context has no GPU (created with device < 0) */
     BLINKY_E_CUDA = -5,      /* CUDA runtime error */
     BLINKY_E_NOMEM = -6,
-    BLINKY_E_STATE = -7      /* lens/globe invalid or lensmap not built */
+    BLINKY_E_STATE = -7      /* lens/globe invalid or lensmap not built; no capture work counter left */
 };
 
 /* zoom.type, fisheye.c:457 */
@@ -218,12 +218,30 @@ int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
  * rowbytes < (x0 + width) * bytes per pixel, or nframes > 1 with
  * screen_frame_stride < (y0 + height) * rowbytes.  Views whose width, origin, rowbytes and frame
  * stride are multiples of 4 pixels take the fast kernels; any other view is warped pixel by pixel.
- * Known limitation, shared with every blinky_warp_device* call: not capturable in a CUDA graph.  The
- * ring kernel draws work tickets from a per-stream counter that is never reset, and each launch is
- * given the counter's value at its start; a replayed graph would reuse a stale value. */
+ *
+ * CUDA graphs.  blinky_warp_device, blinky_warp_device_rgba, blinky_warp_device_view and
+ * blinky_warp_device_view_rgba may be called while `stream` is capturing (cudaStreamBeginCapture in any
+ * mode, torch.cuda.graph): they then allocate, copy and synchronise nothing, and the launches land in
+ * the graph.  A replay, on any stream and beside eager warps and other graphs of the same context, reads
+ *   - the lensmap and tile plan of the capture (a later blinky_build_lensmap does not invalidate the
+ *     graph: the buffers it would free are kept for the graph);
+ *   - the faces and output pointers given at capture, with whatever they hold when the replay runs;
+ *   - the background, rubix LUTs and RGBA table as they are when the replay runs (after a rebuild to
+ *     another view size: the background of the captured size).
+ * Each captured launch of the ring kernel takes one of 4096 work counters; when none is left the call
+ * fails with BLINKY_E_STATE and launches nothing.  blinky_warp_host, blinky_shard_warp_gather,
+ * blinky_build_lensmap, blinky_set_background and blinky_set_rgba_table must not be called while a
+ * stream is capturing. */
 int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen,
                             size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
                             int keep_unmapped, void *stream);
+/* States that no graph which captured a warp of this context will run again (destroy those graphs
+ * first, or keep them and never launch them): synchronises the device, frees the lensmap buffers
+ * rebuilds kept for graphs, and returns every capture work counter.  Call it after retiring a set of
+ * graphs, e.g. when a lens change makes them stale.  BLINKY_E_INVALID, changing nothing, while a capture
+ * that holds a warp of this context is still open (it asks each stream such a warp was captured on, so
+ * call it before destroying those streams).  blinky_destroy does the same. */
+int blinky_release_captures(blinky_ctx *ctx);
 
 /* End to end from HOST buffers: pinned-staged cudaMemcpyAsync of each frame's
  * displayed plates, the warp, and the copy back, software-pipelined over
@@ -318,9 +336,10 @@ int blinky_get_tile_plan(blinky_ctx *ctx, void *tiles_out, size_t tiles_cap, voi
 /* FNV-1a digest of the tile table + entry blocks planned on `threads` host threads (the plan
  * must not depend on the thread count; used by the tests) */
 uint64_t blinky_plan_digest(blinky_ctx *ctx, int threads);
-/* number of kernel launches issued by this context so far */
+/* number of kernel launches issued by this context so far (launches captured into a graph count once,
+ * at capture; replays do not count) */
 int64_t blinky_launch_count(blinky_ctx *ctx);
-/* last warp kernel's name and launch geometry, for reports */
+/* last warp kernel's name and launch geometry, for reports (a captured launch included) */
 const char *blinky_last_kernel(blinky_ctx *ctx);
 
 #ifdef __cplusplus
