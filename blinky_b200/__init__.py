@@ -100,6 +100,8 @@ _SIGNATURES = [
     ("blinky_warp_device", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p]),
     ("blinky_warp_device_view", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     ("blinky_warp_device_view_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    ("blinky_warp_device_view_rgba_tables", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int,
+                                                    c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_host", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int]),
     ("blinky_upload_bytes_per_frame", c_int64, [_CTX]),
     ("blinky_alloc_pinned", c_int, [_CTX, c_size_t, POINTER(c_void_p)]),
@@ -401,23 +403,51 @@ class Fisheye:
             self._check(self._lib.blinky_set_background(self._ctx, bg.ctypes.data))
 
     def warp(self, d_faces, d_out, nframes: int = 1, face_stride: int | None = None, out_stride: int | None = None,
-             stream: int | None = None, rgba: bool = False):
+             stream: int | None = None, rgba: bool = False, tables=None):
         """device-resident batch; d_faces/d_out are torch CUDA tensors (or raw device addresses).  May be captured
-        into a CUDA graph (torch.cuda.graph; see release_captures)."""
+        into a CUDA graph (torch.cuda.graph; see release_captures).  tables (RGBA): per-frame palette tables, see
+        warp_view."""
         ps2 = self.platesize * self.platesize
         if face_stride is None:
             face_stride = self.numplates * ps2
         if out_stride is None:
             out_stride = self.width * self.height * (4 if rgba else 1)
+        if tables is not None:
+            # the dense frames are the view at (0, 0) of screens exactly as wide as the view
+            self.warp_view(d_faces, _ptr(d_out), x0=0, y0=0, rowbytes=self.width * 4, nframes=nframes, rgba=rgba,
+                           face_stride=face_stride, screen_stride=out_stride, stream=stream, tables=tables)
+            return
         fn = self._lib.blinky_warp_device_rgba if rgba else self._lib.blinky_warp_device
         self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_out), out_stride, nframes, _warp_stream(stream)))
 
+    @staticmethod
+    def _table_args(tables, rgba: bool, nframes: int) -> tuple[int, int]:
+        """(device address, stride in bytes) of per-frame RGBA tables: a CUDA tensor of 4-byte elements, [256] (one
+        table for every frame, stride 0) or [N >= nframes, 256] with a contiguous last dimension"""
+        if not rgba:
+            raise ValueError("tables: per-frame palette tables need rgba=True")
+        if not (hasattr(tables, "is_cuda") and hasattr(tables, "element_size")) or not tables.is_cuda:
+            raise ValueError("tables: expected a CUDA tensor")
+        if tables.element_size() != 4:
+            raise ValueError(f"tables: expected 4-byte elements, got {tables.dtype}")
+        if tables.dim() == 1 and tuple(tables.shape) == (256,) and tables.stride(0) == 1:
+            return tables.data_ptr(), 0
+        if tables.dim() == 2 and tables.shape[1] == 256 and tables.stride(1) == 1 and tables.shape[0] >= nframes:
+            return tables.data_ptr(), tables.stride(0) * 4
+        raise ValueError(f"tables: expected shape [256] or [N >= {nframes}, 256] with a contiguous last dimension, "
+                         f"got {tuple(tables.shape)} with strides {tuple(tables.stride())}")
+
     def warp_view(self, d_faces, d_screen, x0: int = 0, y0: int = 0, rowbytes: int | None = None, nframes: int = 1,
                   keep_unmapped: bool = False, rgba: bool = False, face_stride: int | None = None,
-                  screen_stride: int | None = None, stream: int | None = None):
+                  screen_stride: int | None = None, stream: int | None = None, tables=None):
         """device-resident batch into the view rectangle at pixel (x0, y0) of device screens (blinky_warp_device_view).
         d_screen: a torch CUDA tensor [N, SH, SW] (or [SH, SW]), whose row pitch and frame stride give rowbytes and
-        screen_stride, or a raw device address.  keep_unmapped: only mapped pixels are written."""
+        screen_stride, or a raw device address.  keep_unmapped: only mapped pixels are written.
+        tables (RGBA only, blinky_warp_device_view_rgba_tables): frame f is expanded through tables[f] instead of
+        the set_rgba_table table — a CUDA tensor of 4-byte elements, [N >= nframes, 256] with a contiguous last
+        dimension, or [256] for one table for every frame.  Read when the launch runs, in stream order."""
+        if tables is not None:
+            d_tables, table_stride = self._table_args(tables, rgba, nframes)
         if face_stride is None:
             face_stride = self.numplates * self.platesize * self.platesize
         bpp = 4 if rgba else 1
@@ -427,6 +457,11 @@ class Fisheye:
         if screen_stride is None:
             screen_stride = (d_screen.stride(-3) * d_screen.element_size() if shape is not None and len(shape) >= 3
                              else (y0 + self.height) * rowbytes)
+        if tables is not None:
+            self._check(self._lib.blinky_warp_device_view_rgba_tables(
+                self._ctx, _ptr(d_faces), face_stride, _ptr(d_screen), screen_stride, rowbytes, x0, y0, nframes,
+                1 if keep_unmapped else 0, d_tables, table_stride, _warp_stream(stream)))
+            return
         fn = self._lib.blinky_warp_device_view_rgba if rgba else self._lib.blinky_warp_device_view
         self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_screen), screen_stride, rowbytes, x0, y0, nframes,
                        1 if keep_unmapped else 0, _warp_stream(stream)))

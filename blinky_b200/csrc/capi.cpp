@@ -353,18 +353,22 @@ namespace {
 // The one way into the device-resident warp: frames land in the view rectangle at (x0, y0) of screens with rows of
 // `rowbytes` bytes.  The dense entry points are the rectangle that is the whole screen.
 int warp_into_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
-                   int rowbytes, int x0, int y0, int nframes, bool keep_unmapped, void *stream, bool rgba) {
+                   int rowbytes, int x0, int y0, int nframes, bool keep_unmapped, void *stream, bool rgba,
+                   const uint32_t *d_tables = nullptr, size_t table_stride = 0) {
     const size_t bpp = rgba ? 4 : 1;
     uint8_t *origin = static_cast<uint8_t *>(d_screen) + static_cast<size_t>(y0) * static_cast<size_t>(rowbytes) + static_cast<size_t>(x0) * bpp;
-    return ctx->dev->warp(d_faces, face_stride, origin, screen_frame_stride, nframes, stream, rgba, static_cast<size_t>(rowbytes), keep_unmapped)
+    return ctx->dev->warp(d_faces, face_stride, origin, screen_frame_stride, nframes, stream, rgba, static_cast<size_t>(rowbytes), keep_unmapped,
+                          d_tables, table_stride)
                ? BLINKY_OK
                : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
+// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose d_tables / table_stride are checked here too
 int warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
-                     int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream, bool rgba) {
+                     int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream, bool rgba,
+                     bool with_tables = false, const uint32_t *d_tables = nullptr, size_t table_stride = 0) {
     NEED_DEVICE(ctx);
-    const char *name = rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
+    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
     auto invalid = [&](const char *why) { return set_err(ctx, BLINKY_E_INVALID, std::string(name) + ": " + why); };
     const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = rgba ? 4 : 1;
     if (!d_faces || !d_screen) return invalid("NULL buffer");
@@ -375,7 +379,14 @@ int warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, v
     if (rgba && ((reinterpret_cast<uintptr_t>(d_screen) + static_cast<uintptr_t>(y0) * static_cast<uintptr_t>(rowbytes)) % 4 != 0 || rowbytes % 4 != 0 ||
                  (nframes > 1 && screen_frame_stride % 4 != 0)))
         return invalid("the RGBA view origin, rowbytes and screen_frame_stride must be 4-byte aligned");
-    return warp_into_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped != 0, stream, rgba);
+    if (with_tables) {
+        // (16 bytes: the ring kernel restages a frame's table with 128-bit loads)
+        if (!d_tables || reinterpret_cast<uintptr_t>(d_tables) % 16 != 0) return invalid("d_tables must be a non-NULL, 16-byte aligned device pointer");
+        if (table_stride != 0 && (table_stride < 256 * sizeof(uint32_t) || table_stride % 16 != 0 || table_stride / 4 > UINT32_MAX))
+            return invalid("table_stride must be 0 (one table for every frame) or at least 1024, a multiple of 16 and below 16 GB");
+    }
+    return warp_into_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped != 0, stream, rgba,
+                          d_tables, table_stride);
 }
 
 }  // namespace
@@ -396,6 +407,13 @@ int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_st
 int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
                                  int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
     return warp_device_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream, true);
+}
+
+int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen_rgba,
+                                        size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes, int keep_unmapped,
+                                        const uint32_t *d_tables, size_t table_stride, void *stream) {
+    return warp_device_view(ctx, d_faces, face_stride, d_screen_rgba, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream,
+                            true, true, d_tables, table_stride);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,

@@ -39,7 +39,7 @@ struct WarpParams {
     size_t face_stride;         // bytes between frames
     const uint32_t *bg32;       // background, 4 pixels per element (padded like the lensmap)
     const uint8_t *lut;         // [6][256] rubix tint LUTs
-    const uint32_t *rgba;       // [256] palette expansion table (RGBA mode)
+    const uint32_t *rgba;       // [256] palette expansion table (RGBA mode); TABLES: frame 0's
     void *out;                  // view origin of frame 0
     size_t out_stride;          // bytes between frames
     uint32_t nquads;            // ceil(W*H / 4)
@@ -47,6 +47,7 @@ struct WarpParams {
     uint32_t width;             // W
     uint32_t out_pitch;         // bytes between output rows
     bool pitched;               // out_pitch != W * bytes per pixel: rows are addressed one by one
+    uint32_t table_words;       // TABLES: words between the tables of consecutive frames
 };
 
 __device__ __forceinline__ uint4 ld_lensmap(const uint4 *p) {
@@ -105,8 +106,10 @@ __device__ __forceinline__ size_t out_offset(const WarpParams &p, uint32_t pix, 
 // needs W % 4 == 0, so that no quad straddles two rows.
 // KEEP (keep_unmapped): unmapped pixels are not written and the background is
 // never read; a partly mapped quad is stored pixel by pixel.
+// TABLES (RGBA only): frame f is expanded through its own table at
+// p.rgba + f * p.table_words, in every kernel below.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA, bool KEEP>
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams p) {
     __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
     __shared__ uint32_t s_rgba[RGBA ? 256 : 1];
@@ -116,7 +119,9 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
         for (int i = threadIdx.x; i < 6 * 256 / 4; i += kThreads) dst[i] = __ldg(src + i);
     }
     if (RGBA) {
-        for (int i = threadIdx.x; i < 256; i += kThreads) s_rgba[i] = __ldg(p.rgba + i);
+        // (one frame per CTA: its table)
+        const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(blockIdx.y) * p.table_words : p.rgba;
+        for (int i = threadIdx.x; i < 256; i += kThreads) s_rgba[i] = __ldg(table + i);
     }
     if (RUBIX || RGBA) __syncthreads();
 
@@ -180,7 +185,7 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
 // unaligned strides, or a view rectangle whose origin or pitch is not a
 // multiple of 4 pixels) — a correctness path for ragged sizes, not a fast path.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA, bool KEEP>
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams p) {
     const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
     if (i >= p.npix) return;
@@ -198,7 +203,7 @@ __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams 
         b = __ldg(reinterpret_cast<const uint8_t *>(p.bg32) + i);
     }
     uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(blockIdx.y) * p.out_stride + out_offset(p, i, RGBA ? 4 : 1);
-    if (RGBA) *reinterpret_cast<uint32_t *>(o) = __ldg(p.rgba + b);
+    if (RGBA) *reinterpret_cast<uint32_t *>(o) = __ldg((TABLES ? p.rgba + static_cast<size_t>(blockIdx.y) * p.table_words : p.rgba) + b);
     else *o = static_cast<uint8_t>(b);
 }
 
@@ -249,6 +254,7 @@ struct RingParams {
     uint32_t ring_grid;     // CTAs [0, ring_grid) are ring warps, the CTAs behind them take one gather item each
     int width, height;
     uint32_t zero;  // always 0, but only the host knows: see stage_dep()
+    uint32_t table_words;   // TABLES: words between the RGBA tables of consecutive frames (rgba: frame 0's)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -358,7 +364,7 @@ __device__ __forceinline__ void st_stream_u32x8(const uint64_t (&a)[8], const ui
 // vacate at the end.
 constexpr int kGatherRows = 8, kGatherFrames = 4;
 
-template <bool RUBIX, bool RGBA, bool KEEP>
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, uint32_t lane) {
     const uint32_t nfg = (p.nframes + kGatherFrames - 1) / kGatherFrames;
     const uint32_t fg = item % nfg, rest = item / nfg;
@@ -400,7 +406,8 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
             uint32_t b = v[g][j] & 0x100u ? bgv : v[g][j];
             if (RUBIX && t != BLINKY_LM_TINT_NONE) b = __ldg(p.lut + t * 256 + b);
             uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(f0 + g) * p.out_stride;
-            if (RGBA) reinterpret_cast<uint32_t *>(o)[opix] = __ldg(p.rgba + b);
+            const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(f0 + g) * p.table_words : p.rgba;
+            if (RGBA) reinterpret_cast<uint32_t *>(o)[opix] = __ldg(table + b);
             else o[opix] = static_cast<uint8_t>(b);
         }
     }
@@ -422,14 +429,14 @@ constexpr int kRingMinBlocks = 16;
 
 // KEEP (keep_unmapped): only mapped pixels are written.  The host gives this instance the BOX tiles alone (EMPTY tiles
 // have nothing to write); a partly mapped quad is stored pixel by pixel and the background is never read.
-template <bool RUBIX, bool RGBA, bool KEEP>
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // XOR with a parameter that is always zero: keeps ptxas from re-reading the special register
     // (S2R, tens of cycles) at every `lane == 0` test instead of holding the lane number in a register
     const uint32_t lane = threadIdx.x ^ p.zero;
     if (blockIdx.x >= p.ring_grid) {   // the CTAs behind the ring warps: one gather item each
-        gather_item<RUBIX, RGBA, KEEP>(p, blockIdx.x - p.ring_grid, lane);
+        gather_item<RUBIX, RGBA, KEEP, TABLES>(p, blockIdx.x - p.ring_grid, lane);
         return;
     }
     const uint32_t R = p.ring_bytes;
@@ -447,11 +454,39 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
         uint32_t *dst = reinterpret_cast<uint32_t *>(s_lut);
         for (uint32_t i = lane; i < 6 * 256 / 4; i += 32) dst[i] = __ldg(src + i);
     }
-    if (RGBA) {
+    if (RGBA && !TABLES) {
         for (uint32_t i = lane; i < 256; i += 32) s_rgba[i] = __ldg(p.rgba + i);
     }
     __syncwarp();
     const uint32_t lut_base = smem_u32(s_lut);
+
+    // TABLES: s_rgba holds one frame's table at a time, restaged before the first lookup of a frame whose table it
+    // does not hold.  Each lane keeps its 8 words of the table it will need next in registers (two 128-bit loads,
+    // issued a frame ahead), so the load latency hides behind a frame of work.  These are plain loads and stores of
+    // this warp alone: __syncwarp orders the lookups in the old table before the stores of the new one, and those
+    // before the next lookups.  The hazard stage_dep guards against (a TMA write overtaking a shared load still in
+    // flight) does not arise: nothing in the async proxy writes s_rgba.
+    uint32_t tab_f = 0xffffffffu, next_f = 0xffffffffu;   // frame whose table s_rgba holds / the registers hold
+    uint4 next_t0 = make_uint4(0u, 0u, 0u, 0u), next_t1 = next_t0;
+    auto fetch_table = [&](uint32_t f) {
+        const uint4 *src = reinterpret_cast<const uint4 *>(p.rgba + static_cast<size_t>(f) * p.table_words) + 2 * lane;
+        next_t0 = __ldg(src);
+        next_t1 = __ldg(src + 1);
+        next_f = f;
+    };
+    // s_rgba := frame f's table; then the registers start loading frame `after`'s
+    auto use_table = [&](uint32_t f, uint32_t after) {
+        if (tab_f != f) {
+            if (next_f != f) fetch_table(f);
+            __syncwarp();
+            uint4 *dst = reinterpret_cast<uint4 *>(s_rgba) + 2 * lane;
+            dst[0] = next_t0;
+            dst[1] = next_t1;
+            __syncwarp();
+            tab_f = f;
+        }
+        if (after != tab_f && after != next_f) fetch_table(after);
+    };
 
     const uint32_t NW = p.ring_grid;
     const uint32_t width = static_cast<uint32_t>(p.width), height = static_cast<uint32_t>(p.height);
@@ -657,10 +692,14 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                 st_stream_v4(reinterpret_cast<uint4 *>(dst), make_uint4(s_rgba[v & 0xffu], s_rgba[(v >> 8) & 0xffu], s_rgba[(v >> 16) & 0xffu], s_rgba[v >> 24]));
             };
 
+            // (TABLES: the next frame is this unit's next, or the first of the unit after it)
+            auto next_frame = [&](uint32_t f) { return f + 1 < A.nf ? A.f0 + f + 1 : B.f0; };
+
             if (type == TILE_BOX_FULL) {
                 for (uint32_t f = 0; f < A.nf; ++f) {
                     uint32_t w[8];
                     gather_frame(w);
+                    if (TABLES) use_table(A.f0 + f, next_frame(f));
                     if (RGBA) {
 #pragma unroll
                         for (int q = 0; q < 8; ++q) store_rgba(o + static_cast<size_t>(static_cast<uint32_t>(q) * row4), w[q]);
@@ -696,6 +735,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                 for (uint32_t f = 0; f < A.nf; ++f) {
                     uint32_t w[8];
                     gather_frame(w);
+                    if (TABLES) use_table(A.f0 + f, next_frame(f));
 #pragma unroll
                     for (int q = 0; q < 8; ++q) {
                         if (!((store_mask >> q) & 1u)) continue;
@@ -729,8 +769,12 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                     const size_t opix = static_cast<size_t>(y) * p.out_pitch + qx;
                     for (uint32_t f = 0; f < A.nf; ++f) {
                         uint8_t *out_frame = static_cast<uint8_t *>(p.out) + static_cast<size_t>(A.f0 + f) * p.out_stride;
-                        if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(out_frame) + (opix >> 2),
-                                               make_uint4(s_rgba[v & 0xffu], s_rgba[(v >> 8) & 0xffu], s_rgba[(v >> 16) & 0xffu], s_rgba[v >> 24]));
+                        if (TABLES) {   // (s_rgba may hold another frame's table: looked up like K3)
+                            const uint32_t *t = p.rgba + static_cast<size_t>(A.f0 + f) * p.table_words;
+                            st_stream_v4(reinterpret_cast<uint4 *>(out_frame) + (opix >> 2),
+                                         make_uint4(__ldg(t + (v & 0xffu)), __ldg(t + ((v >> 8) & 0xffu)), __ldg(t + ((v >> 16) & 0xffu)), __ldg(t + (v >> 24))));
+                        } else if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(out_frame) + (opix >> 2),
+                                                      make_uint4(s_rgba[v & 0xffu], s_rgba[(v >> 8) & 0xffu], s_rgba[(v >> 16) & 0xffu], s_rgba[v >> 24]));
                         else st_stream_u32(reinterpret_cast<uint32_t *>(out_frame) + (opix >> 2), v);
                     }
                 }
@@ -761,7 +805,7 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
 // --------------------------------------------------------------------------
 constexpr int kGatherFramesPerCta = 4;
 
-template <bool RUBIX, bool RGBA, bool KEEP>
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid_constant__ RingParams p, const uint32_t first_tile) {
     const uint32_t tid = threadIdx.x;
     const uint4 d = __ldg(reinterpret_cast<const uint4 *>(p.tiles + first_tile + blockIdx.x));
@@ -782,7 +826,8 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
         const size_t opix = static_cast<size_t>(y) * p.out_pitch + x;
         for (uint32_t f = f0; f < f1; ++f) {
             uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(f) * p.out_stride;
-            if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(o) + (opix >> 2), make_uint4(__ldg(p.rgba + px[0]), __ldg(p.rgba + px[1]), __ldg(p.rgba + px[2]), __ldg(p.rgba + px[3])));
+            const uint32_t *t = TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : p.rgba;
+            if (RGBA) st_stream_v4(reinterpret_cast<uint4 *>(o) + (opix >> 2), make_uint4(__ldg(t + px[0]), __ldg(t + px[1]), __ldg(t + px[2]), __ldg(t + px[3])));
             else st_stream_u32(reinterpret_cast<uint32_t *>(o) + (opix >> 2), bgw);
         }
         return;
@@ -817,6 +862,7 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
         const uint32_t f = f0 + g;
         if (f >= f1) break;
         uint8_t *o = static_cast<uint8_t *>(p.out) + static_cast<size_t>(f) * p.out_stride;
+        const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : p.rgba;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const uint32_t y = tile_y + warp * 4 + j;
@@ -827,7 +873,7 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
                     if (t != BLINKY_LM_TINT_NONE) b = __ldg(p.lut + t * 256 + b);
                 }
                 const size_t pix = static_cast<size_t>(y) * p.out_pitch + x;
-                if (RGBA) reinterpret_cast<uint32_t *>(o)[pix] = __ldg(p.rgba + b);
+                if (RGBA) reinterpret_cast<uint32_t *>(o)[pix] = __ldg(table + b);
                 else o[pix] = static_cast<uint8_t>(b);
             }
         }
@@ -1041,7 +1087,7 @@ bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
 }
 
 bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                      bool rgba, size_t out_pitch, bool keep_unmapped) {
+                      bool rgba, size_t out_pitch, bool keep_unmapped, const uint32_t *d_tables, size_t table_stride) {
     err_code_ = BLINKY_E_CUDA;
     if (!have_lensmap_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
@@ -1075,9 +1121,10 @@ bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size
         CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(stream), &cap, &cap_id));
     const bool capturing = cap != cudaStreamCaptureStatusNone;
     const bool ok = variant_ == BLINKY_KERNEL_GATHER || !tiled_ok
-                        ? launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped)
+                        ? launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
+                                      d_tables, table_stride)
                         : launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
-                                      capturing);
+                                      d_tables, table_stride, capturing);
     if (capturing) {
         captured_ = bg_captured_ = true;
         bool known = false;
@@ -1175,23 +1222,25 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
 
-// Calls f(R, C, K) with std::bool_constant arguments for (rubix, rgba, keep): one place turns the run-time flags into
-// the kernels' template arguments.
+// Calls f(R, C, K, T) with std::bool_constant arguments for (rubix, rgba, keep, tables): one place turns the run-time
+// flags into the kernels' template arguments.  Per-frame tables exist only in RGBA: 12 combinations.
 template <typename F>
-static auto with_variant(bool rubix, bool rgba, bool keep, F &&f) {
+static auto with_variant(bool rubix, bool rgba, bool keep, bool tables, F &&f) {
     using T = std::true_type;
     using N = std::false_type;
     if (rubix) {
-        if (rgba) return keep ? f(T{}, T{}, T{}) : f(T{}, T{}, N{});
-        return keep ? f(T{}, N{}, T{}) : f(T{}, N{}, N{});
+        if (rgba && tables) return keep ? f(T{}, T{}, T{}, T{}) : f(T{}, T{}, N{}, T{});
+        if (rgba) return keep ? f(T{}, T{}, T{}, N{}) : f(T{}, T{}, N{}, N{});
+        return keep ? f(T{}, N{}, T{}, N{}) : f(T{}, N{}, N{}, N{});
     }
-    if (rgba) return keep ? f(N{}, T{}, T{}) : f(N{}, T{}, N{});
-    return keep ? f(N{}, N{}, T{}) : f(N{}, N{}, N{});
+    if (rgba && tables) return keep ? f(N{}, T{}, T{}, T{}) : f(N{}, T{}, N{}, T{});
+    if (rgba) return keep ? f(N{}, T{}, T{}, N{}) : f(N{}, T{}, N{}, N{});
+    return keep ? f(N{}, N{}, T{}, N{}) : f(N{}, N{}, N{}, N{});
 }
 
-static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, size_t smem, int *n) {
-    return with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
-        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value>;
+static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, bool tables, size_t smem, int *n) {
+    return with_variant(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) {
+        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value>;
         cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
         if (e != cudaSuccess) return e;
         return cudaOccupancyMaxActiveBlocksPerMultiprocessor(n, kernel, 32, smem);
@@ -1199,7 +1248,7 @@ static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, size_t smem, 
 }
 
 bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep, bool capturing) {
+                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     RingParams p;
     p.tiles = static_cast<const TileDesc *>(d_tiles_);
@@ -1215,7 +1264,9 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.face_stride = face_stride;
     p.bg = d_bg_;
     p.lut = d_lut_;
-    p.rgba = d_rgba_;
+    p.rgba = tables ? tables : d_rgba_;
+    p.table_words = static_cast<uint32_t>(table_stride / 4);
+    const bool per_frame = rgba && tables && table_stride != 0;
     p.out = d_out;
     p.out_stride = out_stride;
     p.out_pitch = out_pitch / (rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
@@ -1227,7 +1278,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.height = height_;
     p.zero = 0;
     const bool rubix = rubix_;
-    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0);
+    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0) | (per_frame ? 8 : 0);
     // The ring kernel takes the BOX tiles [0, nbox) and the EMPTY tiles; the GATHER tiles in between go to the
     // gather kernel K3 on the context's side stream (forked from and joined to the caller's stream), so the two
     // kernels share the GPU instead of queueing behind each other.  With keep_unmapped an EMPTY tile has nothing
@@ -1272,7 +1323,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     const size_t smem = static_cast<size_t>(ring_bytes) + fixed;
     if (ring_ctas_per_sm_[vi] == 0 || ring_smem_[vi] != smem) {
         int n = 0;
-        cudaError_t e = ring_config_v(rubix, rgba, keep, smem, &n);
+        cudaError_t e = ring_config_v(rubix, rgba, keep, per_frame, smem, &n);
         if (e != cudaSuccess) return fail("ring kernel configuration (shared memory / occupancy)", e);
         if (n < 1) {
             err_ = "ring kernel does not fit on an SM";
@@ -1335,17 +1386,17 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     }
     char buf[640];
     int nbuf = 0;
-    const char *keep_tag = keep ? ",keep=1" : "";
+    const char *tags = keep && per_frame ? ",keep=1,tables=1" : keep ? ",keep=1" : per_frame ? ",tables=1" : "";
     // GATHER tiles: one-warp CTAs behind the ring warps in the same grid (see gather_item); only a plan without BOX and
     // EMPTY tiles (with keep_unmapped: without BOX tiles) launches the stand-alone gather kernel.
     snprintf(buf, sizeof buf, "%s", ngather_tiles_ == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
     if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
         dim3 g2(ngather_tiles_, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
-        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
-            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
+        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
+            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
         });
         ++launches_;
-        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, g2.x, g2.y, kThreads);
+        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, g2.x, g2.y, kThreads);
     }
     if (grid > 0) {
         // static share of the schedule (see the kernel): static_pct_ percent of the units, whole rounds
@@ -1365,15 +1416,15 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
 
         p.ring_grid = grid;
         const uint32_t extra = merged_gather ? gather_items : 0u;
-        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
-            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid + extra, 32, smem, st>>>(p, *tm);
+        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
+            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid + extra, 32, smem, st>>>(p, *tm);
         });
         ++launches_;
         nbuf = static_cast<int>(strlen(buf));
         snprintf(buf + nbuf, sizeof buf - static_cast<size_t>(nbuf),
                  "%swarp_ring_kernel<rubix=%d,rgba=%d%s> grid=%u+%u block=32 (%d ring warps/SM, TMA box ring of %u B, <=%u boxes in flight, %u frames/unit, %u units; "
                  "%u gather CTAs of %dx32 px x %d frames)",
-                 nbuf ? " + " : "", rubix, rgba, keep_tag, grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows, kGatherFrames);
+                 nbuf ? " + " : "", rubix, rgba, tags, grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows, kGatherFrames);
     }
     last_kernel_ = buf;
     CK(cudaGetLastError());
@@ -1381,7 +1432,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
 }
 
 bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep) {
+                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride) {
     // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out
     // unless the caller made its own) — NOT this context's private stream.
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1391,7 +1442,9 @@ bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_ou
     p.face_stride = face_stride;
     p.bg32 = reinterpret_cast<const uint32_t *>(d_bg_);
     p.lut = d_lut_;
-    p.rgba = d_rgba_;
+    p.rgba = tables ? tables : d_rgba_;
+    p.table_words = static_cast<uint32_t>(table_stride / 4);
+    const bool per_frame = rgba && tables && table_stride != 0;
     p.out = d_out;
     p.out_stride = out_stride;
     p.nquads = static_cast<uint32_t>((npix_ + 3) / 4);
@@ -1405,20 +1458,20 @@ bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_ou
     const bool vector_ok = (p.pitched ? width_ % 4 == 0 && out_pitch % (4 * opx) == 0 : npix_ % 4 == 0) &&
                            (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (out_stride % (4 * opx) == 0 || nframes == 1);
     const bool rubix = rubix_;
-    const char *keep_tag = keep ? ",keep=1" : "";
+    const char *tags = keep && per_frame ? ",keep=1,tables=1" : keep ? ",keep=1" : per_frame ? ",tables=1" : "";
     char buf[160];
     if (vector_ok) {
         dim3 grid(static_cast<unsigned>(npix_pad_ / kPixelsPerBlock), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
-            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid, kThreads, 0, st>>>(p);
+        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
+            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid, kThreads, 0, st>>>(p);
         });
-        snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, grid.x, grid.y, kThreads);
+        snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
     } else {
         dim3 grid(static_cast<unsigned>((npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, [&](auto R, auto C, auto K) {
-            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value><<<grid, kThreads, 0, st>>>(p);
+        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
+            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid, kThreads, 0, st>>>(p);
         });
-        snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, keep_tag, grid.x, grid.y, kThreads);
+        snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
     }
     last_kernel_ = buf;
     ++launches_;

@@ -50,9 +50,12 @@ public:
     // device-resident batch (asynchronous on `stream`, nullptr = CUDA default stream).  d_out is the view origin of
     // frame 0; rows are out_pitch bytes apart (0: dense, W * bytes per pixel).  keep_unmapped: only mapped pixels
     // are written, the others keep what the caller's buffer holds.  May be captured into a CUDA graph: see
-    // release_captures.
+    // release_captures.  RGBA with d_tables: frame f is expanded through the 256-entry device table at
+    // d_tables + f * table_stride bytes (table_stride 0: one table for every frame) instead of set_rgba_table's; the
+    // tables are read when the launch runs.  d_tables 16-byte aligned, table_stride a multiple of 16.
     bool warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-              bool rgba, size_t out_pitch = 0, bool keep_unmapped = false);
+              bool rgba, size_t out_pitch = 0, bool keep_unmapped = false, const uint32_t *d_tables = nullptr,
+              size_t table_stride = 0);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, frees
     // the buffers upload_lensmap retired for such graphs and returns every capture counter slot to the pool.
     bool release_captures();
@@ -128,13 +131,13 @@ private:
     uint64_t tmap_tick_ = 0;
     std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on (eagerly)
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
-    int ring_ctas_per_sm_[8] = {};       // per ring kernel instance: rubix | rgba << 1 | keep << 2
-    size_t ring_smem_[8] = {};
+    int ring_ctas_per_sm_[16] = {};      // per ring kernel instance: rubix | rgba << 1 | keep << 2 | per-frame tables << 3
+    size_t ring_smem_[16] = {};
     TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes);
     bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep, bool capturing);
+                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing);
     bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep);
+                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride);
 
     // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
     // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are

@@ -219,13 +219,15 @@ int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
  * screen_frame_stride < (y0 + height) * rowbytes.  Views whose width, origin, rowbytes and frame
  * stride are multiples of 4 pixels take the fast kernels; any other view is warped pixel by pixel.
  *
- * CUDA graphs.  blinky_warp_device, blinky_warp_device_rgba, blinky_warp_device_view and
- * blinky_warp_device_view_rgba may be called while `stream` is capturing (cudaStreamBeginCapture in any
- * mode, torch.cuda.graph): they then allocate, copy and synchronise nothing, and the launches land in
- * the graph.  A replay, on any stream and beside eager warps and other graphs of the same context, reads
+ * CUDA graphs.  blinky_warp_device, blinky_warp_device_rgba, blinky_warp_device_view,
+ * blinky_warp_device_view_rgba and blinky_warp_device_view_rgba_tables may be called while `stream` is
+ * capturing (cudaStreamBeginCapture in any mode, torch.cuda.graph): they then allocate, copy and
+ * synchronise nothing, and the launches land in the graph.  A replay, on any stream and beside eager
+ * warps and other graphs of the same context, reads
  *   - the lensmap and tile plan of the capture (a later blinky_build_lensmap does not invalidate the
  *     graph: the buffers it would free are kept for the graph);
- *   - the faces and output pointers given at capture, with whatever they hold when the replay runs;
+ *   - the faces, output and per-frame table pointers given at capture, with whatever they hold when the
+ *     replay runs (so a cudaMemcpyAsync into the tables on the replay's stream changes the palette);
  *   - the background, rubix LUTs and RGBA table as they are when the replay runs (after a rebuild to
  *     another view size: the background of the captured size).
  * Each captured launch of the ring kernel takes one of 4096 work counters; when none is left the call
@@ -307,7 +309,11 @@ int blinky_shard_sync(blinky_ctx *ctx);
 int blinky_shard_close(blinky_ctx *ctx);
 
 /* Fused 8-bit -> 32-bit palette expansion (engine/common/vid_sdl.c:539-546,
- * d_8to24table): same warp, output one uint32 per pixel.  table: 256 entries. */
+ * d_8to24table): same warp, output one uint32 per pixel.  table: 256 entries.
+ * blinky_set_rgba_table is a blocking host-side replacement of the context's one table (a synchronous
+ * copy, outside any stream's order; not while a stream captures).  To change palettes from frame to frame
+ * in stream order (V_UpdatePalette's flashes and fades), and per frame within a batch, use
+ * blinky_warp_device_view_rgba_tables. */
 int blinky_set_rgba_table(blinky_ctx *ctx, const uint32_t table[256]);
 int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out_rgba,
                             size_t out_stride, int nframes, void *stream);
@@ -317,6 +323,20 @@ int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_st
 int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen_rgba,
                                  size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
                                  int keep_unmapped, void *stream);
+/* blinky_warp_device_view_rgba, with frame f expanded through its own 256-entry table at
+ * d_tables + f * table_stride bytes instead of the context's blinky_set_rgba_table table.
+ * table_stride == 0: one table for every frame.  The tables are device memory, read when the
+ * launch runs (stream order: a cudaMemcpyAsync into them earlier on `stream` is seen), so the call
+ * is capturable like every blinky_warp_device* call and a replay reads the tables' contents at
+ * replay time.  The context's own table is neither read nor changed.  Rubix tints apply before the
+ * expansion; without keep_unmapped an unmapped pixel is the background byte through frame f's table.
+ * Besides the checks of blinky_warp_device_view_rgba, fails with BLINKY_E_INVALID, launching nothing,
+ * when d_tables is NULL or not 16-byte aligned, or table_stride is nonzero and below 1024 or not a
+ * multiple of 16. */
+int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
+                                        void *d_screen_rgba, size_t screen_frame_stride, int rowbytes, int x0,
+                                        int y0, int nframes, int keep_unmapped, const uint32_t *d_tables,
+                                        size_t table_stride, void *stream);
 
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
