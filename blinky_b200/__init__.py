@@ -91,6 +91,7 @@ _SIGNATURES = [
     ("blinky_mapped_pixels", c_int64, [_CTX]),
     ("blinky_lens_inverse", c_int, [_CTX, c_double, c_double, POINTER(c_double)]),
     ("blinky_lens_forward", c_int, [_CTX, c_double, c_double, c_double, POINTER(c_double), POINTER(c_double)]),
+    ("blinky_globe_plate", c_int, [_CTX, c_double, c_double, c_double, POINTER(c_int)]),
     ("blinky_lens_source", c_int, [_CTX, c_int, c_void_p, c_size_t]),
     ("blinky_write_config", c_int, [_CTX, c_void_p, c_size_t]),
     ("blinky_saveglobe_pending", c_int, [_CTX]),
@@ -365,10 +366,19 @@ class Fisheye:
         st = self._lib.blinky_lens_forward(self._ctx, rx, ry, rz, ctypes.byref(x), ctypes.byref(y))
         return st, (x.value, y.value)
 
-    def lens_source(self, cuda: bool = False, forward: bool = False, with_kernel: bool = False) -> str:
+    def globe_plate(self, x: float, y: float, z: float):
+        """(status, plate) of the globe's globe_plate script as the lensmap build reads it: status 1 with the plate
+        (last value returned, converted like lua_tointeger), 0 with -1 for no value / nil / not a number, negative
+        for an error (-2: the globe has no globe_plate, -3: script error)"""
+        plate = c_int()
+        st = self._lib.blinky_globe_plate(self._ctx, x, y, z, ctypes.byref(plate))
+        return st, plate.value
+
+    def lens_source(self, cuda: bool = False, forward: bool = False, with_kernel: bool = False, globe_plate: bool = False) -> str:
         """The current ``lens_inverse`` (or ``lens_forward``) translated to C++/CUDA (raises when not translatable);
-        ``with_kernel`` appends the fixed kernel the device builder launches."""
-        flavour = int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0)
+        ``with_kernel`` appends the fixed kernel the device builder launches and translates the globe's
+        ``globe_plate`` into the same unit when there is one.  ``globe_plate``: that function translated alone."""
+        flavour = int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0) | (8 if globe_plate else 0)
         n = self._lib.blinky_lens_source(self._ctx, flavour, None, 0)
         if n < 0:
             self._check(n)

@@ -217,7 +217,7 @@ const char *blinky_build_info(blinky_ctx *ctx) { return ctx->build_info.c_str();
 
 int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes) {
     std::string src, why;
-    if (!ctx->host.lens_device_source(true, &src, &why, forward != 0)) return set_err(ctx, BLINKY_E_SCRIPT, why);
+    if (!ctx->host.lens_device_source(true, &src, &why, forward != 0, true)) return set_err(ctx, BLINKY_E_SCRIPT, why);
     std::vector<char> cubin;
     std::string log;
     if (!LensDevice::compile(src, forward != 0, &cubin, &log)) return set_err(ctx, BLINKY_E_CUDA, log);
@@ -296,10 +296,23 @@ int blinky_lens_forward(blinky_ctx *ctx, double rx, double ry, double rz, double
     return ctx->host.lens_forward(rx, ry, rz, x, y);
 }
 
+int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate) {
+    int p = -1;
+    const int rc = ctx->host.globe_plate(x, y, z, &p);
+    if (plate) *plate = p;
+    return rc;
+}
+
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize) {
     std::string s, why;
-    if (!ctx->host.lens_device_source((flavour & 1) != 0, &s, &why, (flavour & 2) != 0)) return set_err(ctx, BLINKY_E_SCRIPT, why);
-    if (flavour & 4) s += LensDevice::kernel_tail((flavour & 2) != 0);
+    if (flavour & 8) {
+        if (!ctx->host.globe_plate_device_source((flavour & 1) != 0, &s, &why)) return set_err(ctx, BLINKY_E_SCRIPT, why);
+    } else {
+        // with the kernel: the unit NVRTC compiles, i.e. with the globe's globe_plate when it has one
+        const bool kernel = (flavour & 4) != 0;
+        if (!ctx->host.lens_device_source((flavour & 1) != 0, &s, &why, (flavour & 2) != 0, kernel)) return set_err(ctx, BLINKY_E_SCRIPT, why);
+        if (kernel) s += LensDevice::kernel_tail((flavour & 2) != 0, blinky::source_has_globe_plate(s));
+    }
     if (buf && bufsize) {
         size_t n = s.size() < bufsize - 1 ? s.size() : bufsize - 1;
         memcpy(buf, s.data(), n);

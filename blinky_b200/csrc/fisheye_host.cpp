@@ -832,22 +832,34 @@ int FisheyeHost::call_forward(Worker &w, const float ray[3], double *x, double *
     return -1;
 }
 
-bool FisheyeHost::lens_device_source(bool cuda, std::string *source, std::string *why, bool forward) {
+bool FisheyeHost::lens_device_source(bool cuda, std::string *source, std::string *why, bool forward, bool with_globe_plate) {
     const Value &fn = forward ? fn_forward_ : fn_inverse_;
     if (!fn.is_function()) {
         *why = forward ? "the lens has no lens_forward" : "the lens has no lens_inverse";
         return false;
     }
-    if (fn_globe_plate_.is_function()) {
-        *why = "the globe selects plates with a script function (globe_plate)";
-        return false;
-    }
-    TranspileResult r = forward ? transpile_lens_forward(*lua_, fn) : transpile_lens(*lua_, fn);
+    const Value *gp = with_globe_plate && fn_globe_plate_.is_function() ? &fn_globe_plate_ : nullptr;
+    TranspileResult r = forward ? transpile_lens_forward(*lua_, fn, gp) : transpile_lens(*lua_, fn, gp);
     if (!r.ok) {
         *why = r.error;
         return false;
     }
     // BLINKY_LENS_NOINLINE=1: script functions become real device calls (faster NVRTC, slower kernel)
+    const char *ni = getenv("BLINKY_LENS_NOINLINE");
+    *source = transpile_prelude(cuda, ni && ni[0] == '1') + r.source;
+    return true;
+}
+
+bool FisheyeHost::globe_plate_device_source(bool cuda, std::string *source, std::string *why) {
+    if (!fn_globe_plate_.is_function()) {
+        *why = "the globe has no globe_plate";
+        return false;
+    }
+    TranspileResult r = transpile_globe_plate(*lua_, fn_globe_plate_);
+    if (!r.ok) {
+        *why = r.error;
+        return false;
+    }
     const char *ni = getenv("BLINKY_LENS_NOINLINE");
     *source = transpile_prelude(cuda, ni && ni[0] == '1') + r.source;
     return true;
@@ -881,6 +893,23 @@ int FisheyeHost::lens_forward(double rx, double ry, double rz, double *x, double
     if (ret.size() == 2 && ret[0].to_number(x) && ret[1].to_number(y)) return 1;
     if (ret.size() == 1 && ret[0].is_nil()) return 0;
     return -1;
+}
+
+int FisheyeHost::globe_plate(double x, double y, double z, int *plate) {
+    *plate = -1;
+    if (!fn_globe_plate_.is_function()) return -2;
+    Value args[3] = {Value(x), Value(y), Value(z)};
+    ValueList ret;
+    try {
+        lua_->call(fn_globe_plate_, args, 3, ret);
+    } catch (LuaError &e) {
+        print("%s\n", e.what());
+        return -3;
+    }
+    double d;  // as ray_to_plate_index converts it
+    if (ret.size() == 0 || !ret[ret.size() - 1].to_number(&d)) return 0;
+    *plate = static_cast<int>(static_cast<ptrdiff_t>(d));
+    return 1;
 }
 
 // ---------------------------------------------------------------------------
@@ -1130,7 +1159,9 @@ LensBuildParams FisheyeHost::device_params() const {
     p.rubix_pad = rubix_pad_;
     const double units = rubix_numcells_ * p.rubix_block + rubix_pad_;
     p.rubix_unit_px = static_cast<double>(platesize_) / units;
-    for (int i = 0; i < numplates_; ++i) {
+    // all six: a globe_plate script may pick a plate >= numplates, and then the host (like the reference,
+    // whose globe.plates is static) uses what an earlier globe left in that slot (0.5 / tan(0) = inf if none)
+    for (int i = 0; i < kMaxPlates; ++i) {
         const Plate &pl = plates_[i];
         p.uv_dist[i] = 0.5 / std::tan(static_cast<double>(pl.fov / 2));
         for (int k = 0; k < 3; ++k) {
@@ -1145,7 +1176,7 @@ LensBuildParams FisheyeHost::device_params() const {
 
 int FisheyeHost::build_inverse_device(int *display, std::string *why) {
     std::string src;
-    if (!lens_device_source(true, &src, why)) return 1;
+    if (!lens_device_source(true, &src, why, false, true)) return 1;
     const LensBuildParams p = device_params();
     const size_t area = idx_.size();
     std::vector<uint32_t> cand(area);
@@ -1292,10 +1323,10 @@ void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const i
 // rasterised on the device in the reference's writer order (lens_device.cu).
 int FisheyeHost::build_forward_device(std::string *why) {
     std::string src;
-    if (!lens_device_source(true, &src, why, true)) return 1;
+    if (!lens_device_source(true, &src, why, true, true)) return 1;
     const LensBuildParams p = device_params();
-    std::vector<uint32_t> undecided;
-    if (!device_builder_->forward_points(src, p, &undecided, why)) return 1;
+    std::vector<uint32_t> undecided, undecided_texels;
+    if (!device_builder_->forward_points(src, p, &undecided, &undecided_texels, why)) return 1;
     std::vector<ForwardPatch> patches(undecided.size());
     const int n1 = platesize_ + 1;
     const int chunk = 256;
@@ -1321,9 +1352,28 @@ int FisheyeHost::build_forward_device(std::string *why) {
     });
     lua_->set_global("__blinky_forward", Value());
     if (rc != 0 || bad.load()) return -1;
+    // with a globe_plate script: the texel owners the device could not decide, from ray_to_plate_index on
+    // the very ray build_forward makes for the texel
+    std::vector<uint32_t> owner_patches(undecided_texels.size());
+    if (!undecided_texels.empty()) {
+        const int ps = platesize_;
+        const int ntexel_items = static_cast<int>((undecided_texels.size() + chunk - 1) / chunk);
+        rc = run_inverse_workers(undecided_texels.size() >= 4096 ? fallback_threads_ : 1, ntexel_items, display_unused, [&](Worker &w, int item, int *) {
+            const size_t b = static_cast<size_t>(item) * chunk, e = std::min(undecided_texels.size(), b + chunk);
+            for (size_t k = b; k < e; ++k) {
+                const uint32_t t = undecided_texels[k];
+                const int px = static_cast<int>(t % ps), py = static_cast<int>(t / ps % ps), plate = static_cast<int>(t / ps / ps);
+                float ray[3];
+                plate_uv_to_ray(plate, static_cast<double>(px) / ps, static_cast<double>(py) / ps, ray);
+                owner_patches[k] = t | (ray_to_plate_index(w, ray) == plate ? kOwnerPatchOwned : 0u);
+            }
+            return 0;
+        });
+        if (rc != 0) return -1;
+    }
     int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
     std::vector<std::pair<uint32_t, int>> messages;
-    if (!device_builder_->forward_finish(patches, idx_.data(), tint_.data(), display, &messages, why)) {
+    if (!device_builder_->forward_finish(patches, owner_patches, idx_.data(), tint_.data(), display, &messages, why)) {
         std::fill(idx_.begin(), idx_.end(), -1);
         std::fill(tint_.begin(), tint_.end(), 255);
         return 1;
@@ -1331,9 +1381,15 @@ int FisheyeHost::build_forward_device(std::string *why) {
     std::sort(messages.begin(), messages.end());
     for (auto &m : messages) print("%d > maxdiff\n", m.second);
     for (int i = 0; i < kMaxPlates; ++i) plates_[i].display = display[i];
-    char info[160];
-    snprintf(info, sizeof info, "device (forward): %zu of %zu grid points re-evaluated by the interpreter", undecided.size(),
-             static_cast<size_t>(numplates_) * n1 * n1);
+    char info[200];
+    if (fn_globe_plate_.is_function()) {
+        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points and %zu of %zu texel owners re-evaluated by the interpreter",
+                 undecided.size(), static_cast<size_t>(numplates_) * n1 * n1, undecided_texels.size(),
+                 static_cast<size_t>(numplates_) * platesize_ * platesize_);
+    } else {
+        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points re-evaluated by the interpreter", undecided.size(),
+                 static_cast<size_t>(numplates_) * n1 * n1);
+    }
     build_info_ = info;
     return 0;
 }

@@ -129,10 +129,16 @@ public:
     // raw script probes: 1 = values, 0 = nil, -1 = bad return, -2 = no such function, -3 = script error
     int lens_inverse(double x, double y, double out[3]);
     int lens_forward(double rx, double ry, double rz, double *x, double *y);
+    // the globe's globe_plate(x, y, z) as ray_to_plate_index reads it: 1 = a number (*plate =
+    // (int)(ptrdiff_t) of the last value returned), 0 = no value / nil / not a number (*plate = -1)
+    int globe_plate(double x, double y, double z, int *plate);
 
     // C++/CUDA source of the current lens_inverse (lua_transpile.h); false + reason when the
-    // lens is outside the transpilable subset
-    bool lens_device_source(bool cuda, std::string *source, std::string *why, bool forward = false);
+    // lens is outside the transpilable subset.  with_globe_plate: a globe_plate script of the globe is
+    // translated into the same unit (what the device builder compiles)
+    bool lens_device_source(bool cuda, std::string *source, std::string *why, bool forward = false, bool with_globe_plate = false);
+    // the globe's globe_plate translated alone; false + reason when there is none or it does not translate
+    bool globe_plate_device_source(bool cuda, std::string *source, std::string *why);
 
     // pure converters, exposed for the Lua-visible wrappers
     static void latlon_to_ray(double lat, double lon, float ray[3]);

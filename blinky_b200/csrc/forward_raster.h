@@ -100,12 +100,21 @@ FWD_HD void fwd_set(const FwdGeom &g, const FwdOut &o, int lx, int ly, unsigned 
     if (!ongrid) fwd_atomic_max(&o.tintkey[at], key);
 }
 
+// a texel owner the host decided (kOwnerPatchOwned | texel)
+FWD_HD void fwd_apply_owner_patch(unsigned char *owner, uint32_t patch) {
+    owner[patch & ~kOwnerPatchOwned] = (patch & kOwnerPatchOwned) ? kOwnerOwned : 0u;
+}
+
 // draw_quad (fisheye.c:2246-2338) for the texel (plate, px, py); key orders the writers like the
 // reference's loops do (plate ascending, py descending, px ascending): the highest key wins.
-FWD_HD void fwd_raster_texel(const FwdGeom &g, const FwdPoint *grid, const FwdOut &o, int plate, int py, int px) {
+// owner: the owner plane of a globe_plate globe (kOwnerOwned per texel), nullptr for the plate argmax.
+FWD_HD void fwd_raster_texel(const FwdGeom &g, const FwdPoint *grid, const FwdOut &o, int plate, int py, int px,
+                             const unsigned char *owner = nullptr) {
     const int ps = g.ps, n1 = ps + 1;
-    // the texel belongs to this plate only if the plate wins the ray's argmax (:2193-2199)
-    {
+    if (owner) {
+        if (!(owner[(static_cast<size_t>(plate) * ps + py) * ps + px] & kOwnerOwned)) return;
+    } else {
+        // the texel belongs to this plate only if the plate wins the ray's argmax (:2193-2199)
         const LensBuildParams::PlateF &P = g.plates[plate];
         double u = static_cast<double>(px) / ps, v = static_cast<double>(py) / ps;
         u -= 0.5;

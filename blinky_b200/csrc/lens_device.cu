@@ -22,7 +22,10 @@ namespace {
 // ray_to_plate_uv, :1984-2013 set_from_ray, :1922-1960 rubix grid) line by line: after the ray is
 // narrowed to float32 everything is IEEE +,-,*,/ and sqrt, compiled with --fmad=false, so it is
 // bit-identical to the host.
-const char *kKernelSource = R"KRN(
+//
+// The text is kept in pieces so that a globe with a globe_plate script can replace the plate argmax
+// (kernel_tail): every other globe gets exactly kKernelHead + kKernelArgmax + kKernelTexel + kKernelEnd.
+const char *kKernelHead = R"KRN(
 struct LtParams {
     int width, height, platesize, numplates;
     double scale;
@@ -54,13 +57,26 @@ extern "C" __global__ void __launch_bounds__(128) lt_build(const __grid_constant
             const float inv = 1 / len;
             ray[0] *= inv; ray[1] *= inv; ray[2] *= inv;
         }
-        int best = 0;
+)KRN";
+
+const char *kKernelArgmax = R"KRN(        int best = 0;
         double best_dp = -2;
         for (int i = 0; i < P.numplates; ++i) {
             const double dp = (double)lt_dot3(ray, P.plates[i].forward);
             if (dp > best_dp) { best_dp = dp; best = i; }
         }
-        const LtPlate &p = P.plates[best];
+)KRN";
+
+// ray_to_plate_index through the globe's script (fisheye.c:2027-2033) and set_from_ray's range checks:
+// a plate outside 0..5 leaves the pixel unmapped; plates numplates..5 are whatever the host keeps there
+const char *kKernelGlobePlateOpen = R"KRN(#ifdef LT_HAS_GLOBE_PLATE
+        int best = -1;
+        lt_globe_plate(c, (double)ray[0], (double)ray[1], (double)ray[2], &best);
+        if (best >= 0 && best < 6) {
+#else
+)KRN";
+
+const char *kKernelTexel = R"KRN(        const LtPlate &p = P.plates[best];
         const double px_ = (double)lt_dot3(p.right, ray);
         const double py_ = (double)lt_dot3(p.up, ray);
         const double pz_ = (double)lt_dot3(p.forward, ray);
@@ -76,7 +92,14 @@ extern "C" __global__ void __launch_bounds__(128) lt_build(const __grid_constant
                 out = 0x80000000u | (ongrid ? 0x40000000u : 0u) | (unsigned)(best * ps * ps + px + py * ps);
             }
         }
-    }
+)KRN";
+
+const char *kKernelGlobePlateClose = R"KRN(#ifdef LT_HAS_GLOBE_PLATE
+        }
+#endif
+)KRN";
+
+const char *kKernelEnd = R"KRN(    }
     if (c.flag) out |= 0x20000000u;
     cand[(size_t)ly * P.width + lx] = out;
 }
@@ -138,6 +161,40 @@ extern "C" __global__ void __launch_bounds__(128) lt_forward_points(const __grid
     grid[point] = out;
     status[point] = st;
 }
+)KRN";
+
+// Forward builder, texel owners (globes with a globe_plate script only): the texel (plate, px, py) is drawn
+// only if globe_plate picks `plate` for the texel's ray (fisheye.c:2193-2199).  lt_plate_to_ray at
+// u = px/ps, v = py/ps is the float arithmetic of fwd_raster_texel / plate_uv_to_ray.  One byte per texel:
+// kOwnerOwned, plus kOwnerRisk (and an entry in `undecided`) where the host has to decide.
+const char *kForwardOwnerKernelSource = R"KRN(
+#ifdef LT_HAS_GLOBE_PLATE
+extern "C" __global__ void __launch_bounds__(128) lt_forward_owner(const __grid_constant__ LtParams P, unsigned char *__restrict__ owner,
+                                                                   unsigned *__restrict__ undecided, unsigned *__restrict__ counter,
+                                                                   unsigned undecided_cap) {
+    const int ps = P.platesize;
+    const int px = blockIdx.x * blockDim.x + threadIdx.x, py = blockIdx.y, plate = blockIdx.z;
+    if (px >= ps) return;
+    const unsigned texel = ((unsigned)plate * ps + py) * ps + px;
+    Ctx c;
+    c.flag = 0;
+    c.steps = 0;
+    c.plates = P.plates;
+    c.numplates = P.numplates;
+    lt_init_mut(c);
+    double ray[3];
+    lt_plate_to_ray(c, LtD((double)plate), LtD((double)px / ps), LtD((double)py / ps), ray);
+    int sel = -1;
+    lt_globe_plate(c, ray[0], ray[1], ray[2], &sel);
+    unsigned char o = sel == plate ? 1 : 0;
+    if (c.flag) {
+        o |= 2;
+        const unsigned at = atomicAdd(counter, 1u);
+        if (at < undecided_cap) undecided[at] = texel;
+    }
+    owner[texel] = o;
+}
+#endif
 )KRN";
 
 struct Nvrtc {
@@ -211,6 +268,7 @@ Driver &driver() {
 struct LensDevice::Module {
     CUmodule mod = nullptr;
     CUfunction fn = nullptr;
+    CUfunction owner_fn = nullptr;  // forward modules of globes with a globe_plate script
 };
 
 // device buffers that live between forward_points() and forward_finish()
@@ -220,8 +278,10 @@ struct LensDevice::ForwardState {
     FwdPoint *grid = nullptr;
     unsigned char *status = nullptr;
     unsigned *undecided = nullptr;
-    unsigned *counters = nullptr;  // [0] undecided points, [1] nil results, [2] messages, [3..8] display flags
+    unsigned *counters = nullptr;  // [0] undecided points, [1] nil results, [2] messages, [3..8] display flags, [9] undecided owners
     unsigned nil_count = 0;
+    unsigned char *owner = nullptr;       // [numplates * ps * ps] texel owners; nullptr: the plate argmax decides
+    unsigned *owner_undecided = nullptr;
 };
 
 namespace {
@@ -243,9 +303,15 @@ __global__ void fwd_stale_kernel(FwdPoint *grid, const unsigned char *status, in
     if (t < 2 * (ps + 1)) fwd_stale_chain(grid, status, ps, numplates, t);
 }
 
-__global__ void __launch_bounds__(128) fwd_raster_kernel(const __grid_constant__ FwdGeom g, const FwdPoint *__restrict__ grid, FwdOut o) {
+__global__ void fwd_owner_patch_kernel(unsigned char *owner, const uint32_t *patches, unsigned n) {
+    const unsigned k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) fwd_apply_owner_patch(owner, patches[k]);
+}
+
+__global__ void __launch_bounds__(128) fwd_raster_kernel(const __grid_constant__ FwdGeom g, const FwdPoint *__restrict__ grid, FwdOut o,
+                                                         const unsigned char *__restrict__ owner) {
     const int px = blockIdx.x * blockDim.x + threadIdx.x;
-    if (px < g.ps) fwd_raster_texel(g, grid, o, static_cast<int>(blockIdx.z), static_cast<int>(blockIdx.y), px);
+    if (px < g.ps) fwd_raster_texel(g, grid, o, static_cast<int>(blockIdx.z), static_cast<int>(blockIdx.y), px, owner);
 }
 
 __global__ void fwd_resolve_kernel(const unsigned *__restrict__ idxkey, const unsigned *__restrict__ tintkey, int32_t *__restrict__ idx,
@@ -270,11 +336,17 @@ void LensDevice::drop_forward_state() {
     cudaFree(fwd_->status);
     cudaFree(fwd_->undecided);
     cudaFree(fwd_->counters);
+    cudaFree(fwd_->owner);
+    cudaFree(fwd_->owner_undecided);
     delete fwd_;
     fwd_ = nullptr;
 }
 
-const char *LensDevice::kernel_tail(bool forward) { return forward ? kForwardKernelSource : kKernelSource; }
+std::string LensDevice::kernel_tail(bool forward, bool globe_plate) {
+    if (forward) return globe_plate ? std::string(kForwardKernelSource) + kForwardOwnerKernelSource : std::string(kForwardKernelSource);
+    if (!globe_plate) return std::string(kKernelHead) + kKernelArgmax + kKernelTexel + kKernelEnd;
+    return std::string(kKernelHead) + kKernelGlobePlateOpen + kKernelArgmax + "#endif\n" + kKernelTexel + kKernelGlobePlateClose + kKernelEnd;
+}
 
 bool LensDevice::compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log) {
     Nvrtc &n = nvrtc();
@@ -282,7 +354,7 @@ bool LensDevice::compile(const std::string &lens_source, bool forward, std::vect
         *log = n.why;
         return false;
     }
-    const std::string src = lens_source + (forward ? kForwardKernelSource : kKernelSource);
+    const std::string src = lens_source + kernel_tail(forward, source_has_globe_plate(lens_source));
     nvrtcProgram prog;
     nvrtcResult rc = n.CreateProgram(&prog, src.c_str(), "lens.cu", 0, nullptr, nullptr);
     if (rc != NVRTC_SUCCESS) {
@@ -336,6 +408,7 @@ LensDevice::Module *LensDevice::module_for(const std::string &lens_source, bool 
     Module *m = new Module;
     CUresult cr = d.ModuleLoadData(&m->mod, cubin.data());
     if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, forward ? "lt_forward_points" : "lt_build");
+    if (cr == CUDA_SUCCESS && forward && source_has_globe_plate(lens_source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
     if (cr != CUDA_SUCCESS) {
         if (m->mod) d.ModuleUnload(m->mod);
         delete m;
@@ -395,7 +468,9 @@ bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p,
     return ok;
 }
 
-bool LensDevice::forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided, std::string *err) {
+bool LensDevice::forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
+                                std::vector<uint32_t> *undecided_texels, std::string *err) {
+    undecided_texels->clear();
     kernel_ms_ = 0;
     drop_forward_state();
     Module *m = module_for(lens_source, true, err);
@@ -415,6 +490,11 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
     if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->undecided, kUndecidedCap * sizeof(unsigned));
     if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->counters, 16 * sizeof(unsigned));
     if (ce == cudaSuccess) ce = cudaMemset(fwd_->counters, 0, 16 * sizeof(unsigned));
+    const size_t ntexels = static_cast<size_t>(p.numplates) * p.platesize * p.platesize;
+    if (m->owner_fn) {
+        if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->owner, ntexels);
+        if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->owner_undecided, kUndecidedCap * sizeof(unsigned));
+    }
     if (ce != cudaSuccess) {
         *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
         drop_forward_state();
@@ -430,6 +510,13 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
     cudaEventRecord(e0, nullptr);
     CUresult cr = d.LaunchKernel(m->fn, static_cast<unsigned>((n1 + block - 1) / block), static_cast<unsigned>(n1), static_cast<unsigned>(p.numplates), block, 1, 1, 0,
                                  nullptr, args, nullptr);
+    if (cr == CUDA_SUCCESS && m->owner_fn) {
+        unsigned *owner_counter = fwd_->counters + 9;
+        void *oargs[] = {&params, &fwd_->owner, &fwd_->owner_undecided, &owner_counter, &cap};
+        const unsigned ps = static_cast<unsigned>(p.platesize);
+        cr = d.LaunchKernel(m->owner_fn, (ps + block - 1) / block, ps, static_cast<unsigned>(p.numplates), block, 1, 1, 0, nullptr, oargs, nullptr);
+        if (cr == CUDA_SUCCESS) ++launches_;
+    }
     cudaEventRecord(e1, nullptr);
     unsigned counters[16] = {};
     bool ok = cr == CUDA_SUCCESS;
@@ -445,6 +532,10 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
         *err = "too many grid points need the interpreter (" + std::to_string(counters[0]) + ")";
         ok = false;
     }
+    if (ok && counters[9] > kUndecidedCap) {
+        *err = "too many texel owners need the interpreter (" + std::to_string(counters[9]) + ")";
+        ok = false;
+    }
     if (ok) {
         float ms = 0;
         cudaEventElapsedTime(&ms, e0, e1);
@@ -453,6 +544,8 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
         fwd_->nil_count = counters[1];
         undecided->resize(counters[0]);
         if (counters[0]) cudaMemcpy(undecided->data(), fwd_->undecided, counters[0] * sizeof(unsigned), cudaMemcpyDeviceToHost);
+        undecided_texels->resize(counters[9]);
+        if (counters[9]) cudaMemcpy(undecided_texels->data(), fwd_->owner_undecided, counters[9] * sizeof(unsigned), cudaMemcpyDeviceToHost);
     }
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
@@ -460,8 +553,8 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
     return ok;
 }
 
-bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, int32_t *idx, uint8_t *tint, int display[6],
-                                std::vector<std::pair<uint32_t, int>> *messages, std::string *err) {
+bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
+                                uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) {
     if (!fwd_) {
         *err = "forward_finish without forward_points";
         return false;
@@ -469,6 +562,7 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, int32_
     const LensBuildParams &p = fwd_->p;
     const size_t npix = static_cast<size_t>(p.width) * p.height;
     ForwardPatch *d_patches = nullptr;
+    uint32_t *d_owner_patches = nullptr;
     unsigned *d_keys = nullptr;  // idxkey[npix] then tintkey[npix]
     FwdMessage *d_messages = nullptr;
     int32_t *d_idx = nullptr;
@@ -488,6 +582,15 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, int32_
             ++launches_;
         }
         for (const ForwardPatch &pt : patches) any_nil = any_nil || pt.status != 1;
+    }
+    if (ce == cudaSuccess && !owner_patches.empty() && fwd_->owner) {
+        ce = cudaMalloc(&d_owner_patches, owner_patches.size() * sizeof(uint32_t));
+        if (ce == cudaSuccess) ce = cudaMemcpy(d_owner_patches, owner_patches.data(), owner_patches.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+        if (ce == cudaSuccess) {
+            const unsigned n = static_cast<unsigned>(owner_patches.size());
+            fwd_owner_patch_kernel<<<(n + 255) / 256, 256>>>(fwd_->owner, d_owner_patches, n);
+            ++launches_;
+        }
     }
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
@@ -510,7 +613,7 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, int32_
         memcpy(g.plates, p.plates, sizeof g.plates);
         FwdOut o{d_keys, d_keys + npix, fwd_->counters, d_messages};
         dim3 grid((p.platesize + 127) / 128, p.platesize, p.numplates);
-        fwd_raster_kernel<<<grid, 128>>>(g, fwd_->grid, o);
+        fwd_raster_kernel<<<grid, 128>>>(g, fwd_->grid, o, fwd_->owner);
         fwd_resolve_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256>>>(d_keys, d_keys + npix, d_idx, d_tint, npix, p.platesize);
         launches_ += 2;
         cudaEventRecord(e1, nullptr);
@@ -538,6 +641,7 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, int32_
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     cudaFree(d_patches);
+    cudaFree(d_owner_patches);
     cudaFree(d_keys);
     cudaFree(d_messages);
     cudaFree(d_idx);

@@ -52,6 +52,16 @@ struct ForwardPatch {
     int32_t lx, ly;
 };
 
+// the owner plane of the forward builder (globes with a globe_plate script): one byte per texel
+// (plate * ps + py) * ps + px
+constexpr uint8_t kOwnerOwned = 1u;  // globe_plate picks this texel's plate for the texel's ray
+constexpr uint8_t kOwnerRisk = 2u;   // not provably the host's answer: the host decides
+// a texel owner the host decided: the texel index, | kOwnerPatchOwned when the texel is owned
+constexpr uint32_t kOwnerPatchOwned = 0x80000000u;
+
+// True when a translated source defines lt_globe_plate (lua_transpile.h).
+inline bool source_has_globe_plate(const std::string &lens_source) { return lens_source.find("\n#define LT_HAS_GLOBE_PLATE 1\n") != std::string::npos; }
+
 // What FisheyeHost needs from a GPU (implemented by LensDevice).  CPU-only contexts have no
 // builder and take the interpreter.
 class DeviceLensBuilder {
@@ -60,12 +70,15 @@ public:
     // inverse lenses: one candidate entry per screen pixel
     virtual bool build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) = 0;
     // forward lenses, step 1: screen position of every plate grid point; `undecided` receives
-    // the points the host has to evaluate itself
-    virtual bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided, std::string *err) = 0;
-    // step 2: host results patched in, quads rasterised in the reference's order (last writer
-    // wins), map resolved.  messages: (order key, value) of every "%d > maxdiff" the reference prints.
-    virtual bool forward_finish(const std::vector<ForwardPatch> &patches, int32_t *idx, uint8_t *tint, int display[6],
-                                std::vector<std::pair<uint32_t, int>> *messages, std::string *err) = 0;
+    // the points the host has to evaluate itself.  When the source has a globe_plate, the texel
+    // owners are computed too and `undecided_texels` receives the texels the host has to decide.
+    virtual bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
+                                std::vector<uint32_t> *undecided_texels, std::string *err) = 0;
+    // step 2: host results patched in (grid points, texel owners), quads rasterised in the reference's
+    // order (last writer wins), map resolved.  messages: (order key, value) of every "%d > maxdiff" the
+    // reference prints.
+    virtual bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
+                                uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) = 0;
 };
 
 class LensDevice : public DeviceLensBuilder {
@@ -77,13 +90,16 @@ public:
     // Fills cand[width*height].  Returns false (reason in *err) when NVRTC is unavailable,
     // the source does not compile, or a CUDA call fails.
     bool build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) override;
-    bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided, std::string *err) override;
-    bool forward_finish(const std::vector<ForwardPatch> &patches, int32_t *idx, uint8_t *tint, int display[6],
-                        std::vector<std::pair<uint32_t, int>> *messages, std::string *err) override;
+    bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
+                        std::vector<uint32_t> *undecided_texels, std::string *err) override;
+    bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx, uint8_t *tint,
+                        int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) override;
 
     // the fixed CUDA source appended to a translated lens (the per-pixel / per-grid-point tail);
-    // exposed so that the CPU test-suite can run the very same text through a host shim
-    static const char *kernel_tail(bool forward);
+    // exposed so that the CPU test-suite can run the very same text through a host shim.
+    // globe_plate: the source defines lt_globe_plate — the inverse tail then lets it pick the plate and
+    // the forward tail gains the owner kernel; without it the tails are unchanged.
+    static std::string kernel_tail(bool forward, bool globe_plate = false);
 
     // compile only (no GPU needed): used by the CPU test-suite and by build()
     static bool compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log);

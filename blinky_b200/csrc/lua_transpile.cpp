@@ -60,6 +60,7 @@ struct FuncInfo {
     std::string cname;
     int arity = -1;
     std::vector<int> res_types;  // per result: -1 unknown yet, else static_cast<int>(VT::Num / VT::Bool)
+    std::vector<bool> exact_params;  // per parameter: a plain double (only entry points have such parameters)
     bool in_progress = false;
     bool done = false;
     std::string code;
@@ -69,46 +70,115 @@ class Transpiler {
 public:
     explicit Transpiler(State &L) : L_(L) { collect_builtins(); }
 
-    TranspileResult run(const Value &entry, int nparams, int nresults, const char *what) {
+    // entry: the lens function (nullptr: globe_plate alone); globe_plate (may be nullptr) joins the same
+    // translation unit: one function table, one set of constant tables, one set of script-level slots
+    TranspileResult run(const Value *entry, int nparams, int nresults, const char *what, const Value *globe_plate) {
         TranspileResult r;
+        bool in_globe_plate = false;
         try {
             const std::string name = what;
-            if (!entry.is_function()) fail(name + " is not a function");
-            const Function *fn = static_cast<const Function *>(entry.obj());
-            if (fn->cfn) fail(name + " is a C function");
-            if (fn->proto->nparams != nparams || fn->proto->is_vararg) fail(name + " must take exactly " + std::to_string(nparams) + " arguments");
-            // pass 1: which script-level variables does the lens assign?
+            const Function *fn = entry ? check_entry(*entry, nparams, name) : nullptr;
+            const Function *gp = nullptr;
+            if (globe_plate) {
+                in_globe_plate = true;
+                gp = check_entry(*globe_plate, 3, "globe_plate");
+                in_globe_plate = false;
+            }
+            // pass 1: which script-level variables do the functions assign?
             std::set<const Function *> seen;
-            scan_function(fn, seen);
-            entry_fn_ = fn;
-            FuncInfo &fi = gen_function(fn);
-            if (fi.arity != nresults) fail(name + " must return " + (nresults == 3 ? std::string("three") : std::to_string(nresults)) + " numbers (or nil)");
-            for (int t : fi.res_types)
-                if (t == static_cast<int>(VT::Bool)) fail(name + " must return numbers, not booleans");
+            if (fn) {
+                scan_function(fn, seen);
+                entry_fns_.insert(fn);
+            }
+            if (gp) {
+                in_globe_plate = true;
+                scope_ = "globe_plate";
+                scan_function(gp, seen);
+                entry_fns_.insert(gp);
+                scope_ = "lens";
+                in_globe_plate = false;
+            }
+            FuncInfo *fip = nullptr;
+            if (fn) {
+                FuncInfo &fi = gen_function(fn);
+                if (fi.arity != nresults) fail(name + " must return " + (nresults == 3 ? std::string("three") : std::to_string(nresults)) + " numbers (or nil)");
+                for (int t : fi.res_types)
+                    if (t == static_cast<int>(VT::Bool)) fail(name + " must return numbers, not booleans");
+                fip = &fi;
+            }
+            FuncInfo *gip = nullptr;
+            if (gp) {
+                in_globe_plate = true;
+                scope_ = "globe_plate";
+                FuncInfo &gi = gen_function(gp);
+                for (int t : gi.res_types)
+                    if (t == static_cast<int>(VT::Bool)) fail("globe_plate must return numbers, not booleans");
+                scope_ = "lens";
+                in_globe_plate = false;
+                gip = &gi;
+            }
             std::ostringstream o;
             o << "LT_FN void lt_init_mut(Ctx &c) {\n    (void)c;\n";
             for (size_t i = 0; i < mutable_init_.size(); ++i) o << "    c.mg[" << i << "] = LtD(" << num_literal(mutable_init_[i]) << ");\n";
             o << "}\n";
-            if (mutable_init_.size() > 32) fail("too many script-level variables are assigned by the lens");
+            if (mutable_init_.size() > 32) fail(std::string("too many script-level variables are assigned by the ") + (gp ? "lens and globe_plate" : "lens"));
             o << tables_.str();
             for (const std::string &c : order_) o << c << "\n";
-            o << "LT_FN bool lt_entry(Ctx &c";
-            for (int i = 0; i < nparams; ++i) o << ", double a" << i;
-            o << ", LtD *r) { return " << fi.cname << "(c";
-            for (int i = 0; i < nparams; ++i) o << ", a" << i;
-            o << ", r); }\n";
+            if (fip) {
+                o << "LT_FN bool lt_entry(Ctx &c";
+                for (int i = 0; i < nparams; ++i) o << ", double a" << i;
+                o << ", LtD *r) { return " << fip->cname << "(c";
+                for (int i = 0; i < nparams; ++i) o << ", a" << i;
+                o << ", r); }\n";
+            }
+            if (gip) emit_globe_plate_entry(o, *gip);
             r.ok = true;
             r.source = o.str();
             r.num_functions = static_cast<int>(order_.size());
             r.num_mutable = static_cast<int>(mutables_.size());
         } catch (Fail &f) {
             r.ok = false;
-            r.error = f.why;
+            r.error = in_globe_plate ? "globe_plate: " + f.why : f.why;
         }
         return r;
     }
 
 private:
+    const Function *check_entry(const Value &entry, int nparams, const std::string &name) {
+        if (!entry.is_function()) fail(name + " is not a function");
+        const Function *fn = static_cast<const Function *>(entry.obj());
+        if (fn->cfn) fail(name + " is a C function");
+        if (fn->proto->nparams != nparams || fn->proto->is_vararg) fail(name + " must take exactly " + std::to_string(nparams) + " arguments");
+        return fn;
+    }
+
+    // ray_to_plate_index with a globe_plate script (fisheye.c:2027-2033, :1634-1651): the LAST value returned
+    // counts; none, nil or a non-number is plate -1; a number d becomes (int)(ptrdiff_t)d (lua_tointeger).
+    // That conversion is a decision: it is flagged when an integer lies within d's error bound, and when d is
+    // NaN, infinite or outside int range, where x86 and CUDA convert differently.
+    void emit_globe_plate_entry(std::ostringstream &o, const FuncInfo &gi) {
+        const int k = gi.arity;
+        o << "#define LT_HAS_GLOBE_PLATE 1\n";
+        o << "LT_FN int lt_plate_int(Ctx &c, LtD x) {\n"
+             "    if (!(fabs(x.v) < 2147483000.0)) { c.flag |= LT_RISK_NEAR; return -1; }\n"
+             "    if (!(x.e == 0.0)) {\n"
+             "        const double n = rint(x.v);\n"
+             "        if (!(fabs(x.v - n) > 2.0 * x.e)) c.flag |= LT_RISK_NEAR;\n"
+             "    }\n"
+             "    return (int)x.v;\n"
+             "}\n";
+        o << "LT_FN bool lt_globe_plate(Ctx &c, double x, double y, double z, int *plate) {\n";
+        o << "    LtD r[" << std::max(1, k) << "];\n";
+        o << "    *plate = -1;\n";
+        if (k == 0) {
+            o << "    " << gi.cname << "(c, x, y, z, r);\n    return false;\n}\n";  // never returns a value
+            return;
+        }
+        o << "    if (!" << gi.cname << "(c, x, y, z, r)) return false;\n";
+        o << "    *plate = lt_plate_int(c, r[" << k - 1 << "]);\n";
+        o << "    return true;\n}\n";
+    }
+
     // ------------------------------------------------------------------ builtins
     void add_builtin(const Value &v, const std::string &name, bool libm) {
         if (v.is_function()) builtins_[v.obj()] = BuiltinInfo{name, libm};
@@ -181,7 +251,7 @@ private:
             return;
         }
         if (!cur.is_number()) {
-            fail("the lens assigns script-level variable '" + var_name(fn, target) + "' whose current value is not a number", target->line);
+            fail("the " + scope_ + " assigns script-level variable '" + var_name(fn, target) + "' whose current value is not a number", target->line);
         }
         mutables_[id] = static_cast<int>(mutable_init_.size());
         mutable_init_.push_back(cur.num());
@@ -193,7 +263,7 @@ private:
     }
     void scan_expr(const Function *fn, const Expr *e, std::set<const Function *> &seen) {
         if (!e) return;
-        if (e->k == EK::Function) fail("closures created inside the lens are not supported", e->line);
+        if (e->k == EK::Function) fail("closures created inside the " + scope_ + " are not supported", e->line);
         if (e->k == EK::Call) {
             Value callee;
             if (static_value(fn, e->l, &callee) && callee.is_function()) {
@@ -218,7 +288,7 @@ private:
         if (s->body) scan_block(fn, s->body, seen);
         for (const Block *b : s->blocks) scan_block(fn, b, seen);
         if (s->k == SK::GenFor) fail("generic 'for ... in' is not supported", s->line);
-        if (s->k == SK::LocalFunction) fail("local functions inside the lens are not supported", s->line);
+        if (s->k == SK::LocalFunction) fail("local functions inside the " + scope_ + " are not supported", s->line);
         if (s->k == SK::Goto || s->k == SK::Label) fail("goto is not supported", s->line);
     }
 
@@ -332,7 +402,7 @@ private:
         Gen g;
         g.fn = fn;
         g.fi = &fi;
-        g.is_entry = fn == entry_fn_;
+        g.is_entry = entry_fns_.count(fn) > 0;
         for (size_t i = 0; i < fn->proto->params.size(); ++i) {
             LocalInfo li;
             li.cname = "p" + std::to_string(i) + "_" + sanitize(fn->proto->params[i]->name);
@@ -348,6 +418,7 @@ private:
         for (size_t i = 0; i < fn->proto->params.size(); ++i) {
             const LocalInfo &li = g.locals[fn->proto->params[i]];
             sig << (li.tainted ? ", LtD " : ", double ") << li.cname;
+            fi.exact_params.push_back(!li.tainted);
         }
         sig << ", LtD *r) {";
         line(g, "(void)c; (void)r;");
@@ -623,7 +694,7 @@ private:
                 res.push_back(o);
             };
             // the interpreter would print once per pixel; a silent device build would change the console output
-            if (n == "print") fail("print() inside the lens function", e->line);
+            if (n == "print") fail("print() inside the " + scope_ + " function", e->line);
             if (n == "math.abs") { need(1); one(std::string(tin ? "lt_fabs(" : "fabs(") + a[0].code + ")", tin); return res; }
             if (n == "math.sqrt") { need(1); one(std::string(tin ? "lt_sqrt(" : "sqrt(") + a[0].code + ")", tin); return res; }
             if (n == "math.floor" || n == "math.ceil") {
@@ -713,7 +784,12 @@ private:
         for (int i = 0; i < cf->proto->nparams; ++i) {
             if (static_cast<size_t>(i) < a.size()) {
                 if (a[static_cast<size_t>(i)].type != VT::Num) fail("non-numeric argument in a call to " + cf->proto->name, e->line);
-                callexpr << ", " << a[static_cast<size_t>(i)].code;
+                // an entry point (e.g. globe_plate called by the lens) takes exact doubles: an argument with an
+                // error bound is accepted only when that bound is zero at run time
+                if (fi.exact_params[static_cast<size_t>(i)] && a[static_cast<size_t>(i)].tainted)
+                    callexpr << ", lt_exact(c, " << a[static_cast<size_t>(i)].code << ")";
+                else
+                    callexpr << ", " << a[static_cast<size_t>(i)].code;
             } else {
                 callexpr << ", LT_NAN";  // missing argument = nil; using it would be an error in Lua too
             }
@@ -957,20 +1033,26 @@ private:
     std::vector<std::string> order_;
     std::ostringstream tables_;
     std::map<const Table *, std::string> table_names_;
-    const Function *entry_fn_ = nullptr;
+    std::set<const Function *> entry_fns_;  // their parameters are exact doubles
+    std::string scope_ = "lens";            // names the function being translated in error messages
     int next_local_ = 0;
 };
 
 }  // namespace
 
-TranspileResult transpile_lens(State &L, const Value &lens_inverse) {
+TranspileResult transpile_lens(State &L, const Value &lens_inverse, const Value *globe_plate) {
     Transpiler t(L);
-    return t.run(lens_inverse, 2, 3, "lens_inverse");
+    return t.run(&lens_inverse, 2, 3, "lens_inverse", globe_plate);
 }
 
-TranspileResult transpile_lens_forward(State &L, const Value &lens_forward) {
+TranspileResult transpile_lens_forward(State &L, const Value &lens_forward, const Value *globe_plate) {
     Transpiler t(L);
-    return t.run(lens_forward, 3, 2, "lens_forward");
+    return t.run(&lens_forward, 3, 2, "lens_forward", globe_plate);
+}
+
+TranspileResult transpile_globe_plate(State &L, const Value &globe_plate) {
+    Transpiler t(L);
+    return t.run(nullptr, 0, 0, "globe_plate", &globe_plate);
 }
 
 std::string transpile_prelude(bool cuda, bool noinline_user_functions) {

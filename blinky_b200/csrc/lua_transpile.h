@@ -40,9 +40,20 @@ struct TranspileResult {
 
 // names of the host-provided script functions (latlon_to_ray, ray_to_latlon, plate_to_ray)
 // are resolved through the State's current globals; `numplates` plates are baked in for plate_to_ray.
-TranspileResult transpile_lens(minilua::State &L, const minilua::Value &lens_inverse);
+//
+// globe_plate (optional): the globe's globe_plate(x, y, z) is translated into the same unit — one
+// function table (a helper both scripts call is emitted once), one set of constant tables and one set
+// of script-level slots, since lens and globe share one Lua state.  The source then also defines
+//   #define LT_HAS_GLOBE_PLATE 1
+//   bool lt_globe_plate(Ctx &c, double x, double y, double z, int *plate)
+// with the host's ray_to_plate_index semantics: false and *plate = -1 for no value / nil, otherwise the
+// last value returned, converted like lua_tointeger (risk-flagged where that conversion is not certain).
+// Without globe_plate the source is exactly what it was before.
+TranspileResult transpile_lens(minilua::State &L, const minilua::Value &lens_inverse, const minilua::Value *globe_plate = nullptr);
 // the same for lens_forward(x, y, z) -> x, y; entry point: bool lt_entry(Ctx &c, double a0, double a1, double a2, LtD *r)
-TranspileResult transpile_lens_forward(minilua::State &L, const minilua::Value &lens_forward);
+TranspileResult transpile_lens_forward(minilua::State &L, const minilua::Value &lens_forward, const minilua::Value *globe_plate = nullptr);
+// globe_plate alone: lt_init_mut, its functions and lt_globe_plate, without lt_entry
+TranspileResult transpile_globe_plate(minilua::State &L, const minilua::Value &globe_plate);
 
 // Support code the generated source needs.  cuda = true: __device__ functions; false: plain C++.
 std::string transpile_prelude(bool cuda, bool noinline_user_functions = false);

@@ -126,10 +126,12 @@ int blinky_set_rubixgrid(blinky_ctx *ctx, int numcells, double cell_size, double
  *                 with NVRTC and evaluated by one kernel — lens_inverse for every screen
  *                 pixel, or, for forward-only lenses, lens_forward for every plate grid point
  *                 followed by the quad rasterisation in the reference's writer order.
+ *                 A globe's globe_plate script is translated with the lens and picks the
+ *                 plate on the device too (for forward lenses: which plate owns each texel).
  *                 Results that are not provably the host's (error bounds on every libm call)
  *                 are re-evaluated by the interpreter, so the map is the same as the host
- *                 build's.  Lenses outside the translatable subset, globes with a
- *                 globe_plate script and CPU-only contexts fall back to threads < 0.
+ *                 build's.  Lenses or globe_plate scripts outside the translatable subset and
+ *                 CPU-only contexts fall back to threads < 0.
  * blinky_build_info() says which way the last build went.
  * On a GPU context the packed map, tile table and tint LUTs are uploaded too. */
 int blinky_build_lensmap(blinky_ctx *ctx, int width, int height, int platesize, int threads);
@@ -178,11 +180,19 @@ int64_t blinky_mapped_pixels(blinky_ctx *ctx);        /* M in the 5*W*H + M byte
  * return 1 = values, 0 = nil, negative = error */
 int blinky_lens_inverse(blinky_ctx *ctx, double x, double y, double ray_out[3]);
 int blinky_lens_forward(blinky_ctx *ctx, double rx, double ry, double rz, double *x, double *y);
+/* the globe's globe_plate(x, y, z) as the lensmap build reads it (ray_to_plate_index,
+ * fisheye.c:2027-2033): 1 = a plate (*plate = the last value returned, converted like
+ * lua_tointeger: (int)(ptrdiff_t)d), 0 = no value, nil or not a number (*plate = -1),
+ * negative = error (-2: the globe has no globe_plate, -3: script error) */
+int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate);
 /* The current lens function translated to C++ / CUDA C++ — what the device lensmap builder
  * compiles (SURVEY 8f).  flavour: bit 0 = CUDA (else plain C++), bit 1 = lens_forward (else
- * lens_inverse), bit 2 = append the fixed kernel (the per-pixel / per-grid-point tail) — with
- * bits 0 and 2 this is exactly what NVRTC is given.  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT when the lens is
- * outside the translatable subset (reason: blinky_last_error). */
+ * lens_inverse), bit 2 = append the fixed kernel (the per-pixel / per-grid-point tail) and, when
+ * the globe has a globe_plate script, translate it into the same unit — with bits 0 and 2 this is
+ * exactly what NVRTC is given.  bit 3 = the globe's globe_plate translated alone (bit 0 still picks
+ * CUDA; bits 1 and 2 are ignored).  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT
+ * when the lens (or globe_plate) is missing or outside the translatable subset (reason:
+ * blinky_last_error). */
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize);
 /* F_WriteConfig text; returns bytes needed (excluding NUL) */
 int blinky_write_config(blinky_ctx *ctx, char *buf, size_t bufsize);
