@@ -98,6 +98,7 @@ _SIGNATURES = [
     ("blinky_save_globe", c_int, [_CTX, c_void_p, c_char_p]),
     ("blinky_set_kernel", c_int, [_CTX, c_int]),
     ("blinky_set_background", c_int, [_CTX, c_void_p]),
+    ("blinky_set_face_layout", c_int, [_CTX, c_int, c_void_p, c_int]),
     ("blinky_warp_device", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p]),
     ("blinky_warp_device_view", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     ("blinky_warp_device_view_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -201,6 +202,7 @@ class Fisheye:
             self._ctx = None
             raise BlinkyError(rc, msg)
         self.device = device
+        self._layout = None   # set_face_layout: (rowbytes, origins) or None for dense faces
         self._lib.blinky_set_basedir(self._ctx, (basedir or SCRIPT_DIR).encode())
         if palette is not None:
             self.set_palette(palette)
@@ -397,6 +399,7 @@ class Fisheye:
         return bool(self._lib.blinky_saveglobe_pending(self._ctx))
 
     def save_globe(self, faces: np.ndarray, directory: str):
+        """faces: one frame, dense [numplates, ps, ps] or, with a face layout, the frame's surface"""
         f = np.ascontiguousarray(faces, dtype=np.uint8)
         self._check(self._lib.blinky_save_globe(self._ctx, f.ctypes.data, directory.encode()))
 
@@ -412,14 +415,45 @@ class Fisheye:
             assert bg.size == self.width * self.height
             self._check(self._lib.blinky_set_background(self._ctx, bg.ctypes.data))
 
+    def set_face_layout(self, rowbytes: int | None = None, origins=None):
+        """Where the plates sit in each frame of the faces (blinky_set_face_layout): rows of ``rowbytes`` bytes,
+        plate i at byte x, row y = origins[i].  No arguments (or rowbytes 0) restores the dense [numplates, ps, ps]
+        faces.  While a layout is set, warp / warp_view / warp_host take the frame stride of a [N, rows, rowbytes]
+        faces tensor or array from its stride(0) (otherwise rows * rowbytes, rows = max(y) + platesize)."""
+        if not rowbytes:
+            self._check(self._lib.blinky_set_face_layout(self._ctx, 0, None, 0))
+            self._layout = None
+            return
+        org = np.ascontiguousarray(np.asarray(origins, dtype=np.int64).reshape(-1, 2))
+        if org.min(initial=0) < np.iinfo(np.int32).min or org.max(initial=0) > np.iinfo(np.int32).max:
+            raise ValueError("set_face_layout: origins must fit 32-bit integers")
+        org = org.astype(np.int32)
+        self._check(self._lib.blinky_set_face_layout(self._ctx, int(rowbytes), org.ctypes.data, len(org)))
+        self._layout = (int(rowbytes), [tuple(int(v) for v in o) for o in org])
+
+    @property
+    def face_layout(self):
+        """(rowbytes, [(x, y), ...]) of the face layout, or None for dense faces"""
+        return self._layout
+
+    def _face_stride(self, faces) -> int:
+        """the default frame stride of `faces`: dense frames, or the face layout's surfaces"""
+        if self._layout is None:
+            return self.numplates * self.platesize * self.platesize
+        if hasattr(faces, "stride") and callable(faces.stride) and faces.dim() >= 3:
+            return faces.stride(0) * faces.element_size()
+        if isinstance(faces, np.ndarray) and faces.ndim >= 3:
+            return faces.strides[0]
+        rowbytes, origins = self._layout
+        return (max(y for _, y in origins) + self.platesize) * rowbytes
+
     def warp(self, d_faces, d_out, nframes: int = 1, face_stride: int | None = None, out_stride: int | None = None,
              stream: int | None = None, rgba: bool = False, tables=None):
         """device-resident batch; d_faces/d_out are torch CUDA tensors (or raw device addresses).  May be captured
         into a CUDA graph (torch.cuda.graph; see release_captures).  tables (RGBA): per-frame palette tables, see
         warp_view."""
-        ps2 = self.platesize * self.platesize
         if face_stride is None:
-            face_stride = self.numplates * ps2
+            face_stride = self._face_stride(d_faces)
         if out_stride is None:
             out_stride = self.width * self.height * (4 if rgba else 1)
         if tables is not None:
@@ -459,7 +493,7 @@ class Fisheye:
         if tables is not None:
             d_tables, table_stride = self._table_args(tables, rgba, nframes)
         if face_stride is None:
-            face_stride = self.numplates * self.platesize * self.platesize
+            face_stride = self._face_stride(d_faces)
         bpp = 4 if rgba else 1
         shape = getattr(d_screen, "shape", None)
         if rowbytes is None:
@@ -485,11 +519,13 @@ class Fisheye:
                   y0: int = 0, nframes: int | None = None, dst_rowbytes: int | None = None,
                   face_stride: int | None = None, dst_frame_stride: int | None = None) -> np.ndarray:
         """end to end from host buffers (numpy uint8, or raw addresses of pinned memory)."""
-        ps2 = self.platesize * self.platesize
         if face_stride is None:
-            face_stride = self.numplates * ps2
+            face_stride = self._face_stride(faces)
         if nframes is None:
-            nframes = int(faces.size // face_stride) if isinstance(faces, np.ndarray) else 1
+            if self._layout is not None and isinstance(faces, np.ndarray) and faces.ndim >= 3:
+                nframes = faces.shape[0]
+            else:
+                nframes = int(faces.size // face_stride) if isinstance(faces, np.ndarray) else 1
         if dst is None:
             dst = np.zeros((nframes, self.height, self.width), np.uint8)
         if dst_rowbytes is None:

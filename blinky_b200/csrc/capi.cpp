@@ -34,6 +34,8 @@ struct blinky_ctx {
     std::string err;
     std::string scratch;
     uint8_t palmaps[BLINKY_MAX_PLATES * 256];
+    int layout_rowbytes = 0;              // blinky_set_face_layout: 0 = dense faces
+    std::vector<int32_t> layout_origins;  // (x, y) per plate
 };
 
 namespace {
@@ -331,12 +333,37 @@ int blinky_write_config(blinky_ctx *ctx, char *buf, size_t bufsize) {
     return static_cast<int>(s.size());
 }
 
+int blinky_set_face_layout(blinky_ctx *ctx, int rowbytes, const int32_t *origins, int nplates) {
+    if (rowbytes < 0) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_face_layout: rowbytes < 0");
+    if (rowbytes > 0) {
+        if (!origins) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_face_layout: origins is NULL");
+        if (nplates < 1 || nplates > BLINKY_MAX_PLATES) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_face_layout: nplates must be 1..6");
+        for (int i = 0; i < 2 * nplates; ++i)
+            if (origins[i] < 0) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_face_layout: negative plate origin");
+        ctx->layout_origins.assign(origins, origins + 2 * nplates);
+    } else {
+        ctx->layout_origins.clear();
+    }
+    ctx->layout_rowbytes = rowbytes;
+    if (ctx->dev) ctx->dev->set_face_layout(rowbytes, ctx->layout_origins.data(), static_cast<int>(ctx->layout_origins.size() / 2));
+    return BLINKY_OK;
+}
+
 int blinky_saveglobe_pending(blinky_ctx *ctx) { return ctx->host.saveglobe_pending() ? 1 : 0; }
 int blinky_save_globe(blinky_ctx *ctx, const uint8_t *faces_host, const char *directory) {
     if (!faces_host) return set_err(ctx, BLINKY_E_INVALID, "faces is NULL");
     if (!ctx->host.built()) return set_err(ctx, BLINKY_E_STATE, "no lensmap built (plate size unknown)");
-    return ctx->host.save_globe(faces_host, directory ? directory : "") ? BLINKY_OK
-                                                                        : set_err(ctx, BLINKY_E_INVALID, "could not write a PCX file");
+    if (ctx->layout_rowbytes > 0) {
+        // every plate is written: each needs an origin that fits the row pitch
+        const int ps = ctx->host.platesize(), n = static_cast<int>(ctx->layout_origins.size() / 2);
+        if (ctx->host.numplates() > n) return set_err(ctx, BLINKY_E_INVALID, "blinky_save_globe: the face layout has no origin for every plate");
+        for (int i = 0; i < n; ++i)
+            if (static_cast<int64_t>(ctx->layout_origins[2 * i]) + ps > ctx->layout_rowbytes)
+                return set_err(ctx, BLINKY_E_INVALID, "blinky_save_globe: a plate of the face layout does not fit its rowbytes");
+    }
+    return ctx->host.save_globe(faces_host, directory ? directory : "", ctx->layout_rowbytes, ctx->layout_origins.data())
+               ? BLINKY_OK
+               : set_err(ctx, BLINKY_E_INVALID, "could not write a PCX file");
 }
 
 // ---- GPU-only entry points: no CPU fallback, fail loudly ------------------
@@ -436,7 +463,7 @@ int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_str
     if (dst_rowbytes < ctx->host.width() + x0) return set_err(ctx, BLINKY_E_INVALID, "dst_rowbytes too small for the view rectangle");
     return ctx->dev->warp_host(faces_host, face_stride, dst_host, dst_frame_stride, dst_rowbytes, x0, y0, nframes, keep_unmapped != 0)
                ? BLINKY_OK
-               : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+               : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int64_t blinky_upload_bytes_per_frame(blinky_ctx *ctx) {

@@ -574,7 +574,7 @@ std::string FisheyeHost::write_config() const {
 // globe export (fisheye.c:1396-1486)
 // ---------------------------------------------------------------------------
 
-std::vector<uint8_t> FisheyeHost::plate_pcx(const uint8_t *faces, int plate, bool with_margins) {
+std::vector<uint8_t> FisheyeHost::plate_pcx(const uint8_t *faces, int plate, bool with_margins, int rowbytes, const int32_t *origins) {
     const int ps = platesize_;
     std::vector<uint8_t> out(128, 0);  // pcx_t header (engine/NQ/client.h:377-391), zero-filled
     auto put16 = [&](size_t at, int v) {
@@ -596,10 +596,14 @@ std::vector<uint8_t> FisheyeHost::plate_pcx(const uint8_t *faces, int plate, boo
     w.L = lua_.get();
     w.globe_plate = fn_globe_plate_;
     w.has_globe_plate = fn_globe_plate_.is_function();
-    const uint8_t *data = faces + static_cast<size_t>(plate) * ps * ps;
+    const bool layout = rowbytes > 0;
+    const size_t pitch = layout ? static_cast<size_t>(rowbytes) : static_cast<size_t>(ps);
+    const uint8_t *plate_data = layout ? faces + static_cast<size_t>(origins[2 * plate + 1]) * pitch + static_cast<size_t>(origins[2 * plate])
+                                       : faces + static_cast<size_t>(plate) * ps * ps;
     out.reserve(128 + static_cast<size_t>(ps) * ps * 2 + 769);
     for (int i = 0; i < ps; ++i) {
         double v = static_cast<double>(i) / ps;
+        const uint8_t *data = plate_data + static_cast<size_t>(i) * pitch;
         for (int j = 0; j < ps; ++j) {
             double u = static_cast<double>(j) / ps;
             uint8_t col = *data++;
@@ -623,13 +627,13 @@ std::vector<uint8_t> FisheyeHost::plate_pcx(const uint8_t *faces, int plate, boo
     return out;
 }
 
-bool FisheyeHost::save_globe(const uint8_t *faces, const std::string &dir) {
+bool FisheyeHost::save_globe(const uint8_t *faces, const std::string &dir, int rowbytes, const int32_t *origins) {
     save_pending_ = false;
     bool ok = true;
     for (int i = 0; i < numplates_; ++i) {
         char name[64];
         snprintf(name, sizeof name, "%s%d.pcx", save_name_.c_str(), i);
-        std::vector<uint8_t> pcx = plate_pcx(faces, i, save_with_margins_ != 0);
+        std::vector<uint8_t> pcx = plate_pcx(faces, i, save_with_margins_ != 0, rowbytes, origins);
         std::string path = dir.empty() ? std::string(name) : dir + "/" + name;
         FILE *f = fopen(path.c_str(), "wb");
         if (f) {

@@ -122,9 +122,10 @@ public:
     bool saveglobe_pending() const { return save_pending_; }
     // PCX image of one plate exactly as WritePCXplate builds it (texels another plate
     // owns are blanked to 0xFE unless with_margins)
-    std::vector<uint8_t> plate_pcx(const uint8_t *faces, int plate, bool with_margins);
+    // rowbytes > 0: the faces follow a face layout (face_layout.h) with the plates' (x, y) origins
+    std::vector<uint8_t> plate_pcx(const uint8_t *faces, int plate, bool with_margins, int rowbytes = 0, const int32_t *origins = nullptr);
     // writes <dir>/<name><i>.pcx for every plate, prints "Wrote ..." and disarms the request
-    bool save_globe(const uint8_t *faces, const std::string &dir);
+    bool save_globe(const uint8_t *faces, const std::string &dir, int rowbytes = 0, const int32_t *origins = nullptr);
 
     // raw script probes: 1 = values, 0 = nil, -1 = bad return, -2 = no such function, -3 = script error
     int lens_inverse(double x, double y, double out[3]);

@@ -22,6 +22,7 @@
 #include <type_traits>
 
 #include "../../include/blinky_b200.h"
+#include "face_layout.h"
 #include "tile_plan.h"
 
 namespace blinky {
@@ -108,9 +109,12 @@ __device__ __forceinline__ size_t out_offset(const WarpParams &p, uint32_t pix, 
 // never read; a partly mapped quad is stored pixel by pixel.
 // TABLES (RGBA only): frame f is expanded through its own table at
 // p.rgba + f * p.table_words, in every kernel below.
+// LAYOUT: the faces follow a face layout (face_layout.h): a texel's address is
+// its plate-space offset split by layout_texel, in every kernel below.  The
+// layout is the kernels' last parameter, which the dense instances never read.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
-__global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams p) {
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
+__global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams p, const __grid_constant__ FaceLayoutParams lay) {
     __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
     __shared__ uint32_t s_rgba[RGBA ? 256 : 1];
     if (RUBIX) {
@@ -139,7 +143,8 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             v[c][k] = 0;
-            if (ent[k] & BLINKY_LM_VALID) v[c][k] = ld_face(faces + (ent[k] & BLINKY_LM_INDEX_MASK));
+            if (ent[k] & BLINKY_LM_VALID)
+                v[c][k] = ld_face(LAYOUT ? faces + layout_texel(ent[k] & BLINKY_LM_INDEX_MASK, lay) : faces + (ent[k] & BLINKY_LM_INDEX_MASK));
         }
     }
 
@@ -185,8 +190,8 @@ __global__ void __launch_bounds__(kThreads) warp_gather_kernel(const WarpParams 
 // unaligned strides, or a view rectangle whose origin or pitch is not a
 // multiple of 4 pixels) — a correctness path for ragged sizes, not a fast path.
 // --------------------------------------------------------------------------
-template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
-__global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams p) {
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
+__global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams p, const __grid_constant__ FaceLayoutParams lay) {
     const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
     if (i >= p.npix) return;
     const uint32_t ent = __ldg(reinterpret_cast<const uint32_t *>(p.lensmap4) + i);
@@ -194,7 +199,7 @@ __global__ void __launch_bounds__(kThreads) warp_scalar_kernel(const WarpParams 
     const uint8_t *faces = p.faces + static_cast<size_t>(blockIdx.y) * p.face_stride;
     uint32_t b;
     if (ent & BLINKY_LM_VALID) {
-        b = ld_face(faces + (ent & BLINKY_LM_INDEX_MASK));
+        b = ld_face(LAYOUT ? faces + layout_texel(ent & BLINKY_LM_INDEX_MASK, lay) : faces + (ent & BLINKY_LM_INDEX_MASK));
         if (RUBIX) {
             const uint32_t t = (ent >> BLINKY_LM_TINT_SHIFT) & 7u;
             if (t != BLINKY_LM_TINT_NONE) b = __ldg(p.lut + t * 256 + b);
@@ -364,8 +369,8 @@ __device__ __forceinline__ void st_stream_u32x8(const uint64_t (&a)[8], const ui
 // vacate at the end.
 constexpr int kGatherRows = 8, kGatherFrames = 4;
 
-template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
-__device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, uint32_t lane) {
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
+__device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, uint32_t lane, const FaceLayoutParams &lay) {
     const uint32_t nfg = (p.nframes + kGatherFrames - 1) / kGatherFrames;
     const uint32_t fg = item % nfg, rest = item / nfg;
     const uint32_t rg = rest % (kTileH / kGatherRows), gt = rest / (kTileH / kGatherRows);
@@ -379,6 +384,11 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
 #pragma unroll
     for (int j = 0; j < kGatherRows; ++j) e[j] = __ldg(ent32 + j * kTileW + lane);
     if (x >= width) return;
+    size_t at[kGatherRows];   // LAYOUT: the entries' byte offsets in a frame, split once for all frames
+    if (LAYOUT) {
+#pragma unroll
+        for (int j = 0; j < kGatherRows; ++j) at[j] = layout_texel(e[j] & BLINKY_LM_INDEX_MASK, lay);
+    }
     uint32_t v[kGatherFrames][kGatherRows];
 #pragma unroll
     for (int g = 0; g < kGatherFrames; ++g) {
@@ -387,7 +397,7 @@ __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, 
 #pragma unroll
         for (int j = 0; j < kGatherRows; ++j) {
             v[g][j] = 0x100u;   // "take the background"
-            if (e[j] & BLINKY_LM_VALID) v[g][j] = ld_face(faces + (e[j] & BLINKY_LM_INDEX_MASK));
+            if (e[j] & BLINKY_LM_VALID) v[g][j] = ld_face(LAYOUT ? faces + at[j] : faces + (e[j] & BLINKY_LM_INDEX_MASK));
         }
     }
 #pragma unroll
@@ -429,14 +439,18 @@ constexpr int kRingMinBlocks = 16;
 
 // KEEP (keep_unmapped): only mapped pixels are written.  The host gives this instance the BOX tiles alone (EMPTY tiles
 // have nothing to write); a partly mapped quad is stored pixel by pixel and the background is never read.
-template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
-__global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm) {
+// LAYOUT: the tensor maps view each frame's surface, (x, y, 1, frame); a unit's box origin is moved from plate to
+// surface coordinates by the plate's origin when the issue cursor enters the unit.  Boxes that overhang their plate
+// stage neighbouring texels, which no entry refers to.
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
+__global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __grid_constant__ RingParams p, const __grid_constant__ RingTmaps tm,
+                                                                      const __grid_constant__ FaceLayoutParams lay) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // XOR with a parameter that is always zero: keeps ptxas from re-reading the special register
     // (S2R, tens of cycles) at every `lane == 0` test instead of holding the lane number in a register
     const uint32_t lane = threadIdx.x ^ p.zero;
     if (blockIdx.x >= p.ring_grid) {   // the CTAs behind the ring warps: one gather item each
-        gather_item<RUBIX, RGBA, KEEP, TABLES>(p, blockIdx.x - p.ring_grid, lane);
+        gather_item<RUBIX, RGBA, KEEP, TABLES, LAYOUT>(p, blockIdx.x - p.ring_grid, lane, lay);
         return;
     }
     const uint32_t R = p.ring_bytes;
@@ -570,6 +584,11 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
                 c_bx = static_cast<int16_t>(dy & 0xffffu);
                 c_by = static_cast<int16_t>(dy >> 16);
                 c_plate = static_cast<int>(dz & 7u);
+                if (LAYOUT) {
+                    c_bx += lay.org_x[c_plate];
+                    c_by += lay.org_y[c_plate];
+                    c_plate = 0;
+                }
                 c_bytes = ((dz >> 16) & 0xffu) * (dz >> 24) * 128u;
             } else {
                 ++c_unit;  // GATHER / EMPTY / no unit: nothing to stage
@@ -805,8 +824,9 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
 // --------------------------------------------------------------------------
 constexpr int kGatherFramesPerCta = 4;
 
-template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
-__global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid_constant__ RingParams p, const uint32_t first_tile) {
+template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
+__global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid_constant__ RingParams p, const uint32_t first_tile,
+                                                                    const __grid_constant__ FaceLayoutParams lay) {
     const uint32_t tid = threadIdx.x;
     const uint4 d = __ldg(reinterpret_cast<const uint4 *>(p.tiles + first_tile + blockIdx.x));
     const uint32_t type = (d.z >> 8) & kTileTypeMask;
@@ -846,6 +866,11 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
         bgv[j] = 0;
         if (!KEEP && !(e[j] & BLINKY_LM_VALID) && y < height) bgv[j] = __ldg(p.bg + static_cast<size_t>(y) * width + x);
     }
+    size_t at[4];   // LAYOUT: the entries' byte offsets in a frame, split once for all frames
+    if (LAYOUT) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) at[j] = layout_texel(e[j] & BLINKY_LM_INDEX_MASK, lay);
+    }
     uint32_t v[kGatherFramesPerCta][4];
 #pragma unroll
     for (int g = 0; g < kGatherFramesPerCta; ++g) {
@@ -854,7 +879,7 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             v[g][j] = bgv[j];
-            if (e[j] & BLINKY_LM_VALID) v[g][j] = ld_face(faces + (e[j] & BLINKY_LM_INDEX_MASK));
+            if (e[j] & BLINKY_LM_VALID) v[g][j] = ld_face(LAYOUT ? faces + at[j] : faces + (e[j] & BLINKY_LM_INDEX_MASK));
         }
     }
 #pragma unroll
@@ -882,6 +907,11 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
+// the instance's flags in last_kernel, after rubix= and rgba=
+std::string variant_tags(bool keep, bool tables, bool layout) {
+    return std::string(keep ? ",keep=1" : "") + (tables ? ",tables=1" : "") + (layout ? ",layout=1" : "");
+}
+
 constexpr uint32_t kCaptureSlots = 4096;   // work counters for captured ring launches (see WarpDevice::CaptureStream)
 
 }  // namespace
@@ -905,6 +935,7 @@ struct WarpDevice::TmapSet {   // host-side: the descriptors travel in the kerne
     const void *faces = nullptr;
     size_t face_stride = 0;
     int nframes = 0;
+    uint32_t rowbytes = 0, rows = 0;   // face layout's surface (0: the dense [plate][ps][ps] frames)
     RingTmaps table;
     uint64_t last_use = 0;
 };
@@ -1086,8 +1117,61 @@ bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
     return true;
 }
 
+void WarpDevice::set_face_layout(int rowbytes, const int32_t *origins, int nplates) {
+    layout_rowbytes_ = rowbytes > 0 ? rowbytes : 0;
+    layout_origins_.assign(origins && rowbytes > 0 ? origins : nullptr, origins && rowbytes > 0 ? origins + 2 * nplates : nullptr);
+}
+
+// The face layout against the current lensmap (the plate size and the plates it samples change with every build):
+// false, with err_code_ BLINKY_E_INVALID, when it does not fit; otherwise the kernels' view of it in *lay.
+bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay) {
+    err_code_ = BLINKY_E_INVALID;
+    const int n = static_cast<int>(layout_origins_.size() / 2);
+    const uint64_t rb = static_cast<uint64_t>(layout_rowbytes_), ps = static_cast<uint64_t>(platesize_);
+    memset(lay, 0, sizeof *lay);
+    uint64_t rows = 0;
+    for (int pl = 0; pl < n; ++pl) {
+        const uint64_t x = static_cast<uint64_t>(layout_origins_[2 * pl]), y = static_cast<uint64_t>(layout_origins_[2 * pl + 1]);
+        if (x + ps > rb) {
+            err_ = "face layout: plate " + std::to_string(pl) + " at x = " + std::to_string(x) + " does not fit rowbytes " + std::to_string(rb) +
+                   " with plate size " + std::to_string(ps);
+            return false;
+        }
+        rows = std::max(rows, y + ps);
+        lay->plate_base[pl] = y * rb + x;
+        lay->org_x[pl] = static_cast<int32_t>(x);
+        lay->org_y[pl] = static_cast<int32_t>(y);
+    }
+    for (int pl = n; pl < kLayoutPlates; ++pl) {
+        const int *r = plate_rect_[pl];
+        if (display_[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
+            err_ = "face layout: the lensmap samples plate " + std::to_string(pl) + ", which has no origin (the layout has " + std::to_string(n) + ")";
+            return false;
+        }
+    }
+    if (nframes > 1 && static_cast<uint64_t>(face_stride) < rows * rb) {
+        err_ = "face layout: face_stride " + std::to_string(face_stride) + " is smaller than a frame's surface (" + std::to_string(rows) + " rows of " +
+               std::to_string(rb) + " bytes)";
+        return false;
+    }
+    lay->rowbytes = static_cast<uint32_t>(rb);
+    lay->ps = static_cast<uint32_t>(ps);
+    lay->ps2 = static_cast<uint32_t>(ps * ps);
+    lay->div_ps = make_fastdiv(lay->ps);
+    lay->div_ps2 = make_fastdiv(lay->ps2);
+    layout_rows_ = static_cast<uint32_t>(rows);
+    err_code_ = BLINKY_E_CUDA;
+    return true;
+}
+
 bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
                       bool rgba, size_t out_pitch, bool keep_unmapped, const uint32_t *d_tables, size_t table_stride) {
+    return warp_faces(d_faces, face_stride, layout_rowbytes_ > 0, d_out, out_stride, nframes, stream, rgba, out_pitch, keep_unmapped, d_tables,
+                      table_stride);
+}
+
+bool WarpDevice::warp_faces(const void *d_faces, size_t face_stride, bool use_layout, void *d_out, size_t out_stride, int nframes, void *stream,
+                            bool rgba, size_t out_pitch, bool keep_unmapped, const uint32_t *d_tables, size_t table_stride) {
     err_code_ = BLINKY_E_CUDA;
     if (!have_lensmap_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
@@ -1112,7 +1196,19 @@ bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size
     // stride aligned to 4 pixels
     const bool vec_ok = (width_ % 4 == 0) && (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (pitch % (4 * opx) == 0) &&
                         (out_stride % (4 * opx) == 0 || nframes == 1);
-    const bool tiled_ok = have_plan_ && vec_ok &&
+    FaceLayoutParams lay_params;
+    const FaceLayoutParams *lay = nullptr;
+    if (use_layout) {
+        if (!make_layout(face_stride, nframes, &lay_params)) return false;
+        lay = &lay_params;
+    }
+    // TMA: 16-byte aligned rows, and box x coordinates (plate origins included) on 16-byte boundaries
+    bool layout_tma_ok = true;
+    if (lay) {
+        layout_tma_ok = lay->rowbytes % 16 == 0;
+        for (size_t i = 0; i < layout_origins_.size(); i += 2) layout_tma_ok = layout_tma_ok && layout_origins_[i] % 16 == 0;
+    }
+    const bool tiled_ok = have_plan_ && vec_ok && layout_tma_ok &&
                           (!plan_has_box_ || (reinterpret_cast<uintptr_t>(d_faces) % 16 == 0 && (face_stride % 16 == 0 || nframes == 1)));
     // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -1122,9 +1218,9 @@ bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size
     const bool capturing = cap != cudaStreamCaptureStatusNone;
     const bool ok = variant_ == BLINKY_KERNEL_GATHER || !tiled_ok
                         ? launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
-                                      d_tables, table_stride)
+                                      d_tables, table_stride, lay)
                         : launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
-                                      d_tables, table_stride, capturing);
+                                      d_tables, table_stride, capturing, lay);
     if (capturing) {
         captured_ = bg_captured_ = true;
         bool known = false;
@@ -1163,10 +1259,10 @@ bool WarpDevice::release_captures() {
     return true;
 }
 
-WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stride, int nframes) {
+WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stride, int nframes, uint32_t rowbytes, uint32_t rows) {
     const uint64_t tick = ++tmap_tick_;
     for (TmapSet *t : tmap_sets_)
-        if (t->faces == d_faces && t->face_stride == face_stride && t->nframes == nframes) {
+        if (t->faces == d_faces && t->face_stride == face_stride && t->nframes == nframes && t->rowbytes == rowbytes && t->rows == rows) {
             t->last_use = tick;
             return t;
         }
@@ -1192,13 +1288,17 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
     t->faces = d_faces;
     t->face_stride = face_stride;
     t->nframes = nframes;
+    t->rowbytes = rowbytes;
+    t->rows = rows;
     t->last_use = tick;
     memset(&t->table, 0, sizeof t->table);
     const cuuint64_t ps = static_cast<cuuint64_t>(platesize_);
-    // 4-D view of the globe: (x, y, plate, frame)
-    const cuuint64_t dims[4] = {ps, ps, static_cast<cuuint64_t>(numplates_), static_cast<cuuint64_t>(nframes)};
-    const cuuint64_t fstride = nframes > 1 ? static_cast<cuuint64_t>(face_stride) : ps * ps * static_cast<cuuint64_t>(numplates_);
-    const cuuint64_t strides[3] = {ps, ps * ps, fstride};
+    // 4-D view of the globe: (x, y, plate, frame); with a face layout (rowbytes > 0) one frame's surface is the single
+    // "plate": (x, y, 1, frame), rowbytes wide and `rows` high
+    const cuuint64_t fw = rowbytes ? rowbytes : ps, fh = rowbytes ? rows : ps, np = rowbytes ? 1 : static_cast<cuuint64_t>(numplates_);
+    const cuuint64_t dims[4] = {fw, fh, np, static_cast<cuuint64_t>(nframes)};
+    const cuuint64_t fstride = nframes > 1 ? static_cast<cuuint64_t>(face_stride) : fw * fh * np;
+    const cuuint64_t strides[3] = {fw, fw * fh, fstride};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
     for (size_t si = 0; si < shapes_.size() && si < static_cast<size_t>(kMaxShapes); ++si) {
         const uint32_t w16 = shapes_[si] >> 8, h8 = shapes_[si] & 0xff;
@@ -1225,7 +1325,7 @@ constexpr int kRingWarpsDefault = 12;
 // Calls f(R, C, K, T) with std::bool_constant arguments for (rubix, rgba, keep, tables): one place turns the run-time
 // flags into the kernels' template arguments.  Per-frame tables exist only in RGBA: 12 combinations.
 template <typename F>
-static auto with_variant(bool rubix, bool rgba, bool keep, bool tables, F &&f) {
+static auto with_variant4(bool rubix, bool rgba, bool keep, bool tables, F &&f) {
     using T = std::true_type;
     using N = std::false_type;
     if (rubix) {
@@ -1238,9 +1338,18 @@ static auto with_variant(bool rubix, bool rgba, bool keep, bool tables, F &&f) {
     return keep ? f(N{}, N{}, T{}, N{}) : f(N{}, N{}, N{}, N{});
 }
 
-static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, bool tables, size_t smem, int *n) {
-    return with_variant(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) {
-        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value>;
+// ... and f(R, C, K, T, L) with the face layout's flag as well: 24 combinations
+template <typename F>
+static auto with_variant(bool rubix, bool rgba, bool keep, bool tables, bool layout, F &&f) {
+    if (layout) return with_variant4(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) { return f(R, C, K, T, std::true_type{}); });
+    return with_variant4(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) { return f(R, C, K, T, std::false_type{}); });
+}
+
+static const FaceLayoutParams kDenseLayout = {};   // the dense instances' last kernel argument (never read)
+
+static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, bool tables, bool layout, size_t smem, int *n) {
+    return with_variant(rubix, rgba, keep, tables, layout, [&](auto R, auto C, auto K, auto T, auto L) {
+        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>;
         cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
         if (e != cudaSuccess) return e;
         return cudaOccupancyMaxActiveBlocksPerMultiprocessor(n, kernel, 32, smem);
@@ -1248,7 +1357,8 @@ static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, bool tables, 
 }
 
 bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing) {
+                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing,
+                             const FaceLayoutParams *lay) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     RingParams p;
     p.tiles = static_cast<const TileDesc *>(d_tiles_);
@@ -1256,7 +1366,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     static const RingTmaps kNoTmaps = {};
     const RingTmaps *tm = &kNoTmaps;
     if (plan_has_box_) {
-        TmapSet *t = get_tmaps(d_faces, face_stride, nframes);
+        TmapSet *t = get_tmaps(d_faces, face_stride, nframes, lay ? lay->rowbytes : 0u, lay ? layout_rows_ : 0u);
         if (!t) return false;
         tm = &t->table;
     }
@@ -1278,7 +1388,8 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     p.height = height_;
     p.zero = 0;
     const bool rubix = rubix_;
-    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0) | (per_frame ? 8 : 0);
+    const bool layout = lay != nullptr;
+    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0) | (per_frame ? 8 : 0) | (layout ? 16 : 0);
     // The ring kernel takes the BOX tiles [0, nbox) and the EMPTY tiles; the GATHER tiles in between go to the
     // gather kernel K3 on the context's side stream (forked from and joined to the caller's stream), so the two
     // kernels share the GPU instead of queueing behind each other.  With keep_unmapped an EMPTY tile has nothing
@@ -1323,7 +1434,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     const size_t smem = static_cast<size_t>(ring_bytes) + fixed;
     if (ring_ctas_per_sm_[vi] == 0 || ring_smem_[vi] != smem) {
         int n = 0;
-        cudaError_t e = ring_config_v(rubix, rgba, keep, per_frame, smem, &n);
+        cudaError_t e = ring_config_v(rubix, rgba, keep, per_frame, layout, smem, &n);
         if (e != cudaSuccess) return fail("ring kernel configuration (shared memory / occupancy)", e);
         if (n < 1) {
             err_ = "ring kernel does not fit on an SM";
@@ -1386,14 +1497,16 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     }
     char buf[640];
     int nbuf = 0;
-    const char *tags = keep && per_frame ? ",keep=1,tables=1" : keep ? ",keep=1" : per_frame ? ",tables=1" : "";
+    const std::string tag_str = variant_tags(keep, per_frame, layout);
+    const char *tags = tag_str.c_str();
     // GATHER tiles: one-warp CTAs behind the ring warps in the same grid (see gather_item); only a plan without BOX and
     // EMPTY tiles (with keep_unmapped: without BOX tiles) launches the stand-alone gather kernel.
     snprintf(buf, sizeof buf, "%s", ngather_tiles_ == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
     if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
         dim3 g2(ngather_tiles_, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
-        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
-            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<g2, kThreads, 0, st>>>(p, nbox_tiles_);
+        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
+            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
+                <<<g2, kThreads, 0, st>>>(p, nbox_tiles_, lay ? *lay : kDenseLayout);
         });
         ++launches_;
         snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, g2.x, g2.y, kThreads);
@@ -1416,8 +1529,9 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
 
         p.ring_grid = grid;
         const uint32_t extra = merged_gather ? gather_items : 0u;
-        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
-            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid + extra, 32, smem, st>>>(p, *tm);
+        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
+            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
+                <<<grid + extra, 32, smem, st>>>(p, *tm, lay ? *lay : kDenseLayout);
         });
         ++launches_;
         nbuf = static_cast<int>(strlen(buf));
@@ -1432,7 +1546,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
 }
 
 bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride) {
+                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, const FaceLayoutParams *lay) {
     // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out
     // unless the caller made its own) — NOT this context's private stream.
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1457,19 +1571,22 @@ bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_ou
     // 4-pixel words: dense frames need W*H % 4 == 0, pitched ones W % 4 == 0 (no quad straddles two rows)
     const bool vector_ok = (p.pitched ? width_ % 4 == 0 && out_pitch % (4 * opx) == 0 : npix_ % 4 == 0) &&
                            (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (out_stride % (4 * opx) == 0 || nframes == 1);
-    const bool rubix = rubix_;
-    const char *tags = keep && per_frame ? ",keep=1,tables=1" : keep ? ",keep=1" : per_frame ? ",tables=1" : "";
+    const bool rubix = rubix_, layout = lay != nullptr;
+    const std::string tag_str = variant_tags(keep, per_frame, layout);
+    const char *tags = tag_str.c_str();
     char buf[160];
     if (vector_ok) {
         dim3 grid(static_cast<unsigned>(npix_pad_ / kPixelsPerBlock), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
-            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid, kThreads, 0, st>>>(p);
+        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
+            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
+                <<<grid, kThreads, 0, st>>>(p, lay ? *lay : kDenseLayout);
         });
         snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
     } else {
         dim3 grid(static_cast<unsigned>((npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, per_frame, [&](auto R, auto C, auto K, auto T) {
-            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value><<<grid, kThreads, 0, st>>>(p);
+        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
+            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
+                <<<grid, kThreads, 0, st>>>(p, lay ? *lay : kDenseLayout);
         });
         snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
     }
@@ -1534,10 +1651,16 @@ static bool is_pinned(const void *p) {
 
 bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
                            int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped) {
+    err_code_ = BLINKY_E_CUDA;
     if (!have_lensmap_) {
         err_ = "warp_host: no lensmap on the device (call blinky_build_lensmap)";
         return false;
     }
+    // with a face layout the plates' rectangles are read out of each frame's surface; the device copy stays dense
+    FaceLayoutParams lay;
+    const bool layout = layout_rowbytes_ > 0;
+    if (layout && !make_layout(face_stride, nframes, &lay)) return false;
+    const size_t src_pitch = layout ? lay.rowbytes : static_cast<size_t>(platesize_);
     CK(cudaSetDevice(device_));
     if (!ensure_slots()) return false;
     const size_t ps2 = static_cast<size_t>(platesize_) * platesize_;
@@ -1566,21 +1689,23 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
             const int *r = plate_rect_[pl];
             if (r[0] > r[2] || r[1] > r[3]) continue;
             const size_t rw = static_cast<size_t>(r[2] - r[0] + 1), rh = static_cast<size_t>(r[3] - r[1] + 1);
-            const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + r[0];
-            const uint8_t *from = src + off;
+            const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + r[0];   // in the dense device copy
+            const uint8_t *from = src + (layout ? lay.plate_base[pl] + static_cast<size_t>(r[1]) * src_pitch + r[0] : off);
+            size_t pitch = src_pitch;
             if (!src_pinned) {
                 uint8_t *stage = s.h_faces + off;
-                for (size_t y = 0; y < rh; ++y) memcpy(stage + y * platesize_, from + y * platesize_, rw);
+                for (size_t y = 0; y < rh; ++y) memcpy(stage + y * platesize_, from + y * src_pitch, rw);
                 from = stage;
+                pitch = static_cast<size_t>(platesize_);
             }
-            // a full-width rectangle is one contiguous run: copy it as such
-            const bool contiguous = rw == static_cast<size_t>(platesize_);
+            // a full-width rectangle of dense rows is one contiguous run: copy it as such
+            const bool contiguous = rw == static_cast<size_t>(platesize_) && pitch == rw;
             const size_t row = contiguous ? rw * rh : static_cast<size_t>(platesize_), rows = contiguous ? 1 : rh;
             cudaMemcpy3DBatchOp &op = ops[nops++];
             memset(&op, 0, sizeof op);
             op.src.type = cudaMemcpyOperandTypePointer;
             op.src.op.ptr.ptr = const_cast<uint8_t *>(from);
-            op.src.op.ptr.rowLength = row;
+            op.src.op.ptr.rowLength = contiguous ? row : pitch;
             op.src.op.ptr.layerHeight = rows;
             op.dst.type = cudaMemcpyOperandTypePointer;
             op.dst.op.ptr.ptr = s.d_faces + off;
@@ -1602,7 +1727,7 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         }
         if (!ok) break;
         s.dst = dst_host + static_cast<size_t>(f) * dst_frame_stride;
-        if (!warp(s.d_faces, slot_face_bytes_, s.d_out, slot_out_bytes_, 1, s.stream, false)) { ok = false; break; }
+        if (!warp_faces(s.d_faces, slot_face_bytes_, false, s.d_out, slot_out_bytes_, 1, s.stream, false)) { ok = false; break; }
         s.dst_rowbytes = dst_rowbytes;
         s.x0 = x0;
         s.y0 = y0;

@@ -11,6 +11,8 @@
 #include <string>
 #include <vector>
 
+#include "face_layout.h"
+
 namespace blinky {
 
 struct TilePlan;  // tile_plan.h
@@ -42,6 +44,9 @@ public:
     bool set_background(const uint8_t *bg_host);   // [H][W] or nullptr -> zeros
     bool set_rgba_table(const uint32_t table[256]);
     void set_kernel(int variant) { variant_ = variant; }
+    // face layout (face_layout.h) of the faces every later warp reads: rowbytes 0 = dense [plate][ps][ps] frames;
+    // origins: nplates (x, y) pairs.  Checked against the lensmap at each warp (BLINKY_E_INVALID when it does not fit).
+    void set_face_layout(int rowbytes, const int32_t *origins, int nplates);
 
     // size of the resident lensmap's view (0 before the first upload)
     int width() const { return width_; }
@@ -82,6 +87,10 @@ private:
     struct Slot;
     bool ensure_slots();
     bool fail(const char *what, int cuda_err);
+    bool make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay);
+    // warp() with the face layout (use_layout) or the dense frames warp_host stages
+    bool warp_faces(const void *d_faces, size_t face_stride, bool use_layout, void *d_out, size_t out_stride, int nframes, void *stream,
+                    bool rgba, size_t out_pitch = 0, bool keep_unmapped = false, const uint32_t *d_tables = nullptr, size_t table_stride = 0);
     void finalize_slot(Slot &s);
 
     int device_ = 0;
@@ -107,6 +116,9 @@ private:
     bool have_rgba_ = false;
     std::vector<int32_t> span_off_, spans_;
     int variant_ = 0;
+    int layout_rowbytes_ = 0;              // face layout: 0 = dense
+    std::vector<int32_t> layout_origins_;  // (x, y) per plate
+    uint32_t layout_rows_ = 0;             // rows of a frame's surface (set by make_layout)
 
     // tiled layout (ring kernel)
     struct TmapSet;
@@ -127,17 +139,19 @@ private:
     int ring_boxes_ = 0;                 // boxes a warp keeps in flight at most (BLINKY_RING_BOXES)
     size_t smem_per_sm_ = 233472;
     std::vector<uint16_t> shapes_;
-    std::vector<TmapSet *> tmap_sets_;   // small cache keyed by (faces ptr, stride, nframes)
+    std::vector<TmapSet *> tmap_sets_;   // small cache keyed by (faces ptr, stride, nframes, face layout's surface)
     uint64_t tmap_tick_ = 0;
     std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on (eagerly)
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
-    int ring_ctas_per_sm_[16] = {};      // per ring kernel instance: rubix | rgba << 1 | keep << 2 | per-frame tables << 3
-    size_t ring_smem_[16] = {};
-    TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes);
+    int ring_ctas_per_sm_[32] = {};      // per ring kernel instance: rubix | rgba << 1 | keep << 2 | per-frame tables << 3 | layout << 4
+    size_t ring_smem_[32] = {};
+    TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes, uint32_t rowbytes, uint32_t rows);
+    // lay: the face layout, nullptr for dense frames
     bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing);
+                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing,
+                     const FaceLayoutParams *lay);
     bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride);
+                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, const FaceLayoutParams *lay);
 
     // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
     // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are

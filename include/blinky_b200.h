@@ -210,6 +210,27 @@ int blinky_set_kernel(blinky_ctx *ctx, int kernel_variant);
  * vid.buffer, :802).  [height][width] bytes, NULL = all zero.  Uploaded once. */
 int blinky_set_background(blinky_ctx *ctx, const uint8_t *background_host);
 
+/* Face layout: where the plates sit in each frame of the faces the warps read, for hosts that render
+ * plates into surfaces of their own (a 3x2 atlas, viewports of one render target, a surface with a
+ * padded row pitch) and warp straight from there instead of repacking.  Each frame is a surface with
+ * rows of `rowbytes` bytes; plate i starts at byte x = origins[2i], row y = origins[2i+1], so texel
+ * (px, py) of plate i in frame f is at
+ *     faces + f * face_stride + (y + py) * rowbytes + x + px.
+ * rowbytes = 0 (origins ignored) restores the dense nframes x [numplates][ps][ps] faces, the default.
+ * Context state read when a warp is enqueued, like blinky_set_background: it applies to
+ * blinky_warp_device, _rgba, _view, _view_rgba, _view_rgba_tables, blinky_warp_host (the sampled
+ * rectangle of each plate is copied out of the surface), blinky_shard_warp_gather and blinky_save_globe.
+ * A captured warp keeps the layout in effect at capture; a later call does not change its replays.
+ * Works on host-only contexts (for blinky_save_globe).  BLINKY_E_INVALID, changing nothing, for
+ * rowbytes < 0, origins NULL with rowbytes > 0, nplates outside 1..6, or a negative coordinate.
+ * The plate size and the plates a lens samples change with every build, so each warp checks the
+ * layout against the current lensmap and fails with BLINKY_E_INVALID, launching nothing, when a plate
+ * the lensmap samples has no origin, a plate's x + ps exceeds rowbytes, or nframes > 1 and
+ * face_stride is less than the surface, max(y + ps) * rowbytes.  The ring kernel reads a layout
+ * through TMA, which needs rowbytes and every x origin to be multiples of 16 (and the faces 16-byte
+ * aligned, as for dense faces); any other layout is warped by the direct-gather kernel. */
+int blinky_set_face_layout(blinky_ctx *ctx, int rowbytes, const int32_t *origins, int nplates);
+
 /* Device-resident batch: d_faces -> d_out on `stream` (a cudaStream_t; NULL is
  * CUDA's default stream).  d_faces: nframes x [numplates][ps][ps]
  * bytes, frame stride face_stride bytes; d_out: nframes x [height][width]
@@ -239,7 +260,8 @@ int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
  *   - the faces, output and per-frame table pointers given at capture, with whatever they hold when the
  *     replay runs (so a cudaMemcpyAsync into the tables on the replay's stream changes the palette);
  *   - the background, rubix LUTs and RGBA table as they are when the replay runs (after a rebuild to
- *     another view size: the background of the captured size).
+ *     another view size: the background of the captured size);
+ *   - the face layout (blinky_set_face_layout) that was in effect at capture.
  * Each captured launch of the ring kernel takes one of 4096 work counters; when none is left the call
  * fails with BLINKY_E_STATE and launches nothing.  blinky_warp_host, blinky_shard_warp_gather,
  * blinky_build_lensmap, blinky_set_background and blinky_set_rgba_table must not be called while a
