@@ -429,6 +429,10 @@ LensDevice::Module *LensDevice::module_for(const std::string &lens_source, bool 
 
 bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) {
     kernel_ms_ = 0;
+    if (p.height > 65535) {   // one row of blocks per screen row, and gridDim.y is at most 65535
+        *err = "screen taller than 65535 rows, the device lens kernel's grid limit";
+        return false;
+    }
     Module *m = module_for(lens_source, false, err);
     if (!m) return false;
     Driver &d = driver();

@@ -133,6 +133,7 @@ TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int plate
     plan.width = width;
     plan.height = height;
     plan.platesize = platesize;
+    if (width > kMaxPlanExtent || height > kMaxPlanExtent) return plan;   // tile origins would not fit TileDesc::px / py
     plan.tiles_x = (width + kTileW - 1) / kTileW;
     plan.tiles_y = (height + kTileH - 1) / kTileH;
     // box heights come in multiples of 8 texel rows; if that needs more than kMaxShapes distinct

@@ -29,6 +29,10 @@ constexpr int kTilePixels = kTileW * kTileH;
 constexpr int kBoxBytesLimit = 16384;      // 14-bit offsets
 constexpr int kDefaultMaxBoxBytes = 8192;  // planner default (BLINKY_MAX_BOX overrides)
 constexpr int kMaxBoxW = 256, kMaxBoxH = 256;  // TMA box dimensions are at most 256 elements
+// A plan covers screens of at most 65536 x 65536 pixels: TileDesc::px / py hold tile origins in 16 bits.  For a
+// wider or taller screen make_tile_plan returns a plan without tiles, and the flat kernels (K1 / K0, which address
+// pixels by their dense index) serve the warp.
+constexpr int kMaxPlanExtent = 65536;
 
 enum TileType : uint8_t { TILE_EMPTY = 0, TILE_BOX = 1, TILE_GATHER = 2, TILE_BOX_FULL = 3 };
 // A plan uses at most kMaxShapes distinct box shapes: the kernel receives one TMA descriptor per
@@ -91,7 +95,8 @@ struct TilePlan {
 // packed: [height][width] entries in the BLINKY_LM_* format.  allow_box = false forces every
 // non-empty tile to GATHER (e.g. platesize not a multiple of 16, which TMA cannot address).
 // max_box_bytes <= 0: default / BLINKY_MAX_BOX.  Tile rows are classified on `threads` host
-// threads; the result does not depend on the thread count.
+// threads; the result does not depend on the thread count.  A screen wider or taller than kMaxPlanExtent gets a
+// plan without tiles.
 TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int platesize, bool allow_box, int threads = 1,
                         int max_box_bytes = 0);
 

@@ -1179,16 +1179,19 @@ bool WarpDevice::warp_faces(const void *d_faces, size_t face_stride, bool use_la
     }
     if (nframes <= 0) return true;
     if (nframes > 65535) {
+        err_code_ = BLINKY_E_INVALID;
         err_ = "warp: at most 65535 frames per launch";
         return false;
     }
     const size_t opx = rgba ? 4 : 1;
     if (rgba && (reinterpret_cast<uintptr_t>(d_out) % 4 != 0 || out_pitch % 4 != 0 || (nframes > 1 && out_stride % 4 != 0))) {
+        err_code_ = BLINKY_E_INVALID;
         err_ = "warp (RGBA): the output buffer, the row pitch and the frame stride must be 4-byte aligned";
         return false;
     }
     const size_t pitch = out_pitch ? out_pitch : static_cast<size_t>(width_) * opx;
     if (pitch < static_cast<size_t>(width_) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
+        err_code_ = BLINKY_E_INVALID;
         err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
         return false;
     }
