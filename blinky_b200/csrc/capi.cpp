@@ -64,6 +64,13 @@ int usable_cpus() {
     return n < 1 ? 1 : n;
 }
 
+// The tile plan of the current lensmap, classified on `threads` host threads.  TMA needs 16-byte aligned plate rows;
+// other plate sizes get GATHER tiles only.
+blinky::TilePlan current_plan(blinky_ctx *c, int threads) {
+    return blinky::make_tile_plan(c->host.packed().data(), c->host.width(), c->host.height(), c->host.platesize(), c->host.platesize() % 16 == 0,
+                                  threads);
+}
+
 bool upload(blinky_ctx *c) {
     if (!c->dev || !c->host.built()) return true;
     blinky::LensmapUpload lm;
@@ -82,8 +89,7 @@ bool upload(blinky_ctx *c) {
     lm.span_off = c->host.row_span_offsets().data();
     lm.spans = c->host.row_spans().data();
     lm.nspans = c->host.row_spans().size() / 2;
-    // TMA needs 16-byte aligned plate rows; other plate sizes use direct gathers only
-    blinky::TilePlan plan = blinky::make_tile_plan(lm.packed, lm.width, lm.height, lm.platesize, lm.platesize % 16 == 0, c->host.worker_threads());
+    blinky::TilePlan plan = current_plan(c, c->host.worker_threads());
     lm.plan = &plan;
     if (!c->dev->upload_lensmap(lm)) {
         c->err = c->dev->last_error();
@@ -390,43 +396,39 @@ int blinky_set_background(blinky_ctx *ctx, const uint8_t *bg) {
 
 namespace {
 
-// The one way into the device-resident warp: frames land in the view rectangle at (x0, y0) of screens with rows of
-// `rowbytes` bytes.  The dense entry points are the rectangle that is the whole screen.
-int warp_into_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
-                   int rowbytes, int x0, int y0, int nframes, bool keep_unmapped, void *stream, bool rgba,
-                   const uint32_t *d_tables = nullptr, size_t table_stride = 0) {
-    const size_t bpp = rgba ? 4 : 1;
-    uint8_t *origin = static_cast<uint8_t *>(d_screen) + static_cast<size_t>(y0) * static_cast<size_t>(rowbytes) + static_cast<size_t>(x0) * bpp;
-    return ctx->dev->warp(d_faces, face_stride, origin, screen_frame_stride, nframes, stream, rgba, static_cast<size_t>(rowbytes), keep_unmapped,
-                          d_tables, table_stride)
-               ? BLINKY_OK
-               : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
+// The one way into the device-resident warp: frames land in the view rectangle at (x0, y0) of the screens r.out, whose
+// rows are rowbytes bytes apart.  The dense entry points are the rectangle that is the whole screen.
+int warp_into_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0) {
+    const size_t bpp = r.rgba ? 4 : 1;
+    r.out_pitch = static_cast<size_t>(rowbytes);
+    r.out = static_cast<uint8_t *>(r.out) + static_cast<size_t>(y0) * r.out_pitch + static_cast<size_t>(x0) * bpp;
+    return ctx->dev->warp(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
-// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose d_tables / table_stride are checked here too
-int warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
-                     int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream, bool rgba,
-                     bool with_tables = false, const uint32_t *d_tables = nullptr, size_t table_stride = 0) {
+// The view entry points: the warp r in keep_unmapped / rgba mode into the view rectangle at (x0, y0), checked first.
+// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose r.tables / r.table_stride are checked here too.
+int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba, bool with_tables = false) {
     NEED_DEVICE(ctx);
-    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
+    r.keep_unmapped = keep_unmapped != 0;
+    r.rgba = rgba;
+    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : r.rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
     auto invalid = [&](const char *why) { return set_err(ctx, BLINKY_E_INVALID, std::string(name) + ": " + why); };
-    const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = rgba ? 4 : 1;
-    if (!d_faces || !d_screen) return invalid("NULL buffer");
+    const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = r.rgba ? 4 : 1;
+    if (!r.faces || !r.out) return invalid("NULL buffer");
     if (x0 < 0 || y0 < 0) return invalid("the view origin (x0, y0) must not be negative");
     if (static_cast<int64_t>(rowbytes) < (x0 + W) * bpp) return invalid("rowbytes too small for the view rectangle");
-    if (nframes > 1 && static_cast<uint64_t>(screen_frame_stride) < static_cast<uint64_t>((y0 + H) * rowbytes))
+    if (r.nframes > 1 && static_cast<uint64_t>(r.out_stride) < static_cast<uint64_t>((y0 + H) * rowbytes))
         return invalid("screen_frame_stride too small for the view rectangle");
-    if (rgba && ((reinterpret_cast<uintptr_t>(d_screen) + static_cast<uintptr_t>(y0) * static_cast<uintptr_t>(rowbytes)) % 4 != 0 || rowbytes % 4 != 0 ||
-                 (nframes > 1 && screen_frame_stride % 4 != 0)))
+    if (r.rgba && ((reinterpret_cast<uintptr_t>(r.out) + static_cast<uintptr_t>(y0) * static_cast<uintptr_t>(rowbytes)) % 4 != 0 || rowbytes % 4 != 0 ||
+                   (r.nframes > 1 && r.out_stride % 4 != 0)))
         return invalid("the RGBA view origin, rowbytes and screen_frame_stride must be 4-byte aligned");
     if (with_tables) {
         // (16 bytes: the ring kernel restages a frame's table with 128-bit loads)
-        if (!d_tables || reinterpret_cast<uintptr_t>(d_tables) % 16 != 0) return invalid("d_tables must be a non-NULL, 16-byte aligned device pointer");
-        if (table_stride != 0 && (table_stride < 256 * sizeof(uint32_t) || table_stride % 16 != 0 || table_stride / 4 > UINT32_MAX))
+        if (!r.tables || reinterpret_cast<uintptr_t>(r.tables) % 16 != 0) return invalid("d_tables must be a non-NULL, 16-byte aligned device pointer");
+        if (r.table_stride != 0 && (r.table_stride < 256 * sizeof(uint32_t) || r.table_stride % 16 != 0 || r.table_stride / 4 > UINT32_MAX))
             return invalid("table_stride must be 0 (one table for every frame) or at least 1024, a multiple of 16 and below 16 GB");
     }
-    return warp_into_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped != 0, stream, rgba,
-                          d_tables, table_stride);
+    return warp_into_view(ctx, r, rowbytes, x0, y0);
 }
 
 }  // namespace
@@ -436,24 +438,26 @@ extern "C" {
 int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                        int nframes, void *stream) {
     NEED_DEVICE(ctx);
-    return warp_into_view(ctx, d_faces, face_stride, d_out, out_stride, ctx->dev->width(), 0, 0, nframes, false, stream, false);
+    return warp_into_view(ctx, blinky::WarpRequest(d_faces, face_stride, d_out, out_stride, nframes, stream), ctx->dev->width(), 0, 0);
 }
 
 int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
                             int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
-    return warp_device_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream, false);
+    return warp_device_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, rowbytes, x0, y0, keep_unmapped, false);
 }
 
 int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
                                  int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
-    return warp_device_view(ctx, d_faces, face_stride, d_screen, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream, true);
+    return warp_device_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, rowbytes, x0, y0, keep_unmapped, true);
 }
 
 int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen_rgba,
                                         size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes, int keep_unmapped,
                                         const uint32_t *d_tables, size_t table_stride, void *stream) {
-    return warp_device_view(ctx, d_faces, face_stride, d_screen_rgba, screen_frame_stride, rowbytes, x0, y0, nframes, keep_unmapped, stream,
-                            true, true, d_tables, table_stride);
+    blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
+    r.tables = d_tables;
+    r.table_stride = table_stride;
+    return warp_device_view(ctx, r, rowbytes, x0, y0, keep_unmapped, true, true);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,
@@ -521,14 +525,15 @@ int blinky_set_rgba_table(blinky_ctx *ctx, const uint32_t table[256]) {
 int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                             int nframes, void *stream) {
     NEED_DEVICE(ctx);
-    return warp_into_view(ctx, d_faces, face_stride, d_out, out_stride, ctx->dev->width() * 4, 0, 0, nframes, false, stream, true);
+    blinky::WarpRequest r(d_faces, face_stride, d_out, out_stride, nframes, stream);
+    r.rgba = true;
+    return warp_into_view(ctx, r, ctx->dev->width() * 4, 0, 0);
 }
 
 int64_t blinky_launch_count(blinky_ctx *ctx) { return ctx->dev ? ctx->dev->launches() : 0; }
 const char *blinky_plan_summary(blinky_ctx *ctx) {
     if (!ctx->host.built()) return "";
-    blinky::TilePlan pl = blinky::make_tile_plan(ctx->host.packed().data(), ctx->host.width(), ctx->host.height(),
-                                                 ctx->host.platesize(), ctx->host.platesize() % 16 == 0);
+    blinky::TilePlan pl = current_plan(ctx, 1);
     const double npix = static_cast<double>(ctx->host.width()) * ctx->host.height();
     char buf[256];
     snprintf(buf, sizeof buf, "tiles %dx%d of %dx%d px: %d box (%d fully mapped; TMA, %.3f B/px staged, %zu shapes), %d gather, %d empty; entries %.3f B/px",
@@ -540,8 +545,7 @@ const char *blinky_plan_summary(blinky_ctx *ctx) {
 int blinky_get_tile_plan(blinky_ctx *ctx, void *tiles_out, size_t tiles_cap, void *entries_out, size_t entries_cap, size_t *ntiles,
                          size_t *entry_bytes) {
     if (!ctx->host.built()) return set_err(ctx, BLINKY_E_STATE, "no lensmap built");
-    blinky::TilePlan pl = blinky::make_tile_plan(ctx->host.packed().data(), ctx->host.width(), ctx->host.height(),
-                                                 ctx->host.platesize(), ctx->host.platesize() % 16 == 0, ctx->host.worker_threads());
+    blinky::TilePlan pl = current_plan(ctx, ctx->host.worker_threads());
     if (ntiles) *ntiles = pl.tiles.size();
     if (entry_bytes) *entry_bytes = pl.entries.size();
     if (tiles_out) {
@@ -557,8 +561,7 @@ int blinky_get_tile_plan(blinky_ctx *ctx, void *tiles_out, size_t tiles_cap, voi
 
 uint64_t blinky_plan_digest(blinky_ctx *ctx, int threads) {
     if (!ctx->host.built()) return 0;
-    blinky::TilePlan pl = blinky::make_tile_plan(ctx->host.packed().data(), ctx->host.width(), ctx->host.height(),
-                                                 ctx->host.platesize(), ctx->host.platesize() % 16 == 0, threads);
+    blinky::TilePlan pl = current_plan(ctx, threads);
     uint64_t h = 1469598103934665603ull;  // FNV-1a over the tile table and the entry blocks
     auto mix = [&](const void *p, size_t n) {
         const unsigned char *b = static_cast<const unsigned char *>(p);

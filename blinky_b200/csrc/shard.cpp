@@ -252,7 +252,7 @@ bool ShardGroup::warp_gather(const void *d_faces, size_t face_stride, int total_
             const int f0 = c * chunk_frames, nf = std::min(chunk_frames, count - f0);
             // rank 0 and PEER_STORE: the kernel writes the frames where they belong in rank 0's buffer
             uint8_t *out = (rank_ == 0 || mode == BLINKY_GATHER_PEER_STORE) ? root + static_cast<size_t>(first + f0) * fb : stage_ + static_cast<size_t>(f0) * fb;
-            if (!dev_->warp(faces + static_cast<size_t>(f0) * face_stride, face_stride, out, fb, nf, comp, false)) {
+            if (!dev_->warp(WarpRequest(faces + static_cast<size_t>(f0) * face_stride, face_stride, out, fb, nf, comp))) {
                 err_ = dev_->last_error();
                 return false;
             }

@@ -19,10 +19,10 @@
 #include <cstdlib>
 #include <cstring>
 #include <stdexcept>
-#include <type_traits>
 
 #include "../../include/blinky_b200.h"
 #include "face_layout.h"
+#include "launch_plan.h"
 #include "tile_plan.h"
 
 namespace blinky {
@@ -366,8 +366,7 @@ __device__ __forceinline__ void st_stream_u32x8(const uint64_t (&a)[8], const ui
 // bound by load latency, so they get plain parallelism: one extra one-warp CTA per (tile, 8 of its rows, 4
 // frames) behind the ring CTAs in the same grid.  The launch leaves shared memory for two of them per SM next
 // to the resident ring warps, so this work runs beside the ring warps from the start and fills the slots they
-// vacate at the end.
-constexpr int kGatherRows = 8, kGatherFrames = 4;
+// vacate at the end.  (kGatherRows, kGatherFrames: launch_plan.h)
 
 template <bool RUBIX, bool RGBA, bool KEEP, bool TABLES, bool LAYOUT>
 __device__ __forceinline__ void gather_item(const RingParams &p, uint32_t item, uint32_t lane, const FaceLayoutParams &lay) {
@@ -814,8 +813,9 @@ __global__ void __launch_bounds__(32, kRingMinBlocks) warp_ring_kernel(const __g
 
 // --------------------------------------------------------------------------
 // K3: the GATHER tiles (plate seams, singular points; thousands of them with minifying lenses, where a tile's
-// texels do not fit a box), launched in front of the ring kernel; in short launches with few GATHER items
-// they ride in the ring kernel's launch instead (gather_item).  Those tiles are bound
+// texels do not fit a box), launched in front of the ring kernel, one CTA column per GATHER tile (tiles
+// [first_tile, first_tile + grid.x) of the plan); in short launches with few GATHER items they ride in the
+// ring kernel's launch instead (gather_item, gather_rides_along).  Those tiles are bound
 // by global-load latency and, at 32-byte sectors scattered over DRAM pages, by DRAM itself (ncu, 4K fisheye1:
 // 4.6 TB/s = 70 % of the measured copy peak with about one useful byte in 20 fetched); they get plain parallelism: grid = (tiles, groups of 4 frames), 256 threads, a warp owns 4 tile rows and lane l is
 // column l (one warp-level load = 32 consecutive screen pixels of one row).  The tile's entries are
@@ -835,6 +835,8 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
     const uint32_t f0 = blockIdx.y * kGatherFramesPerCta;
     const uint32_t f1 = min(f0 + kGatherFramesPerCta, p.nframes);
 
+    // Never taken (the grid holds GATHER tiles only), but without it ptxas allocates the instances' registers differently
+    // and the RGBA-with-layout one loses a CTA per SM: 8 % slower on the 16-frame 4K fisheye1 batch (H100, 700 W).
     if (type == TILE_EMPTY) {
         if (KEEP) return;   // nothing mapped, nothing to write
         // quad layout: thread t copies 4 background pixels of row t/8
@@ -907,9 +909,22 @@ __global__ void __launch_bounds__(kThreads) warp_tile_gather_kernel(const __grid
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
-// the instance's flags in last_kernel, after rubix= and rgba=
-std::string variant_tags(bool keep, bool tables, bool layout) {
-    return std::string(keep ? ",keep=1" : "") + (tables ? ",tables=1" : "") + (layout ? ",layout=1" : "");
+// The flags of KernelVariant index I as constants: the kernels' template arguments.
+template <int I>
+struct VariantT {
+    static constexpr bool rubix = I & 1, rgba = I & 2, keep = I & 4, tables = I & 8, layout = I & 16;
+};
+
+// Calls f(VariantT<v.index()>{}): the one place that turns the run-time flags into a kernel instance.  Only the
+// indices that exist are instantiated.
+template <int I = 0, typename F>
+void with_variant(int index, F &&f) {
+    if constexpr (I < 32) {
+        if constexpr (KernelVariant::exists(I)) {
+            if (index == I) return f(VariantT<I>{});
+        }
+        with_variant<I + 1>(index, f);
+    }
 }
 
 constexpr uint32_t kCaptureSlots = 4096;   // work counters for captured ring launches (see WarpDevice::CaptureStream)
@@ -978,10 +993,6 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     if (const char *e = getenv("BLINKY_FCHUNK")) fchunk_ = atoi(e);
     if (const char *e = getenv("BLINKY_SERIAL_GATHER")) serial_gather_ = atoi(e) != 0;  // GATHER tiles in their own kernel before the ring kernel (A/B)
     if (const char *e = getenv("BLINKY_STATIC_PCT")) static_pct_ = std::max(0, std::min(100, atoi(e)));
-    cudaStream_t s;
-    e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-    if (e != cudaSuccess) throw std::runtime_error(std::string("cudaStreamCreate: ") + cudaGetErrorString(e));
-    stream_ = s;
     e = cudaMalloc(&d_lut_, 6 * 256);
     if (e == cudaSuccess) e = cudaMemset(d_lut_, 0, 6 * 256);
     if (e == cudaSuccess) e = cudaMalloc(&d_rgba_, 256 * 4);
@@ -1014,7 +1025,6 @@ WarpDevice::~WarpDevice() {
     for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
     cudaFree(d_capture_slots_);
     for (void *p : retired_) cudaFree(p);
-    if (stream_) cudaStreamDestroy(static_cast<cudaStream_t>(stream_));
 }
 
 bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
@@ -1078,11 +1088,6 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
         shapes_ = pl.shapes;
         plan_has_box_ = pl.n_box > 0;
         have_plan_ = true;
-        char buf[256];
-        snprintf(buf, sizeof buf, "tiles %dx%d of %dx%d px: %d box (TMA, %.2f B/px staged), %d gather, %d empty; entries %.2f B/px",
-                 pl.tiles_x, pl.tiles_y, kTileW, kTileH, pl.n_box, static_cast<double>(pl.box_bytes) / static_cast<double>(npix),
-                 pl.n_gather, pl.n_empty, static_cast<double>(pl.entries.size()) / static_cast<double>(npix));
-        plan_summary_ = buf;
     }
     // frame slots depend on the sizes: rebuild lazily
     for (Slot *s : slots_) {
@@ -1113,7 +1118,6 @@ bool WarpDevice::set_background(const uint8_t *bg_host) {
 bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
     CK(cudaSetDevice(device_));
     CK(cudaMemcpy(d_rgba_, table, 256 * 4, cudaMemcpyHostToDevice));
-    have_rgba_ = true;
     return true;
 }
 
@@ -1164,72 +1168,50 @@ bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *
     return true;
 }
 
-bool WarpDevice::warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-                      bool rgba, size_t out_pitch, bool keep_unmapped, const uint32_t *d_tables, size_t table_stride) {
-    return warp_faces(d_faces, face_stride, layout_rowbytes_ > 0, d_out, out_stride, nframes, stream, rgba, out_pitch, keep_unmapped, d_tables,
-                      table_stride);
-}
-
-bool WarpDevice::warp_faces(const void *d_faces, size_t face_stride, bool use_layout, void *d_out, size_t out_stride, int nframes, void *stream,
-                            bool rgba, size_t out_pitch, bool keep_unmapped, const uint32_t *d_tables, size_t table_stride) {
+bool WarpDevice::warp(const WarpRequest &r) {
     err_code_ = BLINKY_E_CUDA;
     if (!have_lensmap_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
         return false;
     }
-    if (nframes <= 0) return true;
-    if (nframes > 65535) {
+    if (r.nframes <= 0) return true;
+    if (r.nframes > 65535) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp: at most 65535 frames per launch";
         return false;
     }
-    const size_t opx = rgba ? 4 : 1;
-    if (rgba && (reinterpret_cast<uintptr_t>(d_out) % 4 != 0 || out_pitch % 4 != 0 || (nframes > 1 && out_stride % 4 != 0))) {
+    const size_t opx = r.rgba ? 4 : 1;
+    if (r.rgba && (reinterpret_cast<uintptr_t>(r.out) % 4 != 0 || r.out_pitch % 4 != 0 || (r.nframes > 1 && r.out_stride % 4 != 0))) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp (RGBA): the output buffer, the row pitch and the frame stride must be 4-byte aligned";
         return false;
     }
-    const size_t pitch = out_pitch ? out_pitch : static_cast<size_t>(width_) * opx;
+    const size_t pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(width_) * opx;
     if (pitch < static_cast<size_t>(width_) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
         return false;
     }
-    // 4-pixel words (the ring kernel, the flat kernel's vector stores): W % 4 == 0 and the view's origin, pitch and frame
-    // stride aligned to 4 pixels
-    const bool vec_ok = (width_ % 4 == 0) && (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (pitch % (4 * opx) == 0) &&
-                        (out_stride % (4 * opx) == 0 || nframes == 1);
-    FaceLayoutParams lay_params;
-    const FaceLayoutParams *lay = nullptr;
-    if (use_layout) {
-        if (!make_layout(face_stride, nframes, &lay_params)) return false;
-        lay = &lay_params;
-    }
-    // TMA: 16-byte aligned rows, and box x coordinates (plate origins included) on 16-byte boundaries
-    bool layout_tma_ok = true;
-    if (lay) {
-        layout_tma_ok = lay->rowbytes % 16 == 0;
-        for (size_t i = 0; i < layout_origins_.size(); i += 2) layout_tma_ok = layout_tma_ok && layout_origins_[i] % 16 == 0;
-    }
-    const bool tiled_ok = have_plan_ && vec_ok && layout_tma_ok &&
-                          (!plan_has_box_ || (reinterpret_cast<uintptr_t>(d_faces) % 16 == 0 && (face_stride % 16 == 0 || nframes == 1)));
+    const bool use_layout = layout_rowbytes_ > 0 && !r.dense_faces;
+    FaceLayoutParams lay = {};   // (dense: the kernels' last argument, never read)
+    if (use_layout && !make_layout(r.face_stride, r.nframes, &lay)) return false;
+    const KernelVariant v = {rubix_, r.rgba, r.keep_unmapped, r.rgba && r.tables && r.table_stride != 0, use_layout};
+    const WarpKernel k = choose_kernel(r, pitch, use_layout ? &lay : nullptr, width_, height_, have_plan_, plan_has_box_,
+                                       variant_ == BLINKY_KERNEL_GATHER);
     // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     unsigned long long cap_id = 0;
-    if (stream != nullptr && static_cast<cudaStream_t>(stream) != cudaStreamLegacy)
-        CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(stream), &cap, &cap_id));
+    if (r.stream != nullptr && static_cast<cudaStream_t>(r.stream) != cudaStreamLegacy)
+        CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(r.stream), &cap, &cap_id));
     const bool capturing = cap != cudaStreamCaptureStatusNone;
-    const bool ok = variant_ == BLINKY_KERNEL_GATHER || !tiled_ok
-                        ? launch_flat(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
-                                      d_tables, table_stride, lay)
-                        : launch_ring(d_faces, face_stride, d_out, out_stride, static_cast<uint32_t>(pitch), nframes, stream, rgba, keep_unmapped,
-                                      d_tables, table_stride, capturing, lay);
+    const bool ok = k == WarpKernel::Ring ? launch_ring(r, static_cast<uint32_t>(pitch), v, lay, capturing)
+                                          : launch_flat(r, static_cast<uint32_t>(pitch), v, lay, k);
     if (capturing) {
         captured_ = bg_captured_ = true;
         bool known = false;
         for (CaptureStream &c : capture_streams_)
-            if (c.stream == stream) c.id = cap_id, known = true;
-        if (!known) capture_streams_.push_back({stream, cap_id});
+            if (c.stream == r.stream) c.id = cap_id, known = true;
+        if (!known) capture_streams_.push_back({r.stream, cap_id});
     }
     return ok;
 }
@@ -1325,119 +1307,63 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
 
-// Calls f(R, C, K, T) with std::bool_constant arguments for (rubix, rgba, keep, tables): one place turns the run-time
-// flags into the kernels' template arguments.  Per-frame tables exist only in RGBA: 12 combinations.
-template <typename F>
-static auto with_variant4(bool rubix, bool rgba, bool keep, bool tables, F &&f) {
-    using T = std::true_type;
-    using N = std::false_type;
-    if (rubix) {
-        if (rgba && tables) return keep ? f(T{}, T{}, T{}, T{}) : f(T{}, T{}, N{}, T{});
-        if (rgba) return keep ? f(T{}, T{}, T{}, N{}) : f(T{}, T{}, N{}, N{});
-        return keep ? f(T{}, N{}, T{}, N{}) : f(T{}, N{}, N{}, N{});
-    }
-    if (rgba && tables) return keep ? f(N{}, T{}, T{}, T{}) : f(N{}, T{}, N{}, T{});
-    if (rgba) return keep ? f(N{}, T{}, T{}, N{}) : f(N{}, T{}, N{}, N{});
-    return keep ? f(N{}, N{}, T{}, N{}) : f(N{}, N{}, N{}, N{});
-}
-
-// ... and f(R, C, K, T, L) with the face layout's flag as well: 24 combinations
-template <typename F>
-static auto with_variant(bool rubix, bool rgba, bool keep, bool tables, bool layout, F &&f) {
-    if (layout) return with_variant4(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) { return f(R, C, K, T, std::true_type{}); });
-    return with_variant4(rubix, rgba, keep, tables, [&](auto R, auto C, auto K, auto T) { return f(R, C, K, T, std::false_type{}); });
-}
-
-static const FaceLayoutParams kDenseLayout = {};   // the dense instances' last kernel argument (never read)
-
-static cudaError_t ring_config_v(bool rubix, bool rgba, bool keep, bool tables, bool layout, size_t smem, int *n) {
-    return with_variant(rubix, rgba, keep, tables, layout, [&](auto R, auto C, auto K, auto T, auto L) {
-        auto *kernel = warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>;
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-        if (e != cudaSuccess) return e;
-        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(n, kernel, 32, smem);
-    });
-}
-
-bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing,
-                             const FaceLayoutParams *lay) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, bool capturing) {
+    cudaStream_t st = static_cast<cudaStream_t>(r.stream);
     RingParams p;
     p.tiles = static_cast<const TileDesc *>(d_tiles_);
     p.entries = d_entries_;
     static const RingTmaps kNoTmaps = {};
     const RingTmaps *tm = &kNoTmaps;
     if (plan_has_box_) {
-        TmapSet *t = get_tmaps(d_faces, face_stride, nframes, lay ? lay->rowbytes : 0u, lay ? layout_rows_ : 0u);
+        TmapSet *t = get_tmaps(r.faces, r.face_stride, r.nframes, lay.rowbytes, v.layout ? layout_rows_ : 0u);
         if (!t) return false;
         tm = &t->table;
     }
-    p.faces = static_cast<const uint8_t *>(d_faces);
-    p.face_stride = face_stride;
+    p.faces = static_cast<const uint8_t *>(r.faces);
+    p.face_stride = r.face_stride;
     p.bg = d_bg_;
     p.lut = d_lut_;
-    p.rgba = tables ? tables : d_rgba_;
-    p.table_words = static_cast<uint32_t>(table_stride / 4);
-    const bool per_frame = rgba && tables && table_stride != 0;
-    p.out = d_out;
-    p.out_stride = out_stride;
-    p.out_pitch = out_pitch / (rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
+    p.rgba = r.tables ? r.tables : d_rgba_;
+    p.table_words = static_cast<uint32_t>(r.table_stride / 4);
+    p.out = r.out;
+    p.out_stride = r.out_stride;
+    p.out_pitch = pitch / (v.rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
     p.nbox = nbox_tiles_;
     p.ngather = ngather_tiles_;
     p.ntiles = ntiles_;
-    p.nframes = static_cast<uint32_t>(nframes);
+    p.nframes = static_cast<uint32_t>(r.nframes);
     p.width = width_;
     p.height = height_;
     p.zero = 0;
-    const bool rubix = rubix_;
-    const bool layout = lay != nullptr;
-    const int vi = (rubix ? 1 : 0) | (rgba ? 2 : 0) | (keep ? 4 : 0) | (per_frame ? 8 : 0) | (layout ? 16 : 0);
-    // The ring kernel takes the BOX tiles [0, nbox) and the EMPTY tiles; the GATHER tiles in between go to the
-    // gather kernel K3 on the context's side stream (forked from and joined to the caller's stream), so the two
-    // kernels share the GPU instead of queueing behind each other.  With keep_unmapped an EMPTY tile has nothing
-    // to write: the ring kernel's units are the BOX tiles alone.
+    // The ring kernel's units are the BOX tiles [0, nbox) and the EMPTY tiles; with keep_unmapped an EMPTY tile has
+    // nothing to write, and the units are the BOX tiles alone.  The GATHER tiles in between ride along as gather CTAs
+    // or go to K3, launched in front on the same stream (gather_rides_along).
     const uint32_t nempty = ntiles_ - nbox_tiles_ - ngather_tiles_;
-    const uint32_t ring_tiles = nbox_tiles_ + (keep ? 0u : nempty);
-    // Ring geometry: as many warps per SM as the registers allow (or BLINKY_RING_CTAS), each with the largest
-    // staging ring that still lets that many CTAs share the SM's shared memory; fewer warps if the plan's
-    // largest box would not fit such a ring.
-    const size_t fixed = kRingBarBytes + (rubix ? 6 * 256 : 0) + (rgba ? 1024 : 0);
+    const uint32_t ring_tiles = nbox_tiles_ + (v.keep ? 0u : nempty);
+    const size_t fixed = kRingBarBytes + (v.rubix ? 6 * 256 : 0) + (v.rgba ? 1024 : 0);
     const uint32_t max_box = std::max<uint32_t>(static_cast<uint32_t>(stage_bytes_ > 0 ? stage_bytes_ : 128), kBoxBlockBytes);  // largest ring item
-    // GATHER tiles ride in the ring kernel's launch (gather_item) only in launches of at most kMergedFramesMax frames
-    // with few GATHER items, where a second kernel launch costs more than they do; otherwise the gather kernel K3 goes
-    // in front.  Measured on the H100 (80GB HBM3, 400 W): riding along is 2-20 % faster for 1-8 frames of 4K panini and
-    // trism, but with 16 frames K3 in front is faster by 1.5-10 % (panini, stereographic, trism, 1080p panini; the
-    // 1080p batch prefers K3 from 8 frames on, by 10 %, and keeps riding along there).
-    constexpr int kMergedFramesMax = 8;
-    const uint32_t gather_items = ngather_tiles_ * (kTileH / kGatherRows) * static_cast<uint32_t>((nframes + kGatherFrames - 1) / kGatherFrames);
-    const bool merged_gather = !serial_gather_ && ngather_tiles_ > 0 && nframes <= kMergedFramesMax &&
-                               gather_items <= static_cast<uint32_t>(merged_items_max_);
-    int want = ring_ctas_cap_ > 0 ? std::min(ring_ctas_cap_, kRingMinBlocks) : kRingWarpsDefault;
-    // ring size: twice the plan's largest box plus an entry block (two boxes of any size and the next unit's entries in
-    // flight), as far as `want`
-    // resident warps — plus two gather CTAs, which
-    // carry the same allocation, when GATHER tiles ride along — leave room in the SM's shared memory
-    uint32_t ring_bytes = 0;
-    for (; want >= 1; --want) {
-        const size_t per_cta = smem_per_sm_ / static_cast<size_t>(want + (merged_gather ? 2 : 0));
-        if (per_cta < 1024 + fixed + max_box) continue;
-        const uint32_t room = static_cast<uint32_t>((per_cta - 1024 - fixed) / 128 * 128);
-        ring_bytes = std::min(room, std::max(2u * max_box + kBoxBlockBytes, 8192u));
-        if (ring_bytes_override_ > 0) ring_bytes = std::min(room, std::max<uint32_t>(max_box, static_cast<uint32_t>(ring_bytes_override_) / 128 * 128));
-        break;
-    }
-    if (want < 1) {
+    const bool merged_gather = gather_rides_along(ngather_tiles_, r.nframes, merged_items_max_, serial_gather_);
+    // as many ring warps per SM as the registers allow (or BLINKY_RING_CTAS), as far as shared memory lets them
+    const RingGeometry geo = ring_geometry(smem_per_sm_, ring_ctas_cap_ > 0 ? std::min(ring_ctas_cap_, kRingMinBlocks) : kRingWarpsDefault,
+                                           merged_gather, fixed, max_box, ring_bytes_override_);
+    if (geo.warps < 1) {
         err_ = "ring kernel: the plan's largest box does not fit the staging ring";
         return false;
     }
-    p.ring_bytes = ring_bytes;
+    p.ring_bytes = geo.ring_bytes;
     // items in flight per warp: two boxes and (at unit boundaries) the next entry block (BLINKY_RING_BOXES overrides)
     p.max_inflight = static_cast<uint32_t>(std::max(1, std::min(ring_boxes_ > 0 ? ring_boxes_ : 3, kRingBoxes)));
-    const size_t smem = static_cast<size_t>(ring_bytes) + fixed;
+    const size_t smem = static_cast<size_t>(geo.ring_bytes) + fixed;
+    const int vi = v.index();
     if (ring_ctas_per_sm_[vi] == 0 || ring_smem_[vi] != smem) {
         int n = 0;
-        cudaError_t e = ring_config_v(rubix, rgba, keep, per_frame, layout, smem, &n);
+        cudaError_t e = cudaSuccess;
+        with_variant(vi, [&](auto vt) {   // the instance's dynamic shared memory and occupancy
+            using V = decltype(vt);
+            auto *kernel = warp_ring_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout>;
+            e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+            if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, 32, smem);
+        });
         if (e != cudaSuccess) return fail("ring kernel configuration (shared memory / occupancy)", e);
         if (n < 1) {
             err_ = "ring kernel does not fit on an SM";
@@ -1446,24 +1372,9 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
         ring_ctas_per_sm_[vi] = n;
         ring_smem_[vi] = smem;
     }
-    int ctas = std::min(ring_ctas_per_sm_[vi], want);
+    int ctas = std::min(ring_ctas_per_sm_[vi], geo.warps);
     uint32_t grid = static_cast<uint32_t>(sm_count_ * ctas);
-    // frames per unit: a unit pays a fixed cost (entry unpack, ring refill across the boundary: ~kUnitCost frame
-    // times) and the launch ends with a tail of about one unit; pick the chunk that minimises
-    // units-per-warp x (chunk + kUnitCost) + chunk.  kUnitCost = 2 fits the H100 (80GB HBM3, 400 W): 16-frame units
-    // beat 8-frame ones by 4-7 % on the 4K batches of ~7900 ring tiles (panini, stereographic, quincuncial, trism),
-    // and lose 1-3 % on those of ~5000 (hammer, fisheye1), which keep 8.
-    constexpr double kUnitCost = 2.0;
-    uint32_t fchunk = fchunk_ > 0 ? static_cast<uint32_t>(fchunk_) : 1;
-    if (fchunk_ <= 0) {
-        double best = 0;
-        for (uint32_t c = 1; c <= std::min<uint32_t>(p.nframes, 16u); ++c) {
-            const double units = static_cast<double>(ring_tiles) * ((p.nframes + c - 1) / c);
-            const double cost = std::max(1.0, units / grid) * (c + kUnitCost) + c;
-            if (c == 1 || cost < best) best = cost, fchunk = c;
-        }
-    }
-    if (fchunk > p.nframes) fchunk = p.nframes;
+    const uint32_t fchunk = frames_per_unit(ring_tiles, p.nframes, grid, fchunk_);
     p.fchunk = fchunk;
     p.nchunks = (p.nframes + fchunk - 1) / fchunk;
     p.nunits = ring_tiles * p.nchunks;
@@ -1482,7 +1393,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     } else if (grid > 0) {
         TicketCounter *tc = nullptr;
         for (TicketCounter &c : tickets_)
-            if (c.stream == stream) tc = &c;
+            if (c.stream == r.stream) tc = &c;
         if (!tc) {
             if (tickets_.size() >= 64) {  // streams come and go: start over
                 CK(cudaDeviceSynchronize());
@@ -1490,7 +1401,7 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
                 tickets_.clear();
             }
             TicketCounter c;
-            c.stream = stream;
+            c.stream = r.stream;
             CK(cudaMalloc(&c.d_counter, sizeof(uint32_t)));
             CK(cudaMemsetAsync(c.d_counter, 0, sizeof(uint32_t), st));
             tickets_.push_back(c);
@@ -1500,99 +1411,68 @@ bool WarpDevice::launch_ring(const void *d_faces, size_t face_stride, void *d_ou
     }
     char buf[640];
     int nbuf = 0;
-    const std::string tag_str = variant_tags(keep, per_frame, layout);
-    const char *tags = tag_str.c_str();
-    // GATHER tiles: one-warp CTAs behind the ring warps in the same grid (see gather_item); only a plan without BOX and
-    // EMPTY tiles (with keep_unmapped: without BOX tiles) launches the stand-alone gather kernel.
+    // GATHER tiles: K3 in front of the ring kernel, unless they ride in its launch (which needs ring units)
     snprintf(buf, sizeof buf, "%s", ngather_tiles_ == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
     if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
-        dim3 g2(ngather_tiles_, static_cast<unsigned>((nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
-        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
-            warp_tile_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
-                <<<g2, kThreads, 0, st>>>(p, nbox_tiles_, lay ? *lay : kDenseLayout);
+        dim3 g2(ngather_tiles_, static_cast<unsigned>((r.nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
+        with_variant(vi, [&](auto vt) {
+            using V = decltype(vt);
+            warp_tile_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<g2, kThreads, 0, st>>>(p, nbox_tiles_, lay);
         });
         ++launches_;
-        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, g2.x, g2.y, kThreads);
+        snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", v.rubix, v.rgba, v.tags(), g2.x, g2.y, kThreads);
     }
     if (grid > 0) {
-        // static share of the schedule (see the kernel): static_pct_ percent of the units, whole rounds
-        uint32_t nstatic = static_cast<uint32_t>(static_cast<uint64_t>(p.nunits) * static_cast<uint64_t>(static_pct_) / 100u / grid);
-        p.nstatic = nstatic;
-        // draws of this launch: every unit beyond the static ones is drawn exactly once, and every warp that
-        // draws at all draws exactly one ticket past the end (it stops at its first bad ticket).  A warp draws
-        // iff its last static ticket is good (all warps when there are no static rounds).
-        const uint64_t nst = static_cast<uint64_t>(nstatic) * grid;
-        const uint32_t good = p.nunits > nst ? static_cast<uint32_t>(p.nunits - nst) : 0u;
-        uint32_t drawers = grid;
-        if (nstatic > 0) {
-            const uint64_t before_last = static_cast<uint64_t>(nstatic - 1) * grid;
-            drawers = p.nunits > before_last ? static_cast<uint32_t>(std::min<uint64_t>(p.nunits - before_last, grid)) : 0u;
-        }
-        p.ndraws = good + drawers;
-
+        const TicketSchedule ts = ticket_schedule(p.nunits, grid, static_pct_);
+        p.nstatic = ts.nstatic;
+        p.ndraws = ts.ndraws;
         p.ring_grid = grid;
-        const uint32_t extra = merged_gather ? gather_items : 0u;
-        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
-            warp_ring_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
-                <<<grid + extra, 32, smem, st>>>(p, *tm, lay ? *lay : kDenseLayout);
+        const uint32_t extra = merged_gather ? gather_items(ngather_tiles_, r.nframes) : 0u;
+        with_variant(vi, [&](auto vt) {
+            using V = decltype(vt);
+            warp_ring_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid + extra, 32, smem, st>>>(p, *tm, lay);
         });
         ++launches_;
         nbuf = static_cast<int>(strlen(buf));
         snprintf(buf + nbuf, sizeof buf - static_cast<size_t>(nbuf),
                  "%swarp_ring_kernel<rubix=%d,rgba=%d%s> grid=%u+%u block=32 (%d ring warps/SM, TMA box ring of %u B, <=%u boxes in flight, %u frames/unit, %u units; "
                  "%u gather CTAs of %dx32 px x %d frames)",
-                 nbuf ? " + " : "", rubix, rgba, tags, grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows, kGatherFrames);
+                 nbuf ? " + " : "", v.rubix, v.rgba, v.tags(), grid, extra, ctas, p.ring_bytes, p.max_inflight, fchunk, p.nunits, extra, kGatherRows,
+                 kGatherFrames);
     }
     last_kernel_ = buf;
     CK(cudaGetLastError());
     return true;
 }
 
-bool WarpDevice::launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                             void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, const FaceLayoutParams *lay) {
-    // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out
-    // unless the caller made its own) — NOT this context's private stream.
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+bool WarpDevice::launch_flat(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, WarpKernel k) {
+    // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out unless the caller made its own)
+    cudaStream_t st = static_cast<cudaStream_t>(r.stream);
     WarpParams p;
     p.lensmap4 = reinterpret_cast<const uint4 *>(d_lensmap_);
-    p.faces = static_cast<const uint8_t *>(d_faces);
-    p.face_stride = face_stride;
+    p.faces = static_cast<const uint8_t *>(r.faces);
+    p.face_stride = r.face_stride;
     p.bg32 = reinterpret_cast<const uint32_t *>(d_bg_);
     p.lut = d_lut_;
-    p.rgba = tables ? tables : d_rgba_;
-    p.table_words = static_cast<uint32_t>(table_stride / 4);
-    const bool per_frame = rgba && tables && table_stride != 0;
-    p.out = d_out;
-    p.out_stride = out_stride;
+    p.rgba = r.tables ? r.tables : d_rgba_;
+    p.table_words = static_cast<uint32_t>(r.table_stride / 4);
+    p.out = r.out;
+    p.out_stride = r.out_stride;
     p.nquads = static_cast<uint32_t>((npix_ + 3) / 4);
     p.npix = static_cast<uint32_t>(npix_);
     p.width = static_cast<uint32_t>(width_);
-    p.out_pitch = out_pitch;
-
-    const size_t opx = rgba ? 4 : 1;  // output bytes per pixel
-    p.pitched = out_pitch != static_cast<size_t>(width_) * opx;
-    // 4-pixel words: dense frames need W*H % 4 == 0, pitched ones W % 4 == 0 (no quad straddles two rows)
-    const bool vector_ok = (p.pitched ? width_ % 4 == 0 && out_pitch % (4 * opx) == 0 : npix_ % 4 == 0) &&
-                           (reinterpret_cast<uintptr_t>(d_out) % (4 * opx) == 0) && (out_stride % (4 * opx) == 0 || nframes == 1);
-    const bool rubix = rubix_, layout = lay != nullptr;
-    const std::string tag_str = variant_tags(keep, per_frame, layout);
-    const char *tags = tag_str.c_str();
+    p.out_pitch = pitch;
+    p.pitched = pitch != static_cast<size_t>(width_) * (v.rgba ? 4 : 1);
+    const bool vector = k == WarpKernel::Vector;
+    const dim3 grid(static_cast<unsigned>(vector ? npix_pad_ / kPixelsPerBlock : (npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(r.nframes));
+    with_variant(v.index(), [&](auto vt) {
+        using V = decltype(vt);
+        if (vector) warp_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, lay);
+        else warp_scalar_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, lay);
+    });
     char buf[160];
-    if (vector_ok) {
-        dim3 grid(static_cast<unsigned>(npix_pad_ / kPixelsPerBlock), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
-            warp_gather_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
-                <<<grid, kThreads, 0, st>>>(p, lay ? *lay : kDenseLayout);
-        });
-        snprintf(buf, sizeof buf, "warp_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
-    } else {
-        dim3 grid(static_cast<unsigned>((npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(nframes));
-        with_variant(rubix, rgba, keep, per_frame, layout, [&](auto R, auto C, auto K, auto T, auto L) {
-            warp_scalar_kernel<decltype(R)::value, decltype(C)::value, decltype(K)::value, decltype(T)::value, decltype(L)::value>
-                <<<grid, kThreads, 0, st>>>(p, lay ? *lay : kDenseLayout);
-        });
-        snprintf(buf, sizeof buf, "warp_scalar_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", rubix, rgba, tags, grid.x, grid.y, kThreads);
-    }
+    snprintf(buf, sizeof buf, "%s<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", vector ? "warp_gather_kernel" : "warp_scalar_kernel", v.rubix, v.rgba,
+             v.tags(), grid.x, grid.y, kThreads);
     last_kernel_ = buf;
     ++launches_;
     CK(cudaGetLastError());
@@ -1730,7 +1610,9 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         }
         if (!ok) break;
         s.dst = dst_host + static_cast<size_t>(f) * dst_frame_stride;
-        if (!warp_faces(s.d_faces, slot_face_bytes_, false, s.d_out, slot_out_bytes_, 1, s.stream, false)) { ok = false; break; }
+        WarpRequest r(s.d_faces, slot_face_bytes_, s.d_out, slot_out_bytes_, 1, s.stream);
+        r.dense_faces = true;   // the device copy is dense whatever the face layout
+        if (!warp(r)) { ok = false; break; }
         s.dst_rowbytes = dst_rowbytes;
         s.x0 = x0;
         s.y0 = y0;
@@ -1756,15 +1638,6 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         if (e != cudaSuccess) ok = fail("warp_host", e);
     }
     return ok;
-}
-
-size_t WarpDevice::upload_bytes_per_frame() const {
-    size_t n = 0;
-    for (int pl = 0; pl < numplates_; ++pl) {
-        const int *r = plate_rect_[pl];
-        if (display_[pl] && r[0] <= r[2] && r[1] <= r[3]) n += static_cast<size_t>(r[2] - r[0] + 1) * static_cast<size_t>(r[3] - r[1] + 1);
-    }
-    return n;
 }
 
 bool WarpDevice::alloc_device(size_t bytes, void **out) {

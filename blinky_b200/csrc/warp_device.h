@@ -15,7 +15,9 @@
 
 namespace blinky {
 
-struct TilePlan;  // tile_plan.h
+struct TilePlan;       // tile_plan.h
+struct KernelVariant;  // launch_plan.h
+enum class WarpKernel;
 
 struct LensmapUpload {
     int width = 0, height = 0, platesize = 0, numplates = 0;
@@ -28,6 +30,28 @@ struct LensmapUpload {
     const int32_t *spans = nullptr;          // pairs
     size_t nspans = 0;
     const TilePlan *plan = nullptr;          // tiled layout (may be null: flat kernels only)
+};
+
+// One device-resident batch (WarpDevice::warp), asynchronous on `stream` (nullptr = CUDA's default stream).  May be
+// captured into a CUDA graph: see WarpDevice::release_captures.
+struct WarpRequest {
+    WarpRequest(const void *faces, size_t face_stride, void *out, size_t out_stride, int nframes, void *stream)
+        : faces(faces), face_stride(face_stride), out(out), out_stride(out_stride), nframes(nframes), stream(stream) {}
+    const void *faces;                 // frame 0's faces, in the face layout (WarpDevice::set_face_layout)
+    size_t face_stride;                // bytes between frames
+    void *out;                         // view origin of frame 0
+    size_t out_stride;                 // bytes between frames
+    size_t out_pitch = 0;              // bytes between rows (0: dense, W * bytes per pixel)
+    int nframes;
+    void *stream;                      // cudaStream_t
+    bool rgba = false;
+    bool keep_unmapped = false;        // only mapped pixels are written, the others keep what the caller's buffer holds
+    // RGBA: frame f is expanded through the 256-entry device table at tables + f * table_stride bytes (table_stride 0:
+    // one table for every frame) instead of set_rgba_table's, read when the launch runs.  tables 16-byte aligned,
+    // table_stride a multiple of 16.
+    const uint32_t *tables = nullptr;
+    size_t table_stride = 0;
+    bool dense_faces = false;          // the faces are dense [plate][ps][ps] frames whatever the face layout
 };
 
 class WarpDevice {
@@ -52,15 +76,7 @@ public:
     int width() const { return width_; }
     int height() const { return height_; }
 
-    // device-resident batch (asynchronous on `stream`, nullptr = CUDA default stream).  d_out is the view origin of
-    // frame 0; rows are out_pitch bytes apart (0: dense, W * bytes per pixel).  keep_unmapped: only mapped pixels
-    // are written, the others keep what the caller's buffer holds.  May be captured into a CUDA graph: see
-    // release_captures.  RGBA with d_tables: frame f is expanded through the 256-entry device table at
-    // d_tables + f * table_stride bytes (table_stride 0: one table for every frame) instead of set_rgba_table's; the
-    // tables are read when the launch runs.  d_tables 16-byte aligned, table_stride a multiple of 16.
-    bool warp(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, int nframes, void *stream,
-              bool rgba, size_t out_pitch = 0, bool keep_unmapped = false, const uint32_t *d_tables = nullptr,
-              size_t table_stride = 0);
+    bool warp(const WarpRequest &r);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, frees
     // the buffers upload_lensmap retired for such graphs and returns every capture counter slot to the pool.
     bool release_captures();
@@ -80,7 +96,6 @@ public:
     bool sync();
 
     int64_t launches() const { return launches_; }
-    size_t upload_bytes_per_frame() const;
     const std::string &last_kernel() const { return last_kernel_; }
 
 private:
@@ -88,14 +103,10 @@ private:
     bool ensure_slots();
     bool fail(const char *what, int cuda_err);
     bool make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay);
-    // warp() with the face layout (use_layout) or the dense frames warp_host stages
-    bool warp_faces(const void *d_faces, size_t face_stride, bool use_layout, void *d_out, size_t out_stride, int nframes, void *stream,
-                    bool rgba, size_t out_pitch = 0, bool keep_unmapped = false, const uint32_t *d_tables = nullptr, size_t table_stride = 0);
     void finalize_slot(Slot &s);
 
     int device_ = 0;
     int sm_count_ = 132;
-    void *stream_ = nullptr;  // cudaStream_t
     bool batch_copies_ = true;   // plate rectangles of a frame in one cudaMemcpy3DBatchAsync (false once the driver refused it)
     const void *pin_src_ptr_ = nullptr, *pin_dst_ptr_ = nullptr;  // last buffers warp_host saw and whether they are pinned
     bool pin_src_ = false, pin_dst_ = false;
@@ -113,7 +124,6 @@ private:
     uint8_t *d_lut_ = nullptr;
     uint8_t *d_bg_ = nullptr;
     uint32_t *d_rgba_ = nullptr;
-    bool have_rgba_ = false;
     std::vector<int32_t> span_off_, spans_;
     int variant_ = 0;
     int layout_rowbytes_ = 0;              // face layout: 0 = dense
@@ -143,15 +153,13 @@ private:
     uint64_t tmap_tick_ = 0;
     std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on (eagerly)
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
-    int ring_ctas_per_sm_[32] = {};      // per ring kernel instance: rubix | rgba << 1 | keep << 2 | per-frame tables << 3 | layout << 4
+    int ring_ctas_per_sm_[32] = {};      // per ring kernel instance (KernelVariant::index)
     size_t ring_smem_[32] = {};
     TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes, uint32_t rowbytes, uint32_t rows);
-    // lay: the face layout, nullptr for dense frames
-    bool launch_ring(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, bool capturing,
-                     const FaceLayoutParams *lay);
-    bool launch_flat(const void *d_faces, size_t face_stride, void *d_out, size_t out_stride, uint32_t out_pitch, int nframes,
-                     void *stream, bool rgba, bool keep, const uint32_t *tables, size_t table_stride, const FaceLayoutParams *lay);
+    // what warp() derived from the request: pitch, the output's bytes between rows; lay, the face layout when v.layout
+    // (zero otherwise)
+    bool launch_ring(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, bool capturing);
+    bool launch_flat(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, WarpKernel k);
 
     // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
     // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are
@@ -167,10 +175,6 @@ private:
     bool bg_captured_ = false;            // a launch was captured since d_bg_ was allocated
     std::vector<void *> retired_;         // device buffers that captured graphs may still read
     std::vector<CaptureStream> capture_streams_;  // where warps were captured (release_captures refuses while one is open)
-    std::string plan_summary_;
-public:
-    const std::string &plan_summary() const { return plan_summary_; }
-private:
 
     // e2e pipeline
     std::vector<Slot *> slots_;
