@@ -59,6 +59,8 @@ _SIGNATURES = [
     ("blinky_set_rubixgrid", c_int, [_CTX, c_int, c_double, c_double]),
     ("blinky_build_lensmap", c_int, [_CTX, c_int, c_int, c_int, c_int]),
     ("blinky_needs_rebuild", c_int, [_CTX, c_int, c_int, c_int]),
+    ("blinky_set_lensmap", c_int, [_CTX, c_int, c_int, c_int, c_int, c_void_p]),
+    ("blinky_set_lensmap_device", c_int, [_CTX, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_build_info", c_char_p, [_CTX]),
     ("blinky_plan_digest", ctypes.c_uint64, [_CTX, c_int]),
     ("blinky_get_tile_plan", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
@@ -264,6 +266,23 @@ class Fisheye:
 
     def build_lensmap(self, width: int, height: int, platesize: int = 0, threads: int = 1):
         self._check(self._lib.blinky_build_lensmap(self._ctx, width, height, platesize, threads))
+
+    def set_lensmap(self, packed, platesize: int, numplates: int, stream: int | None = None):
+        """Replaces the lensmap with a caller's map of packed entries (LM_* format), [H, W] 32-bit: a numpy array
+        (blinky_set_lensmap) or a CUDA tensor (blinky_set_lensmap_device, read on `stream` after the work already
+        there, and planned on the GPU).  Rows must be dense."""
+        if isinstance(packed, np.ndarray):
+            m = np.ascontiguousarray(packed)
+            if m.ndim != 2 or m.dtype.itemsize != 4 or m.dtype.kind not in "ui":
+                raise ValueError(f"set_lensmap: expected a [H, W] array of 32-bit entries, got {m.dtype} {m.shape}")
+            self._check(self._lib.blinky_set_lensmap(self._ctx, m.shape[1], m.shape[0], platesize, numplates, m.ctypes.data))
+            return
+        if not (hasattr(packed, "is_cuda") and packed.is_cuda):
+            raise TypeError("set_lensmap: expected a numpy array or a CUDA tensor")
+        if packed.dim() != 2 or packed.element_size() != 4 or not packed.is_contiguous():
+            raise ValueError(f"set_lensmap: expected a contiguous [H, W] tensor of 32-bit entries, got {packed.dtype} {tuple(packed.shape)}")
+        self._check(self._lib.blinky_set_lensmap_device(self._ctx, packed.shape[1], packed.shape[0], platesize, numplates,
+                                                        packed.data_ptr(), stream))
 
     @property
     def build_info(self) -> str:

@@ -18,6 +18,7 @@
 #include "lens_device.h"
 #include "shard.h"
 #include "tile_plan.h"
+#include "tile_plan_device.h"
 #include "warp_device.h"
 
 using blinky::FisheyeHost;
@@ -36,6 +37,7 @@ struct blinky_ctx {
     uint8_t palmaps[BLINKY_MAX_PLATES * 256];
     int layout_rowbytes = 0;              // blinky_set_face_layout: 0 = dense faces
     std::vector<int32_t> layout_origins;  // (x, y) per plate
+    bool device_plan = false;             // the resident tile plan was made on the GPU (blinky_set_lensmap_device)
 };
 
 namespace {
@@ -71,17 +73,31 @@ blinky::TilePlan current_plan(blinky_ctx *c, int threads) {
                                   threads);
 }
 
-bool upload(blinky_ctx *c) {
+// A map planned on the GPU stays there until a host-side query needs it; then it is copied back once and kept.
+bool host_map(blinky_ctx *c) {
+    if (c->host.map_on_host()) return true;
+    std::vector<uint32_t> m(static_cast<size_t>(c->host.width()) * c->host.height());
+    if (!c->dev->download_lensmap(m.data())) {
+        c->err = c->dev->last_error();
+        return false;
+    }
+    c->host.fill_lensmap(std::move(m));
+    return true;
+}
+
+// The device upload of the current lensmap: the host's map, planned here, or (device != null) a map and plan the
+// GPU planner left in device memory.
+bool upload(blinky_ctx *c, const blinky::DevicePlan *device = nullptr) {
     if (!c->dev || !c->host.built()) return true;
+    if (!device && !host_map(c)) return false;
     blinky::LensmapUpload lm;
     lm.width = c->host.width();
     lm.height = c->host.height();
     lm.platesize = c->host.platesize();
-    lm.numplates = c->host.numplates();
-    lm.packed = c->host.packed().data();
+    lm.numplates = c->host.map_numplates();
     for (int i = 0; i < BLINKY_MAX_PLATES; ++i) {
         memcpy(c->palmaps + i * 256, c->host.plate(i).palette, 256);
-        lm.display[i] = i < c->host.numplates() ? c->host.plate(i).display : 0;
+        lm.display[i] = i < c->host.map_numplates() ? c->host.plate(i).display : 0;
         memcpy(lm.plate_rect[i], c->host.plate_rect(i), sizeof lm.plate_rect[i]);
     }
     lm.palmaps = c->palmaps;
@@ -89,8 +105,15 @@ bool upload(blinky_ctx *c) {
     lm.span_off = c->host.row_span_offsets().data();
     lm.spans = c->host.row_spans().data();
     lm.nspans = c->host.row_spans().size() / 2;
-    blinky::TilePlan plan = current_plan(c, c->host.worker_threads());
-    lm.plan = &plan;
+    blinky::TilePlan plan;
+    if (device) {
+        lm.device = device;
+    } else {
+        lm.packed = c->host.packed().data();
+        plan = current_plan(c, c->host.worker_threads());
+        lm.plan = &plan;
+    }
+    c->device_plan = device != nullptr;
     if (!c->dev->upload_lensmap(lm)) {
         c->err = c->dev->last_error();
         return false;
@@ -221,6 +244,25 @@ int blinky_build_lensmap(blinky_ctx *ctx, int width, int height, int platesize, 
     }
 }
 
+int blinky_set_lensmap(blinky_ctx *ctx, int width, int height, int platesize, int numplates, const uint32_t *packed) {
+    std::string why;
+    auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point t) {
+        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+    };
+    if (!ctx->host.set_lensmap(width, height, platesize, numplates, packed, &why)) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_lensmap: " + why);
+    char t[128];
+    snprintf(t, sizeof t, "supplied (host memory); finish %.1f ms", ms_since(t0));
+    ctx->build_info = t;
+    t0 = std::chrono::steady_clock::now();
+    const bool uploaded = upload(ctx);
+    if (ctx->dev) {
+        snprintf(t, sizeof t, ", plan+upload %.1f ms", ms_since(t0));
+        ctx->build_info += t;
+    }
+    return uploaded ? BLINKY_OK : BLINKY_E_CUDA;
+}
+
 const char *blinky_build_info(blinky_ctx *ctx) { return ctx->build_info.c_str(); }
 
 int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes) {
@@ -270,7 +312,8 @@ int blinky_get_plates(blinky_ctx *ctx, float *out, int max_plates) {
 }
 
 int blinky_get_display(blinky_ctx *ctx, int out[BLINKY_MAX_PLATES]) {
-    for (int i = 0; i < BLINKY_MAX_PLATES; ++i) out[i] = i < ctx->host.numplates() ? ctx->host.plate(i).display : 0;
+    const int n = ctx->host.built() ? ctx->host.map_numplates() : ctx->host.numplates();
+    for (int i = 0; i < BLINKY_MAX_PLATES; ++i) out[i] = i < n ? ctx->host.plate(i).display : 0;
     return BLINKY_OK;
 }
 
@@ -286,6 +329,7 @@ int blinky_get_palmaps(blinky_ctx *ctx, uint8_t out[BLINKY_MAX_PLATES * 256]) {
 
 int blinky_get_lensmap(blinky_ctx *ctx, int32_t *idx, uint8_t *tint) {
     if (!ctx->host.built()) return set_err(ctx, BLINKY_E_STATE, "no lensmap built");
+    if (!host_map(ctx)) return BLINKY_E_CUDA;
     if (idx) memcpy(idx, ctx->host.indices().data(), ctx->host.indices().size() * sizeof(int32_t));
     if (tint) memcpy(tint, ctx->host.tints().data(), ctx->host.tints().size());
     return BLINKY_OK;
@@ -293,6 +337,7 @@ int blinky_get_lensmap(blinky_ctx *ctx, int32_t *idx, uint8_t *tint) {
 
 int blinky_get_lensmap_packed(blinky_ctx *ctx, uint32_t *out) {
     if (!ctx->host.built()) return set_err(ctx, BLINKY_E_STATE, "no lensmap built");
+    if (!host_map(ctx)) return BLINKY_E_CUDA;
     memcpy(out, ctx->host.packed().data(), ctx->host.packed().size() * sizeof(uint32_t));
     return BLINKY_OK;
 }
@@ -387,6 +432,27 @@ int blinky_set_kernel(blinky_ctx *ctx, int variant) {
     return BLINKY_OK;
 }
 
+int blinky_set_lensmap_device(blinky_ctx *ctx, int width, int height, int platesize, int numplates, const uint32_t *d_packed, void *stream) {
+    NEED_DEVICE(ctx);
+    std::string why;
+    if (!FisheyeHost::check_lensmap_size(width, height, platesize, numplates, &why)) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_lensmap_device: " + why);
+    if (!d_packed) return set_err(ctx, BLINKY_E_INVALID, "blinky_set_lensmap_device: map is NULL");
+    auto t0 = std::chrono::steady_clock::now();
+    blinky::DevicePlan dp;
+    const int rc = blinky::plan_lensmap_device(ctx->dev->device(), d_packed, width, height, platesize, numplates,
+                                               WarpDevice::padded_pixels(static_cast<size_t>(width) * height), stream, &dp, &why);
+    if (rc != BLINKY_OK) return set_err(ctx, rc, why);
+    const double ms_plan = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    t0 = std::chrono::steady_clock::now();
+    ctx->host.adopt_lensmap(width, height, platesize, numplates, dp.display, dp.rect, dp.mapped, std::move(dp.span_off), std::move(dp.spans));
+    if (!upload(ctx, &dp)) return BLINKY_E_CUDA;
+    char t[128];
+    snprintf(t, sizeof t, "supplied (device memory); plan %.3f ms, adopt %.3f ms", ms_plan,
+             std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+    ctx->build_info = t;
+    return BLINKY_OK;
+}
+
 int blinky_set_background(blinky_ctx *ctx, const uint8_t *bg) {
     NEED_DEVICE(ctx);
     return ctx->dev->set_background(bg) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
@@ -473,7 +539,7 @@ int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_str
 int64_t blinky_upload_bytes_per_frame(blinky_ctx *ctx) {
     int64_t n = 0;
     if (!ctx->host.built()) return 0;
-    for (int i = 0; i < ctx->host.numplates(); ++i) {
+    for (int i = 0; i < ctx->host.map_numplates(); ++i) {
         const int *r = ctx->host.plate_rect(i);
         if (ctx->host.plate(i).display && r[0] <= r[2] && r[1] <= r[3]) n += static_cast<int64_t>(r[2] - r[0] + 1) * (r[3] - r[1] + 1);
     }
@@ -532,7 +598,7 @@ int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_st
 
 int64_t blinky_launch_count(blinky_ctx *ctx) { return ctx->dev ? ctx->dev->launches() : 0; }
 const char *blinky_plan_summary(blinky_ctx *ctx) {
-    if (!ctx->host.built()) return "";
+    if (!ctx->host.built() || !host_map(ctx)) return "";
     blinky::TilePlan pl = current_plan(ctx, 1);
     const double npix = static_cast<double>(ctx->host.width()) * ctx->host.height();
     char buf[256];
@@ -545,6 +611,16 @@ const char *blinky_plan_summary(blinky_ctx *ctx) {
 int blinky_get_tile_plan(blinky_ctx *ctx, void *tiles_out, size_t tiles_cap, void *entries_out, size_t entries_cap, size_t *ntiles,
                          size_t *entry_bytes) {
     if (!ctx->host.built()) return set_err(ctx, BLINKY_E_STATE, "no lensmap built");
+    if (ctx->device_plan) {
+        // the plan the GPU planner wrote, as the kernels read it
+        const size_t nt = ctx->dev->plan_tiles(), nb = ctx->dev->plan_entry_bytes();
+        if (ntiles) *ntiles = nt;
+        if (entry_bytes) *entry_bytes = nb;
+        if (tiles_out && tiles_cap < nt * sizeof(blinky::TileDesc)) return set_err(ctx, BLINKY_E_INVALID, "tile buffer too small");
+        if (entries_out && entries_cap < nb) return set_err(ctx, BLINKY_E_INVALID, "entry buffer too small");
+        return ctx->dev->download_plan(tiles_out, entries_out, entries_out ? nb : 0) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
+    }
+    if (!host_map(ctx)) return BLINKY_E_CUDA;
     blinky::TilePlan pl = current_plan(ctx, ctx->host.worker_threads());
     if (ntiles) *ntiles = pl.tiles.size();
     if (entry_bytes) *entry_bytes = pl.entries.size();
@@ -560,7 +636,7 @@ int blinky_get_tile_plan(blinky_ctx *ctx, void *tiles_out, size_t tiles_cap, voi
 }
 
 uint64_t blinky_plan_digest(blinky_ctx *ctx, int threads) {
-    if (!ctx->host.built()) return 0;
+    if (!ctx->host.built() || !host_map(ctx)) return 0;
     blinky::TilePlan pl = current_plan(ctx, threads);
     uint64_t h = 1469598103934665603ull;  // FNV-1a over the tile table and the entry blocks
     auto mix = [&](const void *p, size_t n) {

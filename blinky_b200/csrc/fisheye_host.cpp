@@ -1483,6 +1483,8 @@ int FisheyeHost::build_lensmap(int width, int height, int platesize, int threads
     idx_.assign(area, -1);
     tint_.assign(area, 255);
     built_ = false;
+    map_on_host_ = true;
+    map_plates_ = numplates_;
     mapped_ = 0;
 
     using clk = std::chrono::steady_clock;
@@ -1626,6 +1628,111 @@ void FisheyeHost::finish_build() {
     span_off_[static_cast<size_t>(height_px_)] = static_cast<int32_t>(spans_.size() / 2);
     mapped_ = mapped;
     built_ = true;
+}
+
+// ---------------------------------------------------------------------------
+// supplied lensmaps: the caller's map in place of a build
+// ---------------------------------------------------------------------------
+
+bool FisheyeHost::check_lensmap_size(int width, int height, int platesize, int numplates, std::string *why) {
+    const char *bad = nullptr;
+    if (width <= 0 || height <= 0) bad = "width and height must be positive";
+    else if (numplates < 1 || numplates > kMaxPlates) bad = "numplates must be 1..6";
+    else if (platesize <= 0) bad = "platesize must be positive";
+    else if (static_cast<int64_t>(platesize) * platesize * numplates > (int64_t{1} << 28)) bad = "numplates * platesize^2 exceeds the 28-bit texel index";
+    if (bad && why) *why = bad;
+    return !bad;
+}
+
+bool FisheyeHost::set_lensmap(int width, int height, int platesize, int numplates, const uint32_t *packed, std::string *why) {
+    if (!check_lensmap_size(width, height, platesize, numplates, why)) return false;
+    if (!packed) {
+        *why = "map is NULL";
+        return false;
+    }
+    const uint32_t limit = static_cast<uint32_t>(static_cast<int64_t>(platesize) * platesize * numplates);
+    const size_t W = static_cast<size_t>(width);
+    // checked in full before anything changes: a refused map leaves the current one in place
+    std::vector<int> first_bad(static_cast<size_t>(height), -1);
+    parallel_for(height, fallback_threads_, [&](int y) {
+        const uint32_t *row = packed + static_cast<size_t>(y) * W;
+        for (int x = 0; x < width; ++x) {
+            const uint32_t e = row[x];
+            if ((e & 0x80000000u) && ((e & 0x0FFFFFFFu) >= limit || ((e >> 28) & 7u) == 6u)) {
+                first_bad[static_cast<size_t>(y)] = x;
+                break;
+            }
+        }
+    });
+    for (int y = 0; y < height; ++y) {
+        const int x = first_bad[static_cast<size_t>(y)];
+        if (x < 0) continue;
+        const uint32_t e = packed[static_cast<size_t>(y) * W + static_cast<size_t>(x)];
+        char buf[160];
+        snprintf(buf, sizeof buf, "entry 0x%08x at (%d, %d): %s", e, x, y,
+                 ((e >> 28) & 7u) == 6u ? "tint 6 is not a tint" : "texel index beyond numplates * platesize^2");
+        *why = buf;
+        return false;
+    }
+    width_px_ = width;
+    height_px_ = height;
+    platesize_ = platesize;
+    unpack_map(packed);
+    map_plates_ = numplates;
+    finish_build();
+    // a plate is displayed when some mapped pixel samples it
+    for (int p = 0; p < kMaxPlates; ++p) plates_[p].display = p < numplates && plate_rect_[p][0] <= plate_rect_[p][2] ? 1 : 0;
+    lens_changed_ = globe_changed_ = zoom_changed_ = false;
+    built_w_ = width;
+    built_h_ = height;
+    built_ps_ = platesize;
+    return true;
+}
+
+void FisheyeHost::adopt_lensmap(int width, int height, int platesize, int numplates, const int display[kMaxPlates], const int rect[kMaxPlates][4],
+                                int64_t mapped, std::vector<int32_t> span_off, std::vector<int32_t> spans) {
+    width_px_ = width;
+    height_px_ = height;
+    platesize_ = platesize;
+    map_plates_ = numplates;
+    for (int p = 0; p < kMaxPlates; ++p) {
+        plates_[p].display = display[p];
+        for (int k = 0; k < 4; ++k) plate_rect_[p][k] = rect[p][k];
+    }
+    mapped_ = mapped;
+    span_off_ = std::move(span_off);
+    spans_ = std::move(spans);
+    idx_ = std::vector<int32_t>();
+    tint_ = std::vector<uint8_t>();
+    packed_ = std::vector<uint32_t>();
+    map_on_host_ = false;
+    built_ = true;
+    lens_changed_ = globe_changed_ = zoom_changed_ = false;
+    built_w_ = width;
+    built_h_ = height;
+    built_ps_ = platesize;
+}
+
+void FisheyeHost::fill_lensmap(std::vector<uint32_t> normalised) {
+    packed_ = std::move(normalised);
+    unpack_map(packed_.data());
+}
+
+// idx_ / tint_ (the reference's terms) of a packed [height_px_][width_px_] map
+void FisheyeHost::unpack_map(const uint32_t *packed) {
+    const size_t W = static_cast<size_t>(width_px_);
+    idx_.resize(W * static_cast<size_t>(height_px_));
+    tint_.resize(idx_.size());
+    parallel_for(height_px_, fallback_threads_, [&](int y) {
+        const size_t at = static_cast<size_t>(y) * W;
+        for (size_t x = 0; x < W; ++x) {
+            const uint32_t e = packed[at + x], t = (e >> 28) & 7u;
+            const bool valid = (e & 0x80000000u) != 0;
+            idx_[at + x] = valid ? static_cast<int32_t>(e & 0x0FFFFFFFu) : -1;
+            tint_[at + x] = valid && t != 7u ? static_cast<uint8_t>(t) : 255;
+        }
+    });
+    map_on_host_ = true;
 }
 
 }  // namespace blinky

@@ -78,6 +78,23 @@ public:
     const std::string &build_info() const { return build_info_; }
     bool needs_rebuild(int width, int height, int platesize) const;
 
+    // ---- supplied lensmaps -------------------------------------------------------
+    // A caller's map replaces the current one as a build would (the lens, globe, zoom and rubix settings stay;
+    // the lens / globe / zoom change flags are consumed).  Entries without BLINKY_LM_VALID are stored unmapped
+    // whatever their other bits hold.  False, changing nothing, with the reason in *why, for a bad size, a NULL
+    // map, an index outside the plates or a tint of 6.
+    bool set_lensmap(int width, int height, int platesize, int numplates, const uint32_t *packed, std::string *why);
+    // the checks of set_lensmap that do not read the map
+    static bool check_lensmap_size(int width, int height, int platesize, int numplates, std::string *why);
+    // What a device planner derived from a map it checked and normalised itself (tile_plan_device.h): the state
+    // set_lensmap would compute, without the map.  The map follows with fill_lensmap when a query needs it.
+    void adopt_lensmap(int width, int height, int platesize, int numplates, const int display[kMaxPlates], const int rect[kMaxPlates][4],
+                       int64_t mapped, std::vector<int32_t> span_off, std::vector<int32_t> spans);
+    bool map_on_host() const { return map_on_host_; }
+    void fill_lensmap(std::vector<uint32_t> normalised);  // [height][width] entries as adopt_lensmap's planner stored them
+    // plates of the current lensmap: the globe's at a build, the caller's for a supplied map
+    int map_numplates() const { return map_plates_; }
+
     // ---- results -------------------------------------------------------------
     int width() const { return width_px_; }
     int height() const { return height_px_; }
@@ -176,6 +193,7 @@ private:
     int uv_to_screen(Worker &w, int plate, double u, double v, int *lx, int *ly);
     void draw_quad(const int *tl, const int *tr, const int *bl, const int *br, int plate, int px, int py, int *display);
     void finish_build();
+    void unpack_map(const uint32_t *packed);
 
     // Lua-visible C functions
     static void lua_latlon_to_ray(minilua::State &, const minilua::Value *, int, minilua::ValueList &, void *);
@@ -234,6 +252,8 @@ private:
 
     // lensmap
     bool built_ = false;
+    bool map_on_host_ = true;  // false after adopt_lensmap until fill_lensmap: idx_ / tint_ / packed_ are not the map yet
+    int map_plates_ = 0;
     int built_w_ = -1, built_h_ = -1, built_ps_ = -1;
     std::vector<int32_t> idx_;
     std::vector<uint8_t> tint_;

@@ -70,15 +70,9 @@ void plan_tile_row(const uint32_t *packed, int width, int height, int platesize,
         }
         bool box = allow_box && one_plate && one_tint;
         uint32_t bw = 0, bh = 0;
-        if (box) {
-            // TMA faults ("illegal instruction") unless the innermost coordinate is a multiple of
-            // 16 bytes (scripts/tma_probe.cu): start the box on a 16-texel
-            // boundary.  The row coordinate is unconstrained.
-            minx &= ~15u;
-            bw = ((maxx - minx + 1) + 15) / 16 * 16;
-            bh = ((maxy - miny + 1) + static_cast<uint32_t>(h_gran) - 1) / static_cast<uint32_t>(h_gran) * static_cast<uint32_t>(h_gran);
-            if (bw > static_cast<uint32_t>(kMaxBoxW) || bh > static_cast<uint32_t>(kMaxBoxH) || bw * bh > static_cast<uint32_t>(max_box_bytes)) box = false;
-        }
+        // (TMA faults, "illegal instruction", unless the innermost coordinate is a multiple of 16 bytes:
+        // scripts/tma_probe.cu)
+        if (box) box = tile_box(minx, maxx, miny, maxy, h_gran, max_box_bytes, &minx, &bw, &bh);
         std::vector<uint8_t> &blk = row.blocks[static_cast<size_t>(tx)];
         if (box) {
             d.type = nvalid == kTilePixels ? TILE_BOX_FULL : TILE_BOX;
@@ -94,15 +88,9 @@ void plan_tile_row(const uint32_t *packed, int width, int height, int platesize,
                 for (int i = 0; i < 32; ++i) {
                     int r, c;
                     box_lane_pixel(lane, i, &r, &c);
-                    const uint32_t e = tile[static_cast<size_t>(r) * kTileW + c];
-                    uint16_t v = 0;  // unmapped: offset 0 (a harmless read), not valid
-                    if (e & BLINKY_LM_VALID) {
-                        const uint32_t rem = (e & BLINKY_LM_INDEX_MASK) % ps2;
-                        const uint32_t py = rem / ps, px = rem % ps;
-                        v = static_cast<uint16_t>(kBoxValid | ((py - miny) * bw + (px - minx)));
-                        if (((e >> BLINKY_LM_TINT_SHIFT) & 7u) != BLINKY_LM_TINT_NONE) tinted[lane] |= 1u << i;
-                    }
-                    ent[((i >> 3) * 32 + lane) * 8 + (i & 7)] = v;
+                    bool tint;
+                    ent[box_entry_slot(lane, i)] = box_entry(tile[static_cast<size_t>(r) * kTileW + c], ps, ps2, minx, miny, bw, &tint);
+                    if (tint) tinted[lane] |= 1u << i;
                 }
             }
             row.box_bytes += static_cast<uint64_t>(bw) * bh;
@@ -119,8 +107,7 @@ void plan_tile_row(const uint32_t *packed, int width, int height, int platesize,
 
 }  // namespace
 
-TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int platesize, bool allow_box, int threads, int max_box_bytes) {
-    TilePlan plan;
+int plan_max_box_bytes(int max_box_bytes) {
     if (max_box_bytes <= 0) {
         max_box_bytes = kDefaultMaxBoxBytes;
         if (const char *e = getenv("BLINKY_MAX_BOX")) {
@@ -128,7 +115,12 @@ TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int plate
             if (v >= 128) max_box_bytes = v;
         }
     }
-    max_box_bytes = std::min(max_box_bytes, kBoxBytesLimit);
+    return std::min(max_box_bytes, kBoxBytesLimit);
+}
+
+TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int platesize, bool allow_box, int threads, int max_box_bytes) {
+    TilePlan plan;
+    max_box_bytes = plan_max_box_bytes(max_box_bytes);
     plan.max_box_bytes = max_box_bytes;
     plan.width = width;
     plan.height = height;

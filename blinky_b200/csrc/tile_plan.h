@@ -62,10 +62,50 @@ constexpr int kBoxBlockBytes = kBoxEntryBytes + kBoxTintBytes;
 // Entry block of a GATHER tile: [32][32] uint32 in the packed BLINKY_LM_* format, row-major.
 constexpr int kGatherBlockBytes = kTilePixels * 4;
 
-inline void box_lane_pixel(int lane, int i, int *row, int *col) {
+// The per-tile rules below are shared by make_tile_plan (host threads) and the device planner
+// (tile_plan_device.cu), so that both produce the same plan byte for byte.
+// (the same definition as face_layout.h's)
+#if defined(__CUDACC__)
+#define BLINKY_HD __host__ __device__ __forceinline__
+#else
+#define BLINKY_HD inline
+#endif
+
+BLINKY_HD void box_lane_pixel(int lane, int i, int *row, int *col) {
     *row = (lane >> 3) + 4 * (i >> 2);
     *col = 4 * (lane & 7) + (i & 3);
 }
+
+// Where entry i of lane `lane` sits among the [4][32][8] uint16 entries of a BOX block.
+BLINKY_HD int box_entry_slot(int lane, int i) { return ((i >> 3) * 32 + lane) * 8 + (i & 7); }
+
+// The box of a tile whose single-plate, single-tint mapped texels span [minx, maxx] x [miny, maxy]:
+// origin x rounded down to 16 texels (TMA needs 16-byte aligned inner coordinates; the row coordinate is
+// unconstrained), width a multiple of 16, height a multiple of h_gran.  False when the box is too large to
+// stage, which makes the tile a GATHER tile.
+BLINKY_HD bool tile_box(uint32_t minx, uint32_t maxx, uint32_t miny, uint32_t maxy, int h_gran, int max_box_bytes, uint32_t *box_x,
+                     uint32_t *bw, uint32_t *bh) {
+    const uint32_t g = static_cast<uint32_t>(h_gran);
+    *box_x = minx & ~15u;
+    *bw = ((maxx - *box_x + 1) + 15) / 16 * 16;
+    *bh = ((maxy - miny + 1) + g - 1) / g * g;
+    return !(*bw > static_cast<uint32_t>(kMaxBoxW) || *bh > static_cast<uint32_t>(kMaxBoxH) || *bw * *bh > static_cast<uint32_t>(max_box_bytes));
+}
+
+// 16-bit BOX entry of packed lensmap entry e in the box at (box_x, box_y), bw texels wide; unmapped pixels get
+// offset 0 (a harmless read), not valid.  *tinted: the pixel carries a tint.
+BLINKY_HD uint16_t box_entry(uint32_t e, uint32_t ps, uint32_t ps2, uint32_t box_x, uint32_t box_y, uint32_t bw, bool *tinted) {
+    *tinted = false;
+    if (!(e & 0x80000000u)) return 0;
+    const uint32_t rem = (e & 0x0FFFFFFFu) % ps2;
+    const uint32_t py = rem / ps, px = rem % ps;
+    *tinted = ((e >> 28) & 7u) != 7u;
+    return static_cast<uint16_t>(kBoxValid | ((py - box_y) * bw + (px - box_x)));
+}
+
+// Index of a box shape (w16 1..16, h8 1..32) in a 512-entry table.
+BLINKY_HD int shape_slot(int w16, int h8) { return (w16 - 1) * 32 + (h8 - 1); }
+constexpr int kShapeSlots = 16 * 32;
 
 struct TileDesc {       // 16 bytes, read by the kernel
     uint32_t entry_offset;  // byte offset of the tile's entry block (= what the index-based rule gives)
@@ -99,5 +139,8 @@ struct TilePlan {
 // plan without tiles.
 TilePlan make_tile_plan(const uint32_t *packed, int width, int height, int platesize, bool allow_box, int threads = 1,
                         int max_box_bytes = 0);
+
+// The box size cap a plan uses for a requested max_box_bytes (<= 0: the default, or BLINKY_MAX_BOX when set).
+int plan_max_box_bytes(int max_box_bytes);
 
 }  // namespace blinky

@@ -24,6 +24,7 @@
 #include "face_layout.h"
 #include "launch_plan.h"
 #include "tile_plan.h"
+#include "tile_plan_device.h"
 
 namespace blinky {
 
@@ -1027,11 +1028,27 @@ WarpDevice::~WarpDevice() {
     for (void *p : retired_) cudaFree(p);
 }
 
+size_t WarpDevice::padded_pixels(size_t npix) { return round_up(npix, kPixelsPerBlock); }
+
+bool WarpDevice::download_lensmap(uint32_t *out) {
+    CK(cudaSetDevice(device_));
+    CK(cudaMemcpy(out, d_lensmap_, npix_ * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return true;
+}
+
+bool WarpDevice::download_plan(void *tiles, void *entries, size_t entry_bytes) {
+    CK(cudaSetDevice(device_));
+    if (!have_plan_) return true;
+    if (tiles && ntiles_) CK(cudaMemcpy(tiles, d_tiles_, ntiles_ * sizeof(TileDesc), cudaMemcpyDeviceToHost));
+    if (entries && entry_bytes) CK(cudaMemcpy(entries, d_entries_, entry_bytes, cudaMemcpyDeviceToHost));
+    return true;
+}
+
 bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
     CK(cudaSetDevice(device_));
     CK(cudaDeviceSynchronize());  // nothing may still be reading the old map
     const size_t npix = static_cast<size_t>(lm.width) * lm.height;
-    const size_t npad = round_up(npix, kPixelsPerBlock);
+    const size_t npad = padded_pixels(npix);
     // A graph captured since the last upload keeps rendering the lensmap and plan it was captured with: their buffers
     // are retired instead of freed or rewritten.  The background stays shared while the view size stays the same, so
     // it is retired when it is replaced and any graph captured since it was allocated reads it.
@@ -1041,7 +1058,10 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
         p = nullptr;
     };
     const bool resize = npad != npix_pad_, new_view = resize || lm.width != width_ || lm.height != height_;
-    if (resize || captured_) {
+    if (lm.device) {
+        drop(d_lensmap_, captured_);
+        d_lensmap_ = lm.device->d_map;
+    } else if (resize || captured_) {
         drop(d_lensmap_, captured_);
         CK(cudaMalloc(&d_lensmap_, npad * sizeof(uint32_t)));
     }
@@ -1051,9 +1071,11 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
         CK(cudaMalloc(&d_bg_, npad));
     }
     if (new_view) CK(cudaMemset(d_bg_, 0, npad));
-    // padding entries are "unmapped"
-    CK(cudaMemset(d_lensmap_, 0, npad * sizeof(uint32_t)));
-    CK(cudaMemcpy(d_lensmap_, lm.packed, npix * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (!lm.device) {
+        // padding entries are "unmapped"
+        CK(cudaMemset(d_lensmap_, 0, npad * sizeof(uint32_t)));
+        CK(cudaMemcpy(d_lensmap_, lm.packed, npix * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    }
     CK(cudaMemcpy(d_lut_, lm.palmaps, 6 * 256, cudaMemcpyHostToDevice));
     width_ = lm.width;
     height_ = lm.height;
@@ -1075,13 +1097,21 @@ bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
     captured_ = false;
     for (TmapSet *t : tmap_sets_) delete t;
     tmap_sets_.clear();
-    if (lm.plan && !lm.plan->tiles.empty()) {
-        const TilePlan &pl = *lm.plan;
-        CK(cudaMalloc(&d_tiles_, pl.tiles.size() * sizeof(TileDesc)));
-        CK(cudaMemcpy(d_tiles_, pl.tiles.data(), pl.tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
-        CK(cudaMalloc(&d_entries_, pl.entries.size()));
-        CK(cudaMemcpy(d_entries_, pl.entries.data(), pl.entries.size(), cudaMemcpyHostToDevice));
-        ntiles_ = static_cast<uint32_t>(pl.tiles.size());
+    if (lm.device ? lm.device->ntiles > 0 : lm.plan && !lm.plan->tiles.empty()) {
+        const TilePlan &pl = lm.device ? lm.device->plan : *lm.plan;
+        if (lm.device) {
+            d_tiles_ = lm.device->d_tiles;
+            d_entries_ = lm.device->d_entries;
+            ntiles_ = lm.device->ntiles;
+            entry_bytes_ = lm.device->entry_bytes;
+        } else {
+            CK(cudaMalloc(&d_tiles_, pl.tiles.size() * sizeof(TileDesc)));
+            CK(cudaMemcpy(d_tiles_, pl.tiles.data(), pl.tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+            CK(cudaMalloc(&d_entries_, pl.entries.size()));
+            CK(cudaMemcpy(d_entries_, pl.entries.data(), pl.entries.size(), cudaMemcpyHostToDevice));
+            ntiles_ = static_cast<uint32_t>(pl.tiles.size());
+            entry_bytes_ = pl.entries.size();
+        }
         nbox_tiles_ = static_cast<uint32_t>(pl.n_box);
         ngather_tiles_ = static_cast<uint32_t>(pl.n_gather);
         stage_bytes_ = pl.stage_bytes;

@@ -16,12 +16,16 @@
 namespace blinky {
 
 struct TilePlan;       // tile_plan.h
+struct DevicePlan;     // tile_plan_device.h
 struct KernelVariant;  // launch_plan.h
 enum class WarpKernel;
 
 struct LensmapUpload {
     int width = 0, height = 0, platesize = 0, numplates = 0;
     const uint32_t *packed = nullptr;        // [height*width]
+    // instead of packed and plan: a map and tile plan already in device memory (plan_lensmap_device), whose
+    // buffers the device takes over as its new generation
+    const DevicePlan *device = nullptr;
     const uint8_t *palmaps = nullptr;        // [6*256]
     int display[6] = {0, 0, 0, 0, 0, 0};
     int plate_rect[6][4] = {};               // texel rectangle each plate is sampled in (x0,y0,x1,y1)
@@ -75,6 +79,13 @@ public:
     // size of the resident lensmap's view (0 before the first upload)
     int width() const { return width_; }
     int height() const { return height_; }
+    // entries of a device lensmap buffer for npix pixels (the kernels read whole blocks; the padding is unmapped)
+    static size_t padded_pixels(size_t npix);
+    // copies of the resident map ([height][width] entries) and tile plan, synchronously
+    bool download_lensmap(uint32_t *out);
+    bool download_plan(void *tiles, void *entries, size_t entry_bytes);
+    size_t plan_tiles() const { return have_plan_ ? ntiles_ : 0; }
+    size_t plan_entry_bytes() const { return have_plan_ ? entry_bytes_ : 0; }
 
     bool warp(const WarpRequest &r);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, frees
@@ -140,6 +151,7 @@ private:
     bool plan_has_box_ = false;
     void *d_tiles_ = nullptr;       // TileDesc[]
     uint8_t *d_entries_ = nullptr;
+    size_t entry_bytes_ = 0;
     uint32_t ntiles_ = 0, nbox_tiles_ = 0, ngather_tiles_ = 0;
     int stage_bytes_ = 0;                // largest staged box of the plan
     int static_pct_ = 85;                // share of the ring kernel's units scheduled statically (BLINKY_STATIC_PCT)

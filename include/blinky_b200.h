@@ -144,6 +144,31 @@ int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes);
 /* 1 if a lens/globe/zoom/rubixgrid/size change since the last build requires a rebuild (:730) */
 int blinky_needs_rebuild(blinky_ctx *ctx, int width, int height, int platesize);
 
+/* Supplied lensmaps: a map the caller made (a calibrated projector or dome warp exported by another
+ * tool, a lens the host evaluates itself, a zoom or morph computed by the host's own kernel) replaces
+ * the current lensmap as a build would.  map: width*height entries in the BLINKY_LM_* format,
+ * row-major, dense (row pitch = width), indexing numplates plates of platesize^2 texels.
+ * Everything that reads the lensmap then reads this one: the warps, blinky_get_lensmap[_packed],
+ * blinky_get_display (a plate is displayed when some mapped entry samples it), blinky_mapped_pixels,
+ * the tile plan and its queries, blinky_upload_bytes_per_frame, blinky_save_globe and the face-layout
+ * checks.  The lens, globe, zoom and rubix settings stay as they are; like a build, the call consumes
+ * the lens / globe / zoom changes, so blinky_needs_rebuild is 0 for this size until the next change.
+ * An entry without BLINKY_LM_VALID is unmapped whatever its other bits hold and is stored as
+ * BLINKY_LM_TINT_NONE << 28, so the map plans and reads back like a build's.  BLINKY_E_INVALID,
+ * changing nothing and launching nothing, for a NULL map, width or height <= 0, numplates outside
+ * 1..6, platesize <= 0, numplates * platesize^2 above 2^28, or a mapped entry whose index is not below
+ * numplates * platesize^2 or whose tint is 6.  A screen wider or taller than 65536 pixels gets no tile
+ * plan (the direct-gather kernels warp it).  A graph that captured a warp before the call keeps
+ * rendering the map it captured until blinky_release_captures.
+ * blinky_set_lensmap reads host memory and also works on host-only contexts (the planner and the
+ * queries without a GPU).  blinky_set_lensmap_device reads device memory on `stream` (a cudaStream_t,
+ * NULL = the default stream) after the work already there, checks and plans the map on the GPU, and
+ * returns once the map is resident: the caller may then reuse d_packed.  BLINKY_E_NODEVICE on a
+ * host-only context.  The map itself is copied to the host only when a host-side query needs it. */
+int blinky_set_lensmap(blinky_ctx *ctx, int width, int height, int platesize, int numplates, const uint32_t *packed);
+int blinky_set_lensmap_device(blinky_ctx *ctx, int width, int height, int platesize, int numplates, const uint32_t *d_packed,
+                              void *stream);
+
 /* ---- state queries ------------------------------------------------------ */
 int blinky_fisheye_enabled(blinky_ctx *ctx);          /* fisheye_enabled, :293 */
 int blinky_lens_valid(blinky_ctx *ctx);
@@ -264,8 +289,8 @@ int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
  *   - the face layout (blinky_set_face_layout) that was in effect at capture.
  * Each captured launch of the ring kernel takes one of 4096 work counters; when none is left the call
  * fails with BLINKY_E_STATE and launches nothing.  blinky_warp_host, blinky_shard_warp_gather,
- * blinky_build_lensmap, blinky_set_background and blinky_set_rgba_table must not be called while a
- * stream is capturing. */
+ * blinky_build_lensmap, blinky_set_lensmap, blinky_set_lensmap_device, blinky_set_background and
+ * blinky_set_rgba_table must not be called while a stream is capturing. */
 int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen,
                             size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
                             int keep_unmapped, void *stream);
