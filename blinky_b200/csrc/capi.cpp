@@ -34,7 +34,6 @@ struct blinky_ctx {
     std::string build_info;
     std::string err;
     std::string scratch;
-    uint8_t palmaps[BLINKY_MAX_PLATES * 256];
     int layout_rowbytes = 0;              // blinky_set_face_layout: 0 = dense faces
     std::vector<int32_t> layout_origins;  // (x, y) per plate
     bool device_plan = false;             // the resident tile plan was made on the GPU (blinky_set_lensmap_device)
@@ -85,36 +84,41 @@ bool host_map(blinky_ctx *c) {
     return true;
 }
 
-// The device upload of the current lensmap: the host's map, planned here, or (device != null) a map and plan the
-// GPU planner left in device memory.
-bool upload(blinky_ctx *c, const blinky::DevicePlan *device = nullptr) {
+// the plates' palette LUTs, as the device keeps them
+void plate_luts(blinky_ctx *c, uint8_t out[BLINKY_MAX_PLATES * 256]) {
+    for (int i = 0; i < BLINKY_MAX_PLATES; ++i) memcpy(out + i * 256, c->host.plate(i).palette, 256);
+}
+
+// Installs the current lensmap on the device: the host's map, planned and staged here, or (device != null) a map and
+// plan the GPU planner left in device memory.
+bool upload(blinky_ctx *c, blinky::DevicePlan *device = nullptr) {
     if (!c->dev || !c->host.built()) return true;
-    if (!device && !host_map(c)) return false;
+    blinky::DevicePlan staged;
+    if (!device) {
+        if (!host_map(c)) return false;
+        const size_t npix = static_cast<size_t>(c->host.width()) * c->host.height();
+        if (blinky::stage_lensmap_host(c->dev->device(), c->host.packed().data(), npix, WarpDevice::padded_pixels(npix),
+                                       current_plan(c, c->host.worker_threads()), &staged, &c->err) != BLINKY_OK)
+            return false;
+    }
     blinky::LensmapUpload lm;
     lm.width = c->host.width();
     lm.height = c->host.height();
     lm.platesize = c->host.platesize();
     lm.numplates = c->host.map_numplates();
     for (int i = 0; i < BLINKY_MAX_PLATES; ++i) {
-        memcpy(c->palmaps + i * 256, c->host.plate(i).palette, 256);
         lm.display[i] = i < c->host.map_numplates() ? c->host.plate(i).display : 0;
         memcpy(lm.plate_rect[i], c->host.plate_rect(i), sizeof lm.plate_rect[i]);
     }
-    lm.palmaps = c->palmaps;
+    uint8_t luts[BLINKY_MAX_PLATES * 256];
+    plate_luts(c, luts);
+    lm.palmaps = luts;
     lm.rubix = c->host.rubix_enabled();
     lm.span_off = c->host.row_span_offsets().data();
     lm.spans = c->host.row_spans().data();
     lm.nspans = c->host.row_spans().size() / 2;
-    blinky::TilePlan plan;
-    if (device) {
-        lm.device = device;
-    } else {
-        lm.packed = c->host.packed().data();
-        plan = current_plan(c, c->host.worker_threads());
-        lm.plan = &plan;
-    }
     c->device_plan = device != nullptr;
-    if (!c->dev->upload_lensmap(lm)) {
+    if (!c->dev->install(lm, std::move(device ? *device : staged))) {
         c->err = c->dev->last_error();
         return false;
     }
@@ -134,7 +138,6 @@ int blinky_create(int device, blinky_ctx **out) {
     } catch (std::exception &) {
         return BLINKY_E_NOMEM;
     }
-    memset(c->palmaps, 0, sizeof c->palmaps);
     c->host.set_worker_threads(usable_cpus());
     if (device >= 0) {
         try {
@@ -171,8 +174,10 @@ int blinky_set_basedir(blinky_ctx *ctx, const char *basedir) {
 int blinky_set_palette(blinky_ctx *ctx, const uint8_t palette[768]) {
     if (!palette) return set_err(ctx, BLINKY_E_INVALID, "palette is NULL");
     ctx->host.set_palette(palette);
-    if (!upload(ctx)) return BLINKY_E_CUDA;
-    return BLINKY_OK;
+    if (!ctx->dev || !ctx->host.built()) return BLINKY_OK;
+    uint8_t luts[BLINKY_MAX_PLATES * 256];
+    plate_luts(ctx, luts);
+    return ctx->dev->set_luts(luts) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, ctx->dev->last_error());
 }
 
 int blinky_command(blinky_ctx *ctx, const char *text) {

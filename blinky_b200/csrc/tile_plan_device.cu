@@ -244,19 +244,26 @@ __global__ void row_spans_kernel(const uint32_t *__restrict__ map, int width, in
     if (prev && lane == 0) out[2 * nend + 1] = width;  // a run that reaches the last column
 }
 
+// *why = "<who>: <call>: <CUDA error>"
+int cuda_failed(std::string *why, const char *who, const char *what, cudaError_t e) {
+    char buf[256];
+    snprintf(buf, sizeof buf, "%s: %s: %s", who, what, cudaGetErrorString(e));
+    *why = buf;
+    return BLINKY_E_CUDA;
+}
+
 }  // namespace
 
-void DevicePlan::release() {
-    cudaFree(d_map);
-    cudaFree(d_tiles);
-    cudaFree(d_entries);
-    d_map = nullptr;
-    d_tiles = nullptr;
-    d_entries = nullptr;
-}
+// (on the way out, every buffer is freed by its owner: the temporaries here, *out's by the caller's DevicePlan)
+#define PK(call)                                                           \
+    do {                                                                   \
+        const cudaError_t e_ = static_cast<cudaError_t>(call);             \
+        if (e_ != cudaSuccess) return cuda_failed(why, who, #call, e_); \
+    } while (0)
 
 int plan_lensmap_device(int device, const uint32_t *d_packed, int width, int height, int platesize, int numplates, size_t padded_pixels,
                         void *stream, DevicePlan *out, std::string *why) {
+    const char *who = "blinky_set_lensmap_device";
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const size_t npix = static_cast<size_t>(width) * height;
     const uint32_t ps = static_cast<uint32_t>(platesize), ps2 = ps * ps;
@@ -272,80 +279,53 @@ int plan_lensmap_device(int device, const uint32_t *d_packed, int width, int hei
         plan.tiles_y = (height + kTileH - 1) / kTileH;
     }
     const uint32_t ntiles = static_cast<uint32_t>(plan.tiles_x) * static_cast<uint32_t>(plan.tiles_y);
-
-    // temporaries, freed on every way out
-    MapSummary *d_msum = nullptr;
-    TileSummary *d_tsum = nullptr;
-    int32_t *d_row_runs = nullptr, *d_span_off = nullptr, *d_spans = nullptr;
-    TileDesc *d_desc = nullptr;
-    unsigned long long *d_cls = nullptr, *d_before = nullptr;
-    uint8_t *d_shape_index = nullptr;
-    void *d_scratch = nullptr;
-    auto cleanup = [&]() {
-        cudaFree(d_msum);
-        cudaFree(d_tsum);
-        cudaFree(d_row_runs);
-        cudaFree(d_span_off);
-        cudaFree(d_spans);
-        cudaFree(d_desc);
-        cudaFree(d_cls);
-        cudaFree(d_before);
-        cudaFree(d_shape_index);
-        cudaFree(d_scratch);
-    };
-    auto cuda_failed = [&](const char *what, cudaError_t e) {
-        char buf[256];
-        snprintf(buf, sizeof buf, "blinky_set_lensmap_device: %s: %s", what, cudaGetErrorString(e));
-        *why = buf;
-        cleanup();
-        out->release();
-        return BLINKY_E_CUDA;
-    };
-#define PK(call)                                               \
-    do {                                                       \
-        cudaError_t e_ = (call);                               \
-        if (e_ != cudaSuccess) return cuda_failed(#call, e_); \
-    } while (0)
+    DeviceBuffer msum_buf, tsum_buf, row_runs_buf, span_off_buf, spans_buf, desc_buf, cls_buf, before_buf, shape_index_buf, scratch;
 
     // 1. per pixel
     PK(cudaSetDevice(device));
-    PK(cudaMalloc(&out->d_map, padded_pixels * sizeof(uint32_t)));
-    PK(cudaMalloc(&d_msum, sizeof(MapSummary)));
-    PK(cudaMalloc(&d_row_runs, (static_cast<size_t>(height) + 1) * sizeof(int32_t)));
-    PK(cudaMalloc(&d_span_off, (static_cast<size_t>(height) + 1) * sizeof(int32_t)));
+    PK(out->d_map.alloc(padded_pixels * sizeof(uint32_t)));
+    PK(msum_buf.alloc(sizeof(MapSummary)));
+    PK(row_runs_buf.alloc((static_cast<size_t>(height) + 1) * sizeof(int32_t)));
+    PK(span_off_buf.alloc((static_cast<size_t>(height) + 1) * sizeof(int32_t)));
+    uint32_t *d_map = out->d_map.as<uint32_t>();
+    MapSummary *d_msum = msum_buf.as<MapSummary>();
+    int32_t *d_row_runs = row_runs_buf.as<int32_t>(), *d_span_off = span_off_buf.as<int32_t>();
     MapSummary msum_init = {0, 0, ~0ull, {}};
     for (int p = 0; p < kMaxPlanPlates; ++p) {
         msum_init.rect[p][0] = msum_init.rect[p][1] = platesize;
         msum_init.rect[p][2] = msum_init.rect[p][3] = -1;
     }
     PK(cudaMemcpyAsync(d_msum, &msum_init, sizeof msum_init, cudaMemcpyHostToDevice, s));
-    if (padded_pixels > npix) PK(cudaMemsetAsync(out->d_map + npix, 0, (padded_pixels - npix) * sizeof(uint32_t), s));
+    if (padded_pixels > npix) PK(cudaMemsetAsync(d_map + npix, 0, (padded_pixels - npix) * sizeof(uint32_t), s));
     PK(cudaMemsetAsync(d_row_runs + height, 0, sizeof(int32_t), s));
     const uint32_t limit = static_cast<uint32_t>(static_cast<uint64_t>(ps2) * static_cast<uint32_t>(numplates));
-    check_map_kernel<<<height, kRowThreads, 0, s>>>(d_packed, out->d_map, width, ps, limit, d_msum, d_row_runs);
+    check_map_kernel<<<height, kRowThreads, 0, s>>>(d_packed, d_map, width, ps, limit, d_msum, d_row_runs);
     PK(cudaGetLastError());
 
     // 2. per tile, at box heights in multiples of 8 rows, coarsened until the shapes fit
     PlanGeometry g = {width, height, plan.tiles_x, ntiles, ps, ps2, platesize % 16 == 0, 8, plan.max_box_bytes};
     const unsigned tile_ctas = (ntiles + kTilesPerCta - 1) / kTilesPerCta;
     TileSummary tsum = {};
+    if (ntiles) {
+        PK(tsum_buf.alloc(sizeof(TileSummary)));
+        PK(desc_buf.alloc(ntiles * sizeof(TileDesc)));
+        PK(cls_buf.alloc(ntiles * sizeof(unsigned long long)));
+        PK(before_buf.alloc(ntiles * sizeof(unsigned long long)));
+    }
+    TileSummary *d_tsum = tsum_buf.as<TileSummary>();
+    TileDesc *d_desc = desc_buf.as<TileDesc>();
+    unsigned long long *d_cls = cls_buf.as<unsigned long long>(), *d_before = before_buf.as<unsigned long long>();
     auto classify = [&]() -> cudaError_t {
         memset(&tsum, 0, sizeof tsum);
         std::fill(tsum.shape_first, tsum.shape_first + kShapeSlots, INT_MAX);
         cudaError_t e = cudaMemcpyAsync(d_tsum, &tsum, sizeof tsum, cudaMemcpyHostToDevice, s);
         if (e != cudaSuccess) return e;
-        classify_kernel<<<tile_ctas, kTilesPerCta * 32, 0, s>>>(out->d_map, g, d_desc, d_cls, d_tsum);
+        classify_kernel<<<tile_ctas, kTilesPerCta * 32, 0, s>>>(d_map, g, d_desc, d_cls, d_tsum);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaMemcpyAsync(&tsum, d_tsum, sizeof tsum, cudaMemcpyDeviceToHost, s);
         return e;
     };
-    if (ntiles) {
-        PK(cudaMalloc(&d_tsum, sizeof(TileSummary)));
-        PK(cudaMalloc(&d_desc, ntiles * sizeof(TileDesc)));
-        PK(cudaMalloc(&d_cls, ntiles * sizeof(unsigned long long)));
-        PK(cudaMalloc(&d_before, ntiles * sizeof(unsigned long long)));
-        PK(classify());
-    }
+    if (ntiles) PK(classify());
     MapSummary msum;
     PK(cudaMemcpyAsync(&msum, d_msum, sizeof msum, cudaMemcpyDeviceToHost, s));
     PK(cudaStreamSynchronize(s));
@@ -356,8 +336,6 @@ int plan_lensmap_device(int device, const uint32_t *d_packed, int width, int hei
         snprintf(buf, sizeof buf, "blinky_set_lensmap_device: entry 0x%08x at (%llu, %llu): %s", e, msum.bad_at % static_cast<unsigned>(width),
                  msum.bad_at / static_cast<unsigned>(width), ((e >> 28) & 7u) == 6u ? "tint 6 is not a tint" : "texel index beyond numplates * platesize^2");
         *why = buf;
-        cleanup();
-        out->release();
         return BLINKY_E_INVALID;
     }
     std::vector<std::pair<int, uint16_t>> first;  // (first BOX tile, shape)
@@ -397,37 +375,35 @@ int plan_lensmap_device(int device, const uint32_t *d_packed, int width, int hei
         PK(cub::DeviceScan::ExclusiveSum(nullptr, b, d_cls, d_before, ntiles, s));
         scratch_bytes = std::max(scratch_bytes, b);
     }
-    PK(cudaMalloc(&d_scratch, scratch_bytes));
-    PK(cub::DeviceScan::ExclusiveSum(d_scratch, scratch_bytes, d_row_runs, d_span_off, height + 1, s));
+    PK(scratch.alloc(scratch_bytes));
+    PK(cub::DeviceScan::ExclusiveSum(scratch.get(), scratch_bytes, d_row_runs, d_span_off, height + 1, s));
 
     // 4. descriptors and entry blocks
     if (ntiles) {
-        PK(cub::DeviceScan::ExclusiveSum(d_scratch, scratch_bytes, d_cls, d_before, ntiles, s));
+        PK(cub::DeviceScan::ExclusiveSum(scratch.get(), scratch_bytes, d_cls, d_before, ntiles, s));
         out->ntiles = ntiles;
         out->entry_bytes = static_cast<size_t>(plan.n_box) * kBoxBlockBytes + static_cast<size_t>(plan.n_gather) * kGatherBlockBytes + 16;
-        PK(cudaMalloc(&out->d_tiles, ntiles * sizeof(TileDesc)));
-        PK(cudaMalloc(&out->d_entries, out->entry_bytes));
-        PK(cudaMalloc(&d_shape_index, sizeof shape_index));
-        PK(cudaMemcpyAsync(d_shape_index, shape_index, sizeof shape_index, cudaMemcpyHostToDevice, s));
-        PK(cudaMemsetAsync(out->d_entries + out->entry_bytes - 16, 0, 16, s));  // the kernels may prefetch one 16-byte vector past a block
-        write_plan_kernel<<<tile_ctas, kTilesPerCta * 32, 0, s>>>(out->d_map, g, d_desc, d_before, d_shape_index, tsum.n_box, tsum.n_gather,
-                                                                 static_cast<TileDesc *>(out->d_tiles), out->d_entries);
+        PK(out->d_tiles.alloc(ntiles * sizeof(TileDesc)));
+        PK(out->d_entries.alloc(out->entry_bytes));
+        PK(shape_index_buf.alloc(sizeof shape_index));
+        PK(cudaMemcpyAsync(shape_index_buf.get(), shape_index, sizeof shape_index, cudaMemcpyHostToDevice, s));
+        PK(cudaMemsetAsync(out->d_entries.as<uint8_t>() + out->entry_bytes - 16, 0, 16, s));  // the kernels may prefetch one 16-byte vector past a block
+        write_plan_kernel<<<tile_ctas, kTilesPerCta * 32, 0, s>>>(d_map, g, d_desc, d_before, shape_index_buf.as<uint8_t>(), tsum.n_box, tsum.n_gather,
+                                                                 out->d_tiles.as<TileDesc>(), out->d_entries.as<uint8_t>());
         PK(cudaGetLastError());
     }
 
     // 5. row spans
     if (msum.runs) {
-        PK(cudaMalloc(&d_spans, msum.runs * 2 * sizeof(int32_t)));
-        row_spans_kernel<<<(height + kTilesPerCta - 1) / kTilesPerCta, kTilesPerCta * 32, 0, s>>>(out->d_map, width, height, d_span_off, d_spans);
+        PK(spans_buf.alloc(msum.runs * 2 * sizeof(int32_t)));
+        row_spans_kernel<<<(height + kTilesPerCta - 1) / kTilesPerCta, kTilesPerCta * 32, 0, s>>>(d_map, width, height, d_span_off, spans_buf.as<int32_t>());
         PK(cudaGetLastError());
     }
     out->span_off.resize(static_cast<size_t>(height) + 1);
     out->spans.resize(msum.runs * 2);
     PK(cudaMemcpyAsync(out->span_off.data(), d_span_off, out->span_off.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (msum.runs) PK(cudaMemcpyAsync(out->spans.data(), d_spans, out->spans.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (msum.runs) PK(cudaMemcpyAsync(out->spans.data(), spans_buf.get(), out->spans.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     PK(cudaStreamSynchronize(s));
-#undef PK
-    cleanup();
     out->mapped = static_cast<int64_t>(msum.mapped);
     for (int p = 0; p < kMaxPlanPlates; ++p) {
         for (int k = 0; k < 4; ++k) out->rect[p][k] = msum.rect[p][k];
@@ -435,5 +411,26 @@ int plan_lensmap_device(int device, const uint32_t *d_packed, int width, int hei
     }
     return BLINKY_OK;
 }
+
+int stage_lensmap_host(int device, const uint32_t *packed, size_t npix, size_t padded_pixels, TilePlan plan, DevicePlan *out,
+                       std::string *why) {
+    const char *who = "lensmap upload";
+    *out = DevicePlan();
+    PK(cudaSetDevice(device));
+    PK(out->d_map.alloc(padded_pixels * sizeof(uint32_t)));
+    PK(cudaMemset(out->d_map.as<uint32_t>() + npix, 0, (padded_pixels - npix) * sizeof(uint32_t)));  // padding entries are unmapped
+    PK(cudaMemcpy(out->d_map.get(), packed, npix * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (!plan.tiles.empty()) {
+        out->ntiles = static_cast<uint32_t>(plan.tiles.size());
+        out->entry_bytes = plan.entries.size();
+        PK(out->d_tiles.alloc(plan.tiles.size() * sizeof(TileDesc)));
+        PK(cudaMemcpy(out->d_tiles.get(), plan.tiles.data(), plan.tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+        PK(out->d_entries.alloc(plan.entries.size()));
+        PK(cudaMemcpy(out->d_entries.get(), plan.entries.data(), plan.entries.size(), cudaMemcpyHostToDevice));
+    }
+    out->plan = std::move(plan);
+    return BLINKY_OK;
+}
+#undef PK
 
 }  // namespace blinky

@@ -932,13 +932,51 @@ constexpr uint32_t kCaptureSlots = 4096;   // work counters for captured ring la
 
 }  // namespace
 
+int DeviceBuffer::alloc(size_t bytes) {
+    reset();
+    return cudaMalloc(&p_, bytes);
+}
+
+void DeviceBuffer::reset() {
+    cudaFree(p_);
+    p_ = nullptr;
+}
+
+// What one install makes resident: the lensmap's view, its map and tile plan, and the background.  Immutable once
+// installed, except for the background's contents (set_background); captured graphs hold it (held_) while they may
+// still read it.
+struct WarpDevice::Generation {
+    int width = 0, height = 0, platesize = 0, numplates = 0;
+    size_t npix = 0, npix_pad = 0;
+    int display[6] = {0, 0, 0, 0, 0, 0};
+    int plate_rect[6][4] = {};
+    std::vector<int32_t> span_off, spans;
+    DeviceBuffer map;       // uint32_t[npix_pad]
+    // tiled layout (ring kernel)
+    bool have_plan = false, plan_has_box = false;
+    DeviceBuffer tiles;     // TileDesc[ntiles]
+    DeviceBuffer entries;   // entry_bytes of entry blocks
+    size_t entry_bytes = 0;
+    uint32_t ntiles = 0, nbox_tiles = 0, ngather_tiles = 0;
+    int stage_bytes = 0;    // largest staged box of the plan
+    std::vector<uint16_t> shapes;
+    // uint8_t[npix_pad]: shared by the generations of one view size (see install)
+    std::shared_ptr<DeviceBuffer> bg;
+};
+
 // ---------------------------------------------------------------------------
 // frame pipeline slot: one frame of blinky_warp_host in flight
 // ---------------------------------------------------------------------------
 struct WarpDevice::Slot {
+    ~Slot() {
+        if (stream) cudaStreamDestroy(stream);
+        if (done) cudaEventDestroy(done);
+        if (h_faces) cudaFreeHost(h_faces);
+        if (h_out) cudaFreeHost(h_out);
+    }
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
-    uint8_t *d_faces = nullptr, *d_out = nullptr;
+    DeviceBuffer d_faces, d_out;
     uint8_t *h_faces = nullptr, *h_out = nullptr;  // pinned staging
     bool busy = false;
     // finalize info
@@ -960,10 +998,10 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-#define CK(call)                                      \
-    do {                                              \
-        cudaError_t e_ = (call);                      \
-        if (e_ != cudaSuccess) return fail(#call, e_); \
+#define CK(call)                                                  \
+    do {                                                          \
+        const cudaError_t e_ = static_cast<cudaError_t>(call);    \
+        if (e_ != cudaSuccess) return fail(#call, e_);            \
     } while (0)
 
 bool WarpDevice::fail(const char *what, int cuda_err) {
@@ -994,160 +1032,116 @@ WarpDevice::WarpDevice(int device) : device_(device) {
     if (const char *e = getenv("BLINKY_FCHUNK")) fchunk_ = atoi(e);
     if (const char *e = getenv("BLINKY_SERIAL_GATHER")) serial_gather_ = atoi(e) != 0;  // GATHER tiles in their own kernel before the ring kernel (A/B)
     if (const char *e = getenv("BLINKY_STATIC_PCT")) static_pct_ = std::max(0, std::min(100, atoi(e)));
-    e = cudaMalloc(&d_lut_, 6 * 256);
-    if (e == cudaSuccess) e = cudaMemset(d_lut_, 0, 6 * 256);
-    if (e == cudaSuccess) e = cudaMalloc(&d_rgba_, 256 * 4);
-    if (e == cudaSuccess) e = cudaMemset(d_rgba_, 0, 256 * 4);
+    e = static_cast<cudaError_t>(d_lut_.alloc(6 * 256));
+    if (e == cudaSuccess) e = cudaMemset(d_lut_.get(), 0, 6 * 256);
+    if (e == cudaSuccess) e = static_cast<cudaError_t>(d_rgba_.alloc(256 * 4));
+    if (e == cudaSuccess) e = cudaMemset(d_rgba_.get(), 0, 256 * 4);
     // (here, not on first use: a capture may allocate nothing)
-    if (e == cudaSuccess) e = cudaMalloc(&d_capture_slots_, kCaptureSlots * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMemset(d_capture_slots_, 0, kCaptureSlots * sizeof(uint32_t));
+    if (e == cudaSuccess) e = static_cast<cudaError_t>(d_capture_slots_.alloc(kCaptureSlots * sizeof(uint32_t)));
+    if (e == cudaSuccess) e = cudaMemset(d_capture_slots_.get(), 0, kCaptureSlots * sizeof(uint32_t));
     if (e != cudaSuccess) throw std::runtime_error(std::string("cudaMalloc: ") + cudaGetErrorString(e));
 }
 
+// (the members then free what they own)
 WarpDevice::~WarpDevice() {
     cudaSetDevice(device_);
     cudaDeviceSynchronize();
-    for (Slot *s : slots_) {
-        if (s->stream) cudaStreamDestroy(s->stream);
-        if (s->done) cudaEventDestroy(s->done);
-        cudaFree(s->d_faces);
-        cudaFree(s->d_out);
-        if (s->h_faces) cudaFreeHost(s->h_faces);
-        if (s->h_out) cudaFreeHost(s->h_out);
-        delete s;
-    }
-    cudaFree(d_lensmap_);
-    cudaFree(d_lut_);
-    cudaFree(d_bg_);
-    cudaFree(d_rgba_);
-    cudaFree(d_tiles_);
-    cudaFree(d_entries_);
-    for (TmapSet *t : tmap_sets_) delete t;
-    for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
-    cudaFree(d_capture_slots_);
-    for (void *p : retired_) cudaFree(p);
 }
 
 size_t WarpDevice::padded_pixels(size_t npix) { return round_up(npix, kPixelsPerBlock); }
+int WarpDevice::width() const { return cur_ ? cur_->width : 0; }
+int WarpDevice::height() const { return cur_ ? cur_->height : 0; }
+size_t WarpDevice::plan_tiles() const { return cur_ && cur_->have_plan ? cur_->ntiles : 0; }
+size_t WarpDevice::plan_entry_bytes() const { return cur_ && cur_->have_plan ? cur_->entry_bytes : 0; }
 
 bool WarpDevice::download_lensmap(uint32_t *out) {
     CK(cudaSetDevice(device_));
-    CK(cudaMemcpy(out, d_lensmap_, npix_ * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (cur_) CK(cudaMemcpy(out, cur_->map.get(), cur_->npix * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return true;
 }
 
 bool WarpDevice::download_plan(void *tiles, void *entries, size_t entry_bytes) {
     CK(cudaSetDevice(device_));
-    if (!have_plan_) return true;
-    if (tiles && ntiles_) CK(cudaMemcpy(tiles, d_tiles_, ntiles_ * sizeof(TileDesc), cudaMemcpyDeviceToHost));
-    if (entries && entry_bytes) CK(cudaMemcpy(entries, d_entries_, entry_bytes, cudaMemcpyDeviceToHost));
+    if (!plan_tiles()) return true;
+    if (tiles) CK(cudaMemcpy(tiles, cur_->tiles.get(), cur_->ntiles * sizeof(TileDesc), cudaMemcpyDeviceToHost));
+    if (entries && entry_bytes) CK(cudaMemcpy(entries, cur_->entries.get(), entry_bytes, cudaMemcpyDeviceToHost));
     return true;
 }
 
-bool WarpDevice::upload_lensmap(const LensmapUpload &lm) {
+bool WarpDevice::install(const LensmapUpload &lm, DevicePlan &&plan) {
     CK(cudaSetDevice(device_));
-    CK(cudaDeviceSynchronize());  // nothing may still be reading the old map
-    const size_t npix = static_cast<size_t>(lm.width) * lm.height;
-    const size_t npad = padded_pixels(npix);
-    // A graph captured since the last upload keeps rendering the lensmap and plan it was captured with: their buffers
-    // are retired instead of freed or rewritten.  The background stays shared while the view size stays the same, so
-    // it is retired when it is replaced and any graph captured since it was allocated reads it.
-    auto drop = [&](auto *&p, bool retire) {
-        if (p && retire) retired_.push_back(p);
-        else cudaFree(p);
-        p = nullptr;
-    };
-    const bool resize = npad != npix_pad_, new_view = resize || lm.width != width_ || lm.height != height_;
-    if (lm.device) {
-        drop(d_lensmap_, captured_);
-        d_lensmap_ = lm.device->d_map;
-    } else if (resize || captured_) {
-        drop(d_lensmap_, captured_);
-        CK(cudaMalloc(&d_lensmap_, npad * sizeof(uint32_t)));
+    CK(cudaDeviceSynchronize());  // nothing may still be reading the buffers freed or rewritten in place below
+    auto g = std::make_shared<Generation>();
+    g->width = lm.width;
+    g->height = lm.height;
+    g->platesize = lm.platesize;
+    g->numplates = lm.numplates;
+    g->npix = static_cast<size_t>(lm.width) * lm.height;
+    g->npix_pad = padded_pixels(g->npix);
+    memcpy(g->display, lm.display, sizeof g->display);
+    memcpy(g->plate_rect, lm.plate_rect, sizeof g->plate_rect);
+    g->span_off.assign(lm.span_off, lm.span_off + lm.height + 1);
+    g->spans.assign(lm.spans, lm.spans + lm.nspans * 2);
+    g->map = std::move(plan.d_map);
+    if (plan.ntiles > 0) {
+        g->tiles = std::move(plan.d_tiles);
+        g->entries = std::move(plan.d_entries);
+        g->ntiles = plan.ntiles;
+        g->entry_bytes = plan.entry_bytes;
+        g->nbox_tiles = static_cast<uint32_t>(plan.plan.n_box);
+        g->ngather_tiles = static_cast<uint32_t>(plan.plan.n_gather);
+        g->stage_bytes = plan.plan.stage_bytes;
+        g->shapes = std::move(plan.plan.shapes);
+        g->plan_has_box = plan.plan.n_box > 0;
+        g->have_plan = true;
     }
-    if (resize || (bg_captured_ && new_view)) {
-        drop(d_bg_, bg_captured_);
-        bg_captured_ = false;
-        CK(cudaMalloc(&d_bg_, npad));
-    }
-    if (new_view) CK(cudaMemset(d_bg_, 0, npad));
-    if (!lm.device) {
-        // padding entries are "unmapped"
-        CK(cudaMemset(d_lensmap_, 0, npad * sizeof(uint32_t)));
-        CK(cudaMemcpy(d_lensmap_, lm.packed, npix * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    }
-    CK(cudaMemcpy(d_lut_, lm.palmaps, 6 * 256, cudaMemcpyHostToDevice));
-    width_ = lm.width;
-    height_ = lm.height;
-    platesize_ = lm.platesize;
-    numplates_ = lm.numplates;
-    npix_ = npix;
-    npix_pad_ = npad;
-    rubix_ = lm.rubix;
-    memcpy(display_, lm.display, sizeof display_);
-    memcpy(plate_rect_, lm.plate_rect, sizeof plate_rect_);
-    span_off_.assign(lm.span_off, lm.span_off + lm.height + 1);
-    spans_.assign(lm.spans, lm.spans + lm.nspans * 2);
-    have_lensmap_ = true;
-    // tiled layout
-    have_plan_ = false;
-    plan_has_box_ = false;
-    drop(d_tiles_, captured_);
-    drop(d_entries_, captured_);
-    captured_ = false;
-    for (TmapSet *t : tmap_sets_) delete t;
-    tmap_sets_.clear();
-    if (lm.device ? lm.device->ntiles > 0 : lm.plan && !lm.plan->tiles.empty()) {
-        const TilePlan &pl = lm.device ? lm.device->plan : *lm.plan;
-        if (lm.device) {
-            d_tiles_ = lm.device->d_tiles;
-            d_entries_ = lm.device->d_entries;
-            ntiles_ = lm.device->ntiles;
-            entry_bytes_ = lm.device->entry_bytes;
+    // The background stays shared, contents and all, while the view size stays the same.  A new view size starts from
+    // zeros: in a new buffer when the padded size changes or a held generation (a captured graph) reads the old one,
+    // otherwise in place.
+    const Generation *old = cur_.get();
+    if (old && old->width == g->width && old->height == g->height) {
+        g->bg = old->bg;
+    } else {
+        bool reuse = old && old->npix_pad == g->npix_pad;
+        for (const auto &h : held_) reuse = reuse && h->bg != old->bg;
+        if (reuse) {
+            g->bg = old->bg;
         } else {
-            CK(cudaMalloc(&d_tiles_, pl.tiles.size() * sizeof(TileDesc)));
-            CK(cudaMemcpy(d_tiles_, pl.tiles.data(), pl.tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
-            CK(cudaMalloc(&d_entries_, pl.entries.size()));
-            CK(cudaMemcpy(d_entries_, pl.entries.data(), pl.entries.size(), cudaMemcpyHostToDevice));
-            ntiles_ = static_cast<uint32_t>(pl.tiles.size());
-            entry_bytes_ = pl.entries.size();
+            g->bg = std::make_shared<DeviceBuffer>();
+            CK(g->bg->alloc(g->npix_pad));
         }
-        nbox_tiles_ = static_cast<uint32_t>(pl.n_box);
-        ngather_tiles_ = static_cast<uint32_t>(pl.n_gather);
-        stage_bytes_ = pl.stage_bytes;
-        shapes_ = pl.shapes;
-        plan_has_box_ = pl.n_box > 0;
-        have_plan_ = true;
+        CK(cudaMemset(g->bg->get(), 0, g->npix_pad));
     }
-    // frame slots depend on the sizes: rebuild lazily
-    for (Slot *s : slots_) {
-        cudaStreamDestroy(s->stream);
-        cudaEventDestroy(s->done);
-        cudaFree(s->d_faces);
-        cudaFree(s->d_out);
-        cudaFreeHost(s->h_faces);
-        cudaFreeHost(s->h_out);
-        delete s;
-    }
-    slots_.clear();
+    if (!set_luts(lm.palmaps)) return false;
+    rubix_ = lm.rubix;
+    cur_ = std::move(g);   // (frees the old generation unless a captured graph holds it)
+    tmap_sets_.clear();
+    slots_.clear();        // frame slots depend on the sizes: rebuilt lazily
+    return true;
+}
+
+bool WarpDevice::set_luts(const uint8_t palmaps[6 * 256]) {
+    CK(cudaSetDevice(device_));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(d_lut_.get(), palmaps, 6 * 256, cudaMemcpyHostToDevice));
     return true;
 }
 
 bool WarpDevice::set_background(const uint8_t *bg_host) {
-    if (!have_lensmap_) {
+    if (!cur_) {
         err_ = "set_background: build a lensmap first (the background has the view's size)";
         return false;
     }
     CK(cudaSetDevice(device_));
     CK(cudaDeviceSynchronize());
-    if (bg_host) CK(cudaMemcpy(d_bg_, bg_host, npix_, cudaMemcpyHostToDevice));
-    else CK(cudaMemset(d_bg_, 0, npix_pad_));
+    if (bg_host) CK(cudaMemcpy(cur_->bg->get(), bg_host, cur_->npix, cudaMemcpyHostToDevice));
+    else CK(cudaMemset(cur_->bg->get(), 0, cur_->npix_pad));
     return true;
 }
 
 bool WarpDevice::set_rgba_table(const uint32_t table[256]) {
     CK(cudaSetDevice(device_));
-    CK(cudaMemcpy(d_rgba_, table, 256 * 4, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_rgba_.get(), table, 256 * 4, cudaMemcpyHostToDevice));
     return true;
 }
 
@@ -1161,7 +1155,7 @@ void WarpDevice::set_face_layout(int rowbytes, const int32_t *origins, int nplat
 bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay) {
     err_code_ = BLINKY_E_INVALID;
     const int n = static_cast<int>(layout_origins_.size() / 2);
-    const uint64_t rb = static_cast<uint64_t>(layout_rowbytes_), ps = static_cast<uint64_t>(platesize_);
+    const uint64_t rb = static_cast<uint64_t>(layout_rowbytes_), ps = static_cast<uint64_t>(cur_->platesize);
     memset(lay, 0, sizeof *lay);
     uint64_t rows = 0;
     for (int pl = 0; pl < n; ++pl) {
@@ -1177,8 +1171,8 @@ bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *
         lay->org_y[pl] = static_cast<int32_t>(y);
     }
     for (int pl = n; pl < kLayoutPlates; ++pl) {
-        const int *r = plate_rect_[pl];
-        if (display_[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
+        const int *r = cur_->plate_rect[pl];
+        if (cur_->display[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
             err_ = "face layout: the lensmap samples plate " + std::to_string(pl) + ", which has no origin (the layout has " + std::to_string(n) + ")";
             return false;
         }
@@ -1200,7 +1194,7 @@ bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *
 
 bool WarpDevice::warp(const WarpRequest &r) {
     err_code_ = BLINKY_E_CUDA;
-    if (!have_lensmap_) {
+    if (!cur_) {
         err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
         return false;
     }
@@ -1216,8 +1210,9 @@ bool WarpDevice::warp(const WarpRequest &r) {
         err_ = "warp (RGBA): the output buffer, the row pitch and the frame stride must be 4-byte aligned";
         return false;
     }
-    const size_t pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(width_) * opx;
-    if (pitch < static_cast<size_t>(width_) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
+    const Generation &g = *cur_;
+    const size_t pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(g.width) * opx;
+    if (pitch < static_cast<size_t>(g.width) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
         return false;
@@ -1226,7 +1221,7 @@ bool WarpDevice::warp(const WarpRequest &r) {
     FaceLayoutParams lay = {};   // (dense: the kernels' last argument, never read)
     if (use_layout && !make_layout(r.face_stride, r.nframes, &lay)) return false;
     const KernelVariant v = {rubix_, r.rgba, r.keep_unmapped, r.rgba && r.tables && r.table_stride != 0, use_layout};
-    const WarpKernel k = choose_kernel(r, pitch, use_layout ? &lay : nullptr, width_, height_, have_plan_, plan_has_box_,
+    const WarpKernel k = choose_kernel(r, pitch, use_layout ? &lay : nullptr, g.width, g.height, g.have_plan, g.plan_has_box,
                                        variant_ == BLINKY_KERNEL_GATHER);
     // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -1237,7 +1232,7 @@ bool WarpDevice::warp(const WarpRequest &r) {
     const bool ok = k == WarpKernel::Ring ? launch_ring(r, static_cast<uint32_t>(pitch), v, lay, capturing)
                                           : launch_flat(r, static_cast<uint32_t>(pitch), v, lay, k);
     if (capturing) {
-        captured_ = bg_captured_ = true;
+        if (held_.empty() || held_.back() != cur_) held_.push_back(cur_);
         bool known = false;
         for (CaptureStream &c : capture_streams_)
             if (c.stream == r.stream) c.id = cap_id, known = true;
@@ -1266,20 +1261,18 @@ bool WarpDevice::release_captures() {
         return fail("release_captures: cudaDeviceSynchronize while a stream is capturing", e);
     }
     if (e != cudaSuccess) return fail("release_captures: cudaDeviceSynchronize", e);
-    for (void *p : retired_) cudaFree(p);
-    retired_.clear();
+    held_.clear();
     capture_streams_.clear();
     capture_slots_used_ = 0;
-    captured_ = bg_captured_ = false;
     return true;
 }
 
 WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stride, int nframes, uint32_t rowbytes, uint32_t rows) {
     const uint64_t tick = ++tmap_tick_;
-    for (TmapSet *t : tmap_sets_)
+    for (const auto &t : tmap_sets_)
         if (t->faces == d_faces && t->face_stride == face_stride && t->nframes == nframes && t->rowbytes == rowbytes && t->rows == rows) {
             t->last_use = tick;
-            return t;
+            return t.get();
         }
     if (!encode_fn_) {
         cudaDriverEntryPointQueryResult qres;
@@ -1293,12 +1286,12 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
     }
     TmapSet *t = nullptr;
     if (tmap_sets_.size() >= 32) {  // host memory only (a launch copies its table into the parameter block): recycle the oldest
-        t = tmap_sets_[0];
-        for (TmapSet *c : tmap_sets_)
-            if (c->last_use < t->last_use) t = c;
+        t = tmap_sets_[0].get();
+        for (const auto &c : tmap_sets_)
+            if (c->last_use < t->last_use) t = c.get();
     } else {
-        t = new TmapSet();
-        tmap_sets_.push_back(t);
+        tmap_sets_.push_back(std::make_unique<TmapSet>());
+        t = tmap_sets_.back().get();
     }
     t->faces = d_faces;
     t->face_stride = face_stride;
@@ -1307,23 +1300,24 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
     t->rows = rows;
     t->last_use = tick;
     memset(&t->table, 0, sizeof t->table);
-    const cuuint64_t ps = static_cast<cuuint64_t>(platesize_);
+    const Generation &g = *cur_;
+    const cuuint64_t ps = static_cast<cuuint64_t>(g.platesize);
     // 4-D view of the globe: (x, y, plate, frame); with a face layout (rowbytes > 0) one frame's surface is the single
     // "plate": (x, y, 1, frame), rowbytes wide and `rows` high
-    const cuuint64_t fw = rowbytes ? rowbytes : ps, fh = rowbytes ? rows : ps, np = rowbytes ? 1 : static_cast<cuuint64_t>(numplates_);
+    const cuuint64_t fw = rowbytes ? rowbytes : ps, fh = rowbytes ? rows : ps, np = rowbytes ? 1 : static_cast<cuuint64_t>(g.numplates);
     const cuuint64_t dims[4] = {fw, fh, np, static_cast<cuuint64_t>(nframes)};
     const cuuint64_t fstride = nframes > 1 ? static_cast<cuuint64_t>(face_stride) : fw * fh * np;
     const cuuint64_t strides[3] = {fw, fw * fh, fstride};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
-    for (size_t si = 0; si < shapes_.size() && si < static_cast<size_t>(kMaxShapes); ++si) {
-        const uint32_t w16 = shapes_[si] >> 8, h8 = shapes_[si] & 0xff;
+    for (size_t si = 0; si < g.shapes.size() && si < static_cast<size_t>(kMaxShapes); ++si) {
+        const uint32_t w16 = g.shapes[si] >> 8, h8 = g.shapes[si] & 0xff;
         const cuuint32_t box[4] = {w16 * 16, h8 * 8, 1, 1};
         CUresult r = reinterpret_cast<EncodeTiledFn>(encode_fn_)(
             &t->table.m[si], CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void *>(d_faces), dims, strides, box, estr,
             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             char buf[160];
-            snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(box %ux%u, ps %d) failed with CUresult %d", w16 * 16, h8 * 8, platesize_, static_cast<int>(r));
+            snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(box %ux%u, ps %d) failed with CUresult %d", w16 * 16, h8 * 8, g.platesize, static_cast<int>(r));
             err_ = buf;
             t->faces = nullptr;
             return nullptr;
@@ -1339,40 +1333,41 @@ constexpr int kRingWarpsDefault = 12;
 
 bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, bool capturing) {
     cudaStream_t st = static_cast<cudaStream_t>(r.stream);
+    const Generation &g = *cur_;
     RingParams p;
-    p.tiles = static_cast<const TileDesc *>(d_tiles_);
-    p.entries = d_entries_;
+    p.tiles = g.tiles.as<const TileDesc>();
+    p.entries = g.entries.as<const uint8_t>();
     static const RingTmaps kNoTmaps = {};
     const RingTmaps *tm = &kNoTmaps;
-    if (plan_has_box_) {
+    if (g.plan_has_box) {
         TmapSet *t = get_tmaps(r.faces, r.face_stride, r.nframes, lay.rowbytes, v.layout ? layout_rows_ : 0u);
         if (!t) return false;
         tm = &t->table;
     }
     p.faces = static_cast<const uint8_t *>(r.faces);
     p.face_stride = r.face_stride;
-    p.bg = d_bg_;
-    p.lut = d_lut_;
-    p.rgba = r.tables ? r.tables : d_rgba_;
+    p.bg = g.bg->as<const uint8_t>();
+    p.lut = d_lut_.as<const uint8_t>();
+    p.rgba = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
     p.table_words = static_cast<uint32_t>(r.table_stride / 4);
     p.out = r.out;
     p.out_stride = r.out_stride;
     p.out_pitch = pitch / (v.rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
-    p.nbox = nbox_tiles_;
-    p.ngather = ngather_tiles_;
-    p.ntiles = ntiles_;
+    p.nbox = g.nbox_tiles;
+    p.ngather = g.ngather_tiles;
+    p.ntiles = g.ntiles;
     p.nframes = static_cast<uint32_t>(r.nframes);
-    p.width = width_;
-    p.height = height_;
+    p.width = g.width;
+    p.height = g.height;
     p.zero = 0;
     // The ring kernel's units are the BOX tiles [0, nbox) and the EMPTY tiles; with keep_unmapped an EMPTY tile has
     // nothing to write, and the units are the BOX tiles alone.  The GATHER tiles in between ride along as gather CTAs
     // or go to K3, launched in front on the same stream (gather_rides_along).
-    const uint32_t nempty = ntiles_ - nbox_tiles_ - ngather_tiles_;
-    const uint32_t ring_tiles = nbox_tiles_ + (v.keep ? 0u : nempty);
+    const uint32_t nempty = g.ntiles - g.nbox_tiles - g.ngather_tiles;
+    const uint32_t ring_tiles = g.nbox_tiles + (v.keep ? 0u : nempty);
     const size_t fixed = kRingBarBytes + (v.rubix ? 6 * 256 : 0) + (v.rgba ? 1024 : 0);
-    const uint32_t max_box = std::max<uint32_t>(static_cast<uint32_t>(stage_bytes_ > 0 ? stage_bytes_ : 128), kBoxBlockBytes);  // largest ring item
-    const bool merged_gather = gather_rides_along(ngather_tiles_, r.nframes, merged_items_max_, serial_gather_);
+    const uint32_t max_box = std::max<uint32_t>(static_cast<uint32_t>(g.stage_bytes > 0 ? g.stage_bytes : 128), kBoxBlockBytes);  // largest ring item
+    const bool merged_gather = gather_rides_along(g.ngather_tiles, r.nframes, merged_items_max_, serial_gather_);
     // as many ring warps per SM as the registers allow (or BLINKY_RING_CTAS), as far as shared memory lets them
     const RingGeometry geo = ring_geometry(smem_per_sm_, ring_ctas_cap_ > 0 ? std::min(ring_ctas_cap_, kRingMinBlocks) : kRingWarpsDefault,
                                            merged_gather, fixed, max_box, ring_bytes_override_);
@@ -1419,7 +1414,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
                    "once the graphs holding them will not run again";
             return false;
         }
-        p.ticket = d_capture_slots_ + capture_slots_used_++;
+        p.ticket = d_capture_slots_.as<uint32_t>() + capture_slots_used_++;
     } else if (grid > 0) {
         TicketCounter *tc = nullptr;
         for (TicketCounter &c : tickets_)
@@ -1427,27 +1422,26 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
         if (!tc) {
             if (tickets_.size() >= 64) {  // streams come and go: start over
                 CK(cudaDeviceSynchronize());
-                for (TicketCounter &c : tickets_) cudaFree(c.d_counter);
                 tickets_.clear();
             }
             TicketCounter c;
             c.stream = r.stream;
-            CK(cudaMalloc(&c.d_counter, sizeof(uint32_t)));
-            CK(cudaMemsetAsync(c.d_counter, 0, sizeof(uint32_t), st));
-            tickets_.push_back(c);
+            CK(c.counter.alloc(sizeof(uint32_t)));
+            CK(cudaMemsetAsync(c.counter.get(), 0, sizeof(uint32_t), st));
+            tickets_.push_back(std::move(c));
             tc = &tickets_.back();
         }
-        p.ticket = tc->d_counter;
+        p.ticket = tc->counter.as<uint32_t>();
     }
     char buf[640];
     int nbuf = 0;
     // GATHER tiles: K3 in front of the ring kernel, unless they ride in its launch (which needs ring units)
-    snprintf(buf, sizeof buf, "%s", ngather_tiles_ == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
-    if (ngather_tiles_ > 0 && (grid == 0 || !merged_gather)) {
-        dim3 g2(ngather_tiles_, static_cast<unsigned>((r.nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
+    snprintf(buf, sizeof buf, "%s", g.ngather_tiles == 0 && grid == 0 ? "no kernel: no tile of the view has a pixel to write" : "");
+    if (g.ngather_tiles > 0 && (grid == 0 || !merged_gather)) {
+        dim3 g2(g.ngather_tiles, static_cast<unsigned>((r.nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
         with_variant(vi, [&](auto vt) {
             using V = decltype(vt);
-            warp_tile_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<g2, kThreads, 0, st>>>(p, nbox_tiles_, lay);
+            warp_tile_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<g2, kThreads, 0, st>>>(p, g.nbox_tiles, lay);
         });
         ++launches_;
         snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", v.rubix, v.rgba, v.tags(), g2.x, g2.y, kThreads);
@@ -1457,7 +1451,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
         p.nstatic = ts.nstatic;
         p.ndraws = ts.ndraws;
         p.ring_grid = grid;
-        const uint32_t extra = merged_gather ? gather_items(ngather_tiles_, r.nframes) : 0u;
+        const uint32_t extra = merged_gather ? gather_items(g.ngather_tiles, r.nframes) : 0u;
         with_variant(vi, [&](auto vt) {
             using V = decltype(vt);
             warp_ring_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid + extra, 32, smem, st>>>(p, *tm, lay);
@@ -1478,23 +1472,24 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
 bool WarpDevice::launch_flat(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, WarpKernel k) {
     // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out unless the caller made its own)
     cudaStream_t st = static_cast<cudaStream_t>(r.stream);
+    const Generation &g = *cur_;
     WarpParams p;
-    p.lensmap4 = reinterpret_cast<const uint4 *>(d_lensmap_);
+    p.lensmap4 = g.map.as<const uint4>();
     p.faces = static_cast<const uint8_t *>(r.faces);
     p.face_stride = r.face_stride;
-    p.bg32 = reinterpret_cast<const uint32_t *>(d_bg_);
-    p.lut = d_lut_;
-    p.rgba = r.tables ? r.tables : d_rgba_;
+    p.bg32 = g.bg->as<const uint32_t>();
+    p.lut = d_lut_.as<const uint8_t>();
+    p.rgba = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
     p.table_words = static_cast<uint32_t>(r.table_stride / 4);
     p.out = r.out;
     p.out_stride = r.out_stride;
-    p.nquads = static_cast<uint32_t>((npix_ + 3) / 4);
-    p.npix = static_cast<uint32_t>(npix_);
-    p.width = static_cast<uint32_t>(width_);
+    p.nquads = static_cast<uint32_t>((g.npix + 3) / 4);
+    p.npix = static_cast<uint32_t>(g.npix);
+    p.width = static_cast<uint32_t>(g.width);
     p.out_pitch = pitch;
-    p.pitched = pitch != static_cast<size_t>(width_) * (v.rgba ? 4 : 1);
+    p.pitched = pitch != static_cast<size_t>(g.width) * (v.rgba ? 4 : 1);
     const bool vector = k == WarpKernel::Vector;
-    const dim3 grid(static_cast<unsigned>(vector ? npix_pad_ / kPixelsPerBlock : (npix_ + kThreads - 1) / kThreads), static_cast<unsigned>(r.nframes));
+    const dim3 grid(static_cast<unsigned>(vector ? g.npix_pad / kPixelsPerBlock : (g.npix + kThreads - 1) / kThreads), static_cast<unsigned>(r.nframes));
     with_variant(v.index(), [&](auto vt) {
         using V = decltype(vt);
         if (vector) warp_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, lay);
@@ -1513,16 +1508,16 @@ bool WarpDevice::ensure_slots() {
     if (!slots_.empty()) return true;
     // three frames in flight overlap upload, warp and copy back; 2-8 measured the same
     constexpr int kSlots = 3;
-    slot_face_bytes_ = static_cast<size_t>(numplates_) * platesize_ * platesize_;
-    slot_out_bytes_ = round_up(npix_, 16);
+    slot_face_bytes_ = static_cast<size_t>(cur_->numplates) * cur_->platesize * cur_->platesize;
+    slot_out_bytes_ = round_up(cur_->npix, 16);
     for (int i = 0; i < kSlots; ++i) {
-        Slot *s = new Slot();
-        slots_.push_back(s);
+        slots_.push_back(std::make_unique<Slot>());
+        Slot *s = slots_.back().get();
         CK(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
-        CK(cudaMalloc(&s->d_faces, slot_face_bytes_));
-        CK(cudaMemset(s->d_faces, 0, slot_face_bytes_));
-        CK(cudaMalloc(&s->d_out, slot_out_bytes_));
+        CK(s->d_faces.alloc(slot_face_bytes_));
+        CK(cudaMemset(s->d_faces.get(), 0, slot_face_bytes_));
+        CK(s->d_out.alloc(slot_out_bytes_));
         // (pinned staging for callers whose buffers are not pinned: allocated when first needed)
     }
     return true;
@@ -1533,15 +1528,16 @@ void WarpDevice::finalize_slot(Slot &s) {
     cudaEventSynchronize(s.done);
     s.busy = false;
     if (s.direct) return;  // the copy engine already wrote the caller's buffer
-    const int W = width_, H = height_;
+    const Generation &g = *cur_;
+    const int W = g.width, H = g.height;
     uint8_t *dst = s.dst + static_cast<size_t>(s.y0) * s.dst_rowbytes + s.x0;
     if (s.keep_unmapped) {
         // only mapped pixels are written, like `if (*lmap)` in render_lensmap (:2413)
         for (int y = 0; y < H; ++y) {
             const uint8_t *src = s.h_out + static_cast<size_t>(y) * W;
             uint8_t *row = dst + static_cast<size_t>(y) * s.dst_rowbytes;
-            for (int32_t j = span_off_[static_cast<size_t>(y)]; j < span_off_[static_cast<size_t>(y) + 1]; ++j) {
-                const int32_t a = spans_[static_cast<size_t>(j) * 2], b = spans_[static_cast<size_t>(j) * 2 + 1];
+            for (int32_t j = g.span_off[static_cast<size_t>(y)]; j < g.span_off[static_cast<size_t>(y) + 1]; ++j) {
+                const int32_t a = g.spans[static_cast<size_t>(j) * 2], b = g.spans[static_cast<size_t>(j) * 2 + 1];
                 memcpy(row + a, src + a, static_cast<size_t>(b - a));
             }
         }
@@ -1565,23 +1561,25 @@ static bool is_pinned(const void *p) {
 bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
                            int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped) {
     err_code_ = BLINKY_E_CUDA;
-    if (!have_lensmap_) {
+    if (!cur_) {
         err_ = "warp_host: no lensmap on the device (call blinky_build_lensmap)";
         return false;
     }
+    const Generation &g = *cur_;
     // with a face layout the plates' rectangles are read out of each frame's surface; the device copy stays dense
     FaceLayoutParams lay;
     const bool layout = layout_rowbytes_ > 0;
     if (layout && !make_layout(face_stride, nframes, &lay)) return false;
-    const size_t src_pitch = layout ? lay.rowbytes : static_cast<size_t>(platesize_);
+    const size_t ps = static_cast<size_t>(g.platesize);
+    const size_t src_pitch = layout ? lay.rowbytes : ps;
     CK(cudaSetDevice(device_));
     if (!ensure_slots()) return false;
-    const size_t ps2 = static_cast<size_t>(platesize_) * platesize_;
+    const size_t ps2 = ps * ps;
     // (one driver query per distinct buffer, not two per call)
     if (faces_host != pin_src_ptr_) pin_src_ptr_ = faces_host, pin_src_ = is_pinned(faces_host);
     if (dst_host != pin_dst_ptr_) pin_dst_ptr_ = dst_host, pin_dst_ = is_pinned(dst_host);
     const bool src_pinned = pin_src_, dst_pinned = pin_dst_;
-    const int W = width_, H = height_;
+    const int W = g.width, H = g.height;
     const bool direct = dst_pinned && !keep_unmapped;  // the copy engine writes the caller's buffer, no staging
     const size_t frame = static_cast<size_t>(W) * H;
     bool ok = true;
@@ -1597,23 +1595,23 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         const uint8_t *src = faces_host + static_cast<size_t>(f) * face_stride;
         cudaMemcpy3DBatchOp ops[BLINKY_MAX_PLATES];
         size_t nops = 0;
-        for (int pl = 0; pl < numplates_; ++pl) {
-            if (!display_[pl]) continue;
-            const int *r = plate_rect_[pl];
+        for (int pl = 0; pl < g.numplates; ++pl) {
+            if (!g.display[pl]) continue;
+            const int *r = g.plate_rect[pl];
             if (r[0] > r[2] || r[1] > r[3]) continue;
             const size_t rw = static_cast<size_t>(r[2] - r[0] + 1), rh = static_cast<size_t>(r[3] - r[1] + 1);
-            const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * platesize_ + r[0];   // in the dense device copy
+            const size_t off = pl * ps2 + static_cast<size_t>(r[1]) * ps + r[0];   // in the dense device copy
             const uint8_t *from = src + (layout ? lay.plate_base[pl] + static_cast<size_t>(r[1]) * src_pitch + r[0] : off);
             size_t pitch = src_pitch;
             if (!src_pinned) {
                 uint8_t *stage = s.h_faces + off;
-                for (size_t y = 0; y < rh; ++y) memcpy(stage + y * platesize_, from + y * src_pitch, rw);
+                for (size_t y = 0; y < rh; ++y) memcpy(stage + y * ps, from + y * src_pitch, rw);
                 from = stage;
-                pitch = static_cast<size_t>(platesize_);
+                pitch = ps;
             }
             // a full-width rectangle of dense rows is one contiguous run: copy it as such
-            const bool contiguous = rw == static_cast<size_t>(platesize_) && pitch == rw;
-            const size_t row = contiguous ? rw * rh : static_cast<size_t>(platesize_), rows = contiguous ? 1 : rh;
+            const bool contiguous = rw == ps && pitch == rw;
+            const size_t row = contiguous ? rw * rh : ps, rows = contiguous ? 1 : rh;
             cudaMemcpy3DBatchOp &op = ops[nops++];
             memset(&op, 0, sizeof op);
             op.src.type = cudaMemcpyOperandTypePointer;
@@ -1621,7 +1619,7 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
             op.src.op.ptr.rowLength = contiguous ? row : pitch;
             op.src.op.ptr.layerHeight = rows;
             op.dst.type = cudaMemcpyOperandTypePointer;
-            op.dst.op.ptr.ptr = s.d_faces + off;
+            op.dst.op.ptr.ptr = s.d_faces.as<uint8_t>() + off;
             op.dst.op.ptr.rowLength = row;
             op.dst.op.ptr.layerHeight = rows;
             op.extent = make_cudaExtent(contiguous ? rw * rh : rw, rows, 1);
@@ -1640,7 +1638,7 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         }
         if (!ok) break;
         s.dst = dst_host + static_cast<size_t>(f) * dst_frame_stride;
-        WarpRequest r(s.d_faces, slot_face_bytes_, s.d_out, slot_out_bytes_, 1, s.stream);
+        WarpRequest r(s.d_faces.get(), slot_face_bytes_, s.d_out.get(), slot_out_bytes_, 1, s.stream);
         r.dense_faces = true;   // the device copy is dense whatever the face layout
         if (!warp(r)) { ok = false; break; }
         s.dst_rowbytes = dst_rowbytes;
@@ -1649,9 +1647,9 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
         s.keep_unmapped = keep_unmapped;
         s.direct = direct;
         uint8_t *to = s.dst + static_cast<size_t>(y0) * dst_rowbytes + x0;
-        cudaError_t e = !direct              ? cudaMemcpyAsync(s.h_out, s.d_out, frame, cudaMemcpyDeviceToHost, s.stream)
-                        : dst_rowbytes == W ? cudaMemcpyAsync(to, s.d_out, frame, cudaMemcpyDeviceToHost, s.stream)
-                                            : cudaMemcpy2DAsync(to, static_cast<size_t>(dst_rowbytes), s.d_out, static_cast<size_t>(W),
+        cudaError_t e = !direct              ? cudaMemcpyAsync(s.h_out, s.d_out.get(), frame, cudaMemcpyDeviceToHost, s.stream)
+                        : dst_rowbytes == W ? cudaMemcpyAsync(to, s.d_out.get(), frame, cudaMemcpyDeviceToHost, s.stream)
+                                            : cudaMemcpy2DAsync(to, static_cast<size_t>(dst_rowbytes), s.d_out.get(), static_cast<size_t>(W),
                                                                 static_cast<size_t>(W), static_cast<size_t>(H), cudaMemcpyDeviceToHost, s.stream);
         if (e != cudaSuccess) { ok = fail("cudaMemcpyAsync(D2H frame)", e); break; }
         e = cudaEventRecord(s.done, s.stream);

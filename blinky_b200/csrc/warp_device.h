@@ -8,24 +8,22 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 #include <string>
 #include <vector>
 
+#include "device_buffer.h"
 #include "face_layout.h"
 
 namespace blinky {
 
-struct TilePlan;       // tile_plan.h
 struct DevicePlan;     // tile_plan_device.h
 struct KernelVariant;  // launch_plan.h
 enum class WarpKernel;
 
+// What WarpDevice::install keeps of a lensmap beside its device buffers (DevicePlan).
 struct LensmapUpload {
     int width = 0, height = 0, platesize = 0, numplates = 0;
-    const uint32_t *packed = nullptr;        // [height*width]
-    // instead of packed and plan: a map and tile plan already in device memory (plan_lensmap_device), whose
-    // buffers the device takes over as its new generation
-    const DevicePlan *device = nullptr;
     const uint8_t *palmaps = nullptr;        // [6*256]
     int display[6] = {0, 0, 0, 0, 0, 0};
     int plate_rect[6][4] = {};               // texel rectangle each plate is sampled in (x0,y0,x1,y1)
@@ -33,7 +31,6 @@ struct LensmapUpload {
     const int32_t *span_off = nullptr;       // [height+1]
     const int32_t *spans = nullptr;          // pairs
     size_t nspans = 0;
-    const TilePlan *plan = nullptr;          // tiled layout (may be null: flat kernels only)
 };
 
 // One device-resident batch (WarpDevice::warp), asynchronous on `stream` (nullptr = CUDA's default stream).  May be
@@ -67,7 +64,11 @@ public:
     int device() const { return device_; }
     const std::string &last_error() const { return err_; }
 
-    bool upload_lensmap(const LensmapUpload &lm);
+    // Makes lm, with plan's map and tile plan (whose buffers it takes over), the resident lensmap, and copies
+    // lm.palmaps into the LUTs.  All or nothing: on failure the current lensmap stays resident.
+    bool install(const LensmapUpload &lm, DevicePlan &&plan);
+    // the plates' palette LUTs, rewritten in place (graphs captured earlier read them too)
+    bool set_luts(const uint8_t palmaps[6 * 256]);
     void set_rubix(bool on) { rubix_ = on; }
     bool set_background(const uint8_t *bg_host);   // [H][W] or nullptr -> zeros
     bool set_rgba_table(const uint32_t table[256]);
@@ -76,20 +77,20 @@ public:
     // origins: nplates (x, y) pairs.  Checked against the lensmap at each warp (BLINKY_E_INVALID when it does not fit).
     void set_face_layout(int rowbytes, const int32_t *origins, int nplates);
 
-    // size of the resident lensmap's view (0 before the first upload)
-    int width() const { return width_; }
-    int height() const { return height_; }
+    // size of the resident lensmap's view (0 before the first install)
+    int width() const;
+    int height() const;
     // entries of a device lensmap buffer for npix pixels (the kernels read whole blocks; the padding is unmapped)
     static size_t padded_pixels(size_t npix);
     // copies of the resident map ([height][width] entries) and tile plan, synchronously
     bool download_lensmap(uint32_t *out);
     bool download_plan(void *tiles, void *entries, size_t entry_bytes);
-    size_t plan_tiles() const { return have_plan_ ? ntiles_ : 0; }
-    size_t plan_entry_bytes() const { return have_plan_ ? entry_bytes_ : 0; }
+    size_t plan_tiles() const;
+    size_t plan_entry_bytes() const;
 
     bool warp(const WarpRequest &r);
-    // The caller will not run again any graph that captured a warp of this object: synchronises the device, frees
-    // the buffers upload_lensmap retired for such graphs and returns every capture counter slot to the pool.
+    // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go
+    // of the generations held for such graphs and returns every capture counter slot to the pool.
     bool release_captures();
     // BLINKY_E_* code of the last failure (BLINKY_E_CUDA unless the call was refused for another reason)
     int last_error_code() const { return err_code_; }
@@ -110,6 +111,7 @@ public:
     const std::string &last_kernel() const { return last_kernel_; }
 
 private:
+    struct Generation;
     struct Slot;
     bool ensure_slots();
     bool fail(const char *what, int cuda_err);
@@ -124,18 +126,12 @@ private:
     std::string err_;
     int err_code_ = 0;
 
-    // resident lensmap
-    int width_ = 0, height_ = 0, platesize_ = 0, numplates_ = 0;
-    size_t npix_ = 0, npix_pad_ = 0;
-    int display_[6] = {0, 0, 0, 0, 0, 0};
-    int plate_rect_[6][4] = {};
+    // the resident lensmap, its plan and background (null before the first install); warp() reads it through this
+    // one pointer
+    std::shared_ptr<const Generation> cur_;
     bool rubix_ = false;
-    bool have_lensmap_ = false;
-    uint32_t *d_lensmap_ = nullptr;
-    uint8_t *d_lut_ = nullptr;
-    uint8_t *d_bg_ = nullptr;
-    uint32_t *d_rgba_ = nullptr;
-    std::vector<int32_t> span_off_, spans_;
+    DeviceBuffer d_lut_;    // uint8_t[6][256]
+    DeviceBuffer d_rgba_;   // uint32_t[256]
     int variant_ = 0;
     int layout_rowbytes_ = 0;              // face layout: 0 = dense
     std::vector<int32_t> layout_origins_;  // (x, y) per plate
@@ -145,23 +141,15 @@ private:
     struct TmapSet;
     struct TicketCounter {
         void *stream = nullptr;
-        uint32_t *d_counter = nullptr;  // 0 between launches: each launch sets it back
+        DeviceBuffer counter;  // uint32_t, 0 between launches: each launch sets it back
     };
-    bool have_plan_ = false;
-    bool plan_has_box_ = false;
-    void *d_tiles_ = nullptr;       // TileDesc[]
-    uint8_t *d_entries_ = nullptr;
-    size_t entry_bytes_ = 0;
-    uint32_t ntiles_ = 0, nbox_tiles_ = 0, ngather_tiles_ = 0;
-    int stage_bytes_ = 0;                // largest staged box of the plan
     int static_pct_ = 85;                // share of the ring kernel's units scheduled statically (BLINKY_STATIC_PCT)
     bool serial_gather_ = false;         // BLINKY_SERIAL_GATHER=1: GATHER tiles in their own kernel instead of as extra CTAs of the ring kernel's launch
     int ring_bytes_override_ = 0, ring_ctas_cap_ = 0, fchunk_ = 0;  // tuning overrides (BLINKY_RING_BYTES / _CTAS, BLINKY_FCHUNK); 0 = automatic
     int merged_items_max_ = 4096;        // gather items up to which GATHER tiles ride in the ring kernel's launch of <= 8 frames (BLINKY_MERGED_ITEMS)
     int ring_boxes_ = 0;                 // boxes a warp keeps in flight at most (BLINKY_RING_BOXES)
     size_t smem_per_sm_ = 233472;
-    std::vector<uint16_t> shapes_;
-    std::vector<TmapSet *> tmap_sets_;   // small cache keyed by (faces ptr, stride, nframes, face layout's surface)
+    std::vector<std::unique_ptr<TmapSet>> tmap_sets_;   // small cache keyed by (faces ptr, stride, nframes, face layout's surface)
     uint64_t tmap_tick_ = 0;
     std::vector<TicketCounter> tickets_; // one work counter per stream the ring kernel was launched on (eagerly)
     void *encode_fn_ = nullptr;          // cuTensorMapEncodeTiled
@@ -175,21 +163,19 @@ private:
 
     // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
     // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are
-    // handed out in order and come back all at once (release_captures).  Buffers a captured launch reads are not
-    // freed by the next upload_lensmap but retired, until release_captures.
+    // handed out in order and come back all at once (release_captures).  The generations captured launches read stay
+    // held, past the install that replaces them, until release_captures.
     struct CaptureStream {
         void *stream;
         unsigned long long id;  // capture sequence a warp was captured into
     };
-    uint32_t *d_capture_slots_ = nullptr;
+    DeviceBuffer d_capture_slots_;        // uint32_t[kCaptureSlots]
     uint32_t capture_slots_used_ = 0;
-    bool captured_ = false;               // a launch was captured since the last upload_lensmap
-    bool bg_captured_ = false;            // a launch was captured since d_bg_ was allocated
-    std::vector<void *> retired_;         // device buffers that captured graphs may still read
+    std::vector<std::shared_ptr<const Generation>> held_;  // generations captured graphs may read
     std::vector<CaptureStream> capture_streams_;  // where warps were captured (release_captures refuses while one is open)
 
     // e2e pipeline
-    std::vector<Slot *> slots_;
+    std::vector<std::unique_ptr<Slot>> slots_;
     size_t slot_face_bytes_ = 0, slot_out_bytes_ = 0;
 
     int64_t launches_ = 0;
