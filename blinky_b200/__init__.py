@@ -61,6 +61,8 @@ _SIGNATURES = [
     ("blinky_needs_rebuild", c_int, [_CTX, c_int, c_int, c_int]),
     ("blinky_set_lensmap", c_int, [_CTX, c_int, c_int, c_int, c_int, c_void_p]),
     ("blinky_set_lensmap_device", c_int, [_CTX, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    ("blinky_set_raymap", c_int, [_CTX, c_int, c_int, c_int, c_void_p]),
+    ("blinky_set_raymap_device", c_int, [_CTX, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_build_info", c_char_p, [_CTX]),
     ("blinky_plan_digest", ctypes.c_uint64, [_CTX, c_int]),
     ("blinky_get_tile_plan", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
@@ -284,6 +286,23 @@ class Fisheye:
         self._check(self._lib.blinky_set_lensmap_device(self._ctx, packed.shape[1], packed.shape[0], platesize, numplates,
                                                         packed.data_ptr(), stream))
 
+    def set_raymap(self, rays, platesize: int = 0, stream: int | None = None):
+        """Maps a view ray per screen pixel through the current globe and installs the result as the lensmap.  rays:
+        [H, W, 3] float32, lens_inverse's result narrowed to float and not normalised (the zero vector for an empty
+        pixel) — a numpy array (blinky_set_raymap) or a contiguous CUDA tensor (blinky_set_raymap_device, read on
+        `stream` after the work already there, mapped and planned on the GPU)."""
+        if isinstance(rays, np.ndarray):
+            r = np.ascontiguousarray(rays)
+            if r.ndim != 3 or r.shape[2] != 3 or r.dtype != np.float32:
+                raise ValueError(f"set_raymap: expected a [H, W, 3] float32 array, got {r.dtype} {r.shape}")
+            self._check(self._lib.blinky_set_raymap(self._ctx, r.shape[1], r.shape[0], platesize, r.ctypes.data))
+            return
+        if not (hasattr(rays, "is_cuda") and rays.is_cuda):
+            raise TypeError("set_raymap: expected a numpy array or a CUDA tensor")
+        if rays.dim() != 3 or rays.shape[2] != 3 or str(rays.dtype) != "torch.float32" or not rays.is_contiguous():
+            raise ValueError(f"set_raymap: expected a contiguous [H, W, 3] float32 tensor, got {rays.dtype} {tuple(rays.shape)}")
+        self._check(self._lib.blinky_set_raymap_device(self._ctx, rays.shape[1], rays.shape[0], platesize, rays.data_ptr(), stream))
+
     @property
     def build_info(self) -> str:
         """How the last lensmap was built ("device: ..." or "host ...")."""
@@ -395,11 +414,13 @@ class Fisheye:
         st = self._lib.blinky_globe_plate(self._ctx, x, y, z, ctypes.byref(plate))
         return st, plate.value
 
-    def lens_source(self, cuda: bool = False, forward: bool = False, with_kernel: bool = False, globe_plate: bool = False) -> str:
+    def lens_source(self, cuda: bool = False, forward: bool = False, with_kernel: bool = False, globe_plate: bool = False,
+                    raymap: bool = False) -> str:
         """The current ``lens_inverse`` (or ``lens_forward``) translated to C++/CUDA (raises when not translatable);
         ``with_kernel`` appends the fixed kernel the device builder launches and translates the globe's
-        ``globe_plate`` into the same unit when there is one.  ``globe_plate``: that function translated alone."""
-        flavour = int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0) | (8 if globe_plate else 0)
+        ``globe_plate`` into the same unit when there is one.  ``globe_plate``: that function translated alone.
+        ``raymap``: the unit of the ray-map kernel (set_raymap on a CUDA tensor), globe_plate and kernel."""
+        flavour = int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0) | (8 if globe_plate else 0) | (16 if raymap else 0)
         n = self._lib.blinky_lens_source(self._ctx, flavour, None, 0)
         if n < 0:
             self._check(n)

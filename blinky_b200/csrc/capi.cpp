@@ -268,6 +268,49 @@ int blinky_set_lensmap(blinky_ctx *ctx, int width, int height, int platesize, in
     return uploaded ? BLINKY_OK : BLINKY_E_CUDA;
 }
 
+}  // extern "C"
+
+namespace {
+
+// blinky_set_raymap and the host path of blinky_set_raymap_device: sizes checked, rays in host memory
+int set_raymap_host(blinky_ctx *ctx, const char *who, int width, int height, int platesize, const float *rays, const std::string &path) {
+    auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point t) {
+        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+    };
+    if (ctx->host.set_raymap(width, height, platesize, rays) != 0)
+        return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": globe_plate failed: " + ctx->host.log());
+    char t[96];
+    snprintf(t, sizeof t, "; map %.1f ms", ms_since(t0));
+    ctx->build_info = "ray map, " + path + t;
+    t0 = std::chrono::steady_clock::now();
+    const bool uploaded = upload(ctx);
+    if (ctx->dev) {
+        snprintf(t, sizeof t, ", plan+upload %.1f ms", ms_since(t0));
+        ctx->build_info += t;
+    }
+    return uploaded ? BLINKY_OK : BLINKY_E_CUDA;
+}
+
+// the checks both ray-map entry points make before anything changes
+int check_raymap(blinky_ctx *ctx, const char *who, int width, int height, int *platesize, const float *rays) {
+    if (!rays || reinterpret_cast<uintptr_t>(rays) % 4 != 0) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": rays must be a non-NULL, 4-byte aligned pointer");
+    std::string why;
+    const int rc = ctx->host.check_raymap(width, height, platesize, &why);
+    if (rc != 0) return set_err(ctx, rc == -7 ? BLINKY_E_STATE : BLINKY_E_INVALID, std::string(who) + ": " + why);
+    return BLINKY_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int blinky_set_raymap(blinky_ctx *ctx, int width, int height, int platesize, const float *rays) {
+    const char *who = "blinky_set_raymap";
+    const int rc = check_raymap(ctx, who, width, height, &platesize, rays);
+    return rc != BLINKY_OK ? rc : set_raymap_host(ctx, who, width, height, platesize, rays, "host");
+}
+
 const char *blinky_build_info(blinky_ctx *ctx) { return ctx->build_info.c_str(); }
 
 int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes) {
@@ -363,7 +406,10 @@ int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate
 
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize) {
     std::string s, why;
-    if (flavour & 8) {
+    if (flavour & 16) {
+        if (!ctx->host.raymap_device_source((flavour & 1) != 0, &s, &why)) return set_err(ctx, BLINKY_E_SCRIPT, why);
+        s += LensDevice::raymap_tail(blinky::source_has_globe_plate(s));
+    } else if (flavour & 8) {
         if (!ctx->host.globe_plate_device_source((flavour & 1) != 0, &s, &why)) return set_err(ctx, BLINKY_E_SCRIPT, why);
     } else {
         // with the kernel: the unit NVRTC compiles, i.e. with the globe's globe_plate when it has one
@@ -454,6 +500,42 @@ int blinky_set_lensmap_device(blinky_ctx *ctx, int width, int height, int plates
     char t[128];
     snprintf(t, sizeof t, "supplied (device memory); plan %.3f ms, adopt %.3f ms", ms_plan,
              std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+    ctx->build_info = t;
+    return BLINKY_OK;
+}
+
+int blinky_set_raymap_device(blinky_ctx *ctx, int width, int height, int platesize, const float *d_rays, void *stream) {
+    NEED_DEVICE(ctx);
+    const char *who = "blinky_set_raymap_device";
+    int rc = check_raymap(ctx, who, width, height, &platesize, d_rays);
+    if (rc != BLINKY_OK) return rc;
+    auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point t) {
+        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+    };
+    const size_t npix = static_cast<size_t>(width) * height;
+    std::string why;
+    uint32_t *d_map = nullptr;
+    size_t settled = 0;
+    rc = ctx->host.raymap_device(width, height, platesize, d_rays, stream, &d_map, &settled, &why);
+    if (rc == -2) return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": globe_plate failed: " + ctx->host.log());
+    if (rc == 1) {
+        std::vector<float> rays(3 * npix);
+        if (!ctx->lens_dev->copy_to_host(rays.data(), d_rays, rays.size() * sizeof(float), stream, &ctx->err)) return BLINKY_E_CUDA;
+        return set_raymap_host(ctx, who, width, height, platesize, rays.data(), "host (" + why + ")");
+    }
+    const double ms_map = ms_since(t0);
+    t0 = std::chrono::steady_clock::now();
+    // entries on the stale slots of a globe_plate may index any of the six plates, as in a build's map
+    blinky::DevicePlan dp;
+    rc = blinky::plan_lensmap_device(ctx->dev->device(), d_map, width, height, platesize, BLINKY_MAX_PLATES, WarpDevice::padded_pixels(npix), stream,
+                                     &dp, &why);
+    if (rc != BLINKY_OK) return set_err(ctx, rc, why);
+    ctx->host.adopt_lensmap(width, height, platesize, ctx->host.numplates(), dp.display, dp.rect, dp.mapped, std::move(dp.span_off), std::move(dp.spans));
+    if (!upload(ctx, &dp)) return BLINKY_E_CUDA;
+    char t[256];
+    snprintf(t, sizeof t, "ray map, device: %zu of %zu pixels settled by the interpreter; map %.3f ms (NVRTC %.0f ms, kernel %.3f ms), plan+adopt %.3f ms",
+             settled, npix, ms_map, ctx->lens_dev->last_compile_ms(), ctx->lens_dev->last_kernel_ms(), ms_since(t0));
     ctx->build_info = t;
     return BLINKY_OK;
 }

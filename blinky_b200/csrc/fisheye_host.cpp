@@ -1021,32 +1021,51 @@ bool FisheyeHost::ray_to_plate_uv(int plate, const float ray[3], double *u, doub
     return *u >= 0 && *u <= 1 && *v >= 0 && *v <= 1;
 }
 
+// rubix grid (:1922-1960): texel (px, py) of a ps x ps plate lies in the padding between the cells
+bool FisheyeHost::on_rubix_grid(int px, int py, int ps) const {
+    double block = rubix_pad_ + rubix_cell_;
+    double units = rubix_numcells_ * block + rubix_pad_;
+    double unit_px = static_cast<double>(ps) / units;
+    double ux = static_cast<double>(px) / unit_px;
+    double uy = static_cast<double>(py) / unit_px;
+    return std::fmod(ux, block) < rubix_pad_ || std::fmod(uy, block) < rubix_pad_;
+}
+
 void FisheyeHost::set_from_plate(int lx, int ly, int px, int py, int plate, int *display) {
     if (lx < 0 || lx >= width_px_ || ly < 0 || ly >= height_px_) return;
     if (px < 0 || px >= platesize_ || py < 0 || py >= platesize_) return;
     display[plate] = 1;
     size_t at = static_cast<size_t>(lx) + static_cast<size_t>(ly) * width_px_;
     idx_[at] = plate * platesize_ * platesize_ + px + py * platesize_;
-    // rubix grid (:1922-1960): cells get the plate's tint, the padding between
-    // them keeps whatever tint the pixel already had
-    double block = rubix_pad_ + rubix_cell_;
-    double units = rubix_numcells_ * block + rubix_pad_;
-    double unit_px = static_cast<double>(platesize_) / units;
-    double ux = static_cast<double>(px) / unit_px;
-    double uy = static_cast<double>(py) / unit_px;
-    bool ongrid = std::fmod(ux, block) < rubix_pad_ || std::fmod(uy, block) < rubix_pad_;
-    if (!ongrid) tint_[at] = static_cast<uint8_t>(plate);
+    // cells get the plate's tint, the padding between them keeps whatever tint the pixel already had
+    if (!on_rubix_grid(px, py, platesize_)) tint_[at] = static_cast<uint8_t>(plate);
+}
+
+// the plate and texel set_from_ray picks for a normalised ray on plates of ps x ps texels (px, py not yet range-checked);
+// false: the ray maps to nothing
+bool FisheyeHost::ray_to_texel(Worker &w, const float ray[3], int ps, int *plate, int *px, int *py) {
+    *plate = ray_to_plate_index(w, ray);
+    if (*plate < 0) return false;
+    if (*plate >= kMaxPlates) return false;  // reference would index plates[] out of range
+    double u, v;
+    if (!ray_to_plate_uv(*plate, ray, &u, &v)) return false;
+    *px = static_cast<int>(u * ps);
+    *py = static_cast<int>(v * ps);
+    return true;
 }
 
 void FisheyeHost::set_from_ray(Worker &w, int lx, int ly, const float ray[3], int *display) {
-    int plate = ray_to_plate_index(w, ray);
-    if (plate < 0) return;
-    if (plate >= kMaxPlates) return;  // reference would index plates[] out of range
-    double u, v;
-    if (!ray_to_plate_uv(plate, ray, &u, &v)) return;
-    int px = static_cast<int>(u * platesize_);
-    int py = static_cast<int>(v * platesize_);
-    set_from_plate(lx, ly, px, py, plate, display);
+    int plate, px, py;
+    if (ray_to_texel(w, ray, platesize_, &plate, &px, &py)) set_from_plate(lx, ly, px, py, plate, display);
+}
+
+// set_from_ray's result as a packed entry, for a pixel no earlier write tinted (ray maps are made in one pass)
+uint32_t FisheyeHost::ray_entry(Worker &w, const float ray[3], int ps, int *display) {
+    int plate, px, py;
+    if (!ray_to_texel(w, ray, ps, &plate, &px, &py) || px < 0 || px >= ps || py < 0 || py >= ps) return 7u << 28;
+    display[plate] = 1;
+    const uint32_t tint = on_rubix_grid(px, py, ps) ? 7u : static_cast<uint32_t>(plate);
+    return 0x80000000u | tint << 28 | static_cast<uint32_t>(plate * ps * ps + px + py * ps);
 }
 
 // ---------------------------------------------------------------------------
@@ -1150,19 +1169,19 @@ int FisheyeHost::run_inverse_workers(int threads, int nitems, int *display, F it
     return rc;
 }
 
-LensBuildParams FisheyeHost::device_params() const {
+LensBuildParams FisheyeHost::device_params(int width, int height, int platesize) const {
     LensBuildParams p;
     memset(&p, 0, sizeof p);
-    p.width = width_px_;
-    p.height = height_px_;
-    p.platesize = platesize_;
+    p.width = width;
+    p.height = height;
+    p.platesize = platesize;
     p.numplates = numplates_;
     p.scale = scale_;
     // rubix grid geometry exactly as set_from_plate derives it
     p.rubix_block = rubix_pad_ + rubix_cell_;
     p.rubix_pad = rubix_pad_;
     const double units = rubix_numcells_ * p.rubix_block + rubix_pad_;
-    p.rubix_unit_px = static_cast<double>(platesize_) / units;
+    p.rubix_unit_px = static_cast<double>(platesize) / units;
     // all six: a globe_plate script may pick a plate >= numplates, and then the host (like the reference,
     // whose globe.plates is static) uses what an earlier globe left in that slot (0.5 / tan(0) = inf if none)
     for (int i = 0; i < kMaxPlates; ++i) {
@@ -1181,7 +1200,7 @@ LensBuildParams FisheyeHost::device_params() const {
 int FisheyeHost::build_inverse_device(int *display, std::string *why) {
     std::string src;
     if (!lens_device_source(true, &src, why, false, true)) return 1;
-    const LensBuildParams p = device_params();
+    const LensBuildParams p = device_params(width_px_, height_px_, platesize_);
     const size_t area = idx_.size();
     std::vector<uint32_t> cand(area);
     if (!device_builder_->build(src, p, cand.data(), why)) return 1;
@@ -1328,7 +1347,7 @@ void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const i
 int FisheyeHost::build_forward_device(std::string *why) {
     std::string src;
     if (!lens_device_source(true, &src, why, true, true)) return 1;
-    const LensBuildParams p = device_params();
+    const LensBuildParams p = device_params(width_px_, height_px_, platesize_);
     std::vector<uint32_t> undecided, undecided_texels;
     if (!device_builder_->forward_points(src, p, &undecided, &undecided_texels, why)) return 1;
     std::vector<ForwardPatch> patches(undecided.size());
@@ -1733,6 +1752,102 @@ void FisheyeHost::unpack_map(const uint32_t *packed) {
         }
     });
     map_on_host_ = true;
+}
+
+// ---------------------------------------------------------------------------
+// ray maps: the lens half supplied as data, the globe half (fisheye.c:1922-2066) as in a build
+// ---------------------------------------------------------------------------
+
+int FisheyeHost::check_raymap(int width, int height, int *platesize, std::string *why) const {
+    if (width <= 0 || height <= 0) {
+        *why = "width and height must be positive";
+        return -1;
+    }
+    if (*platesize <= 0) *platesize = width < height ? width : height;  // as a build (:707)
+    // a globe_plate may pick any of the six slots: the build's own limit
+    if (static_cast<int64_t>(*platesize) * *platesize * kMaxPlates > 0x0FFFFFFF) {
+        *why = "6 * platesize^2 exceeds the 28-bit texel index";
+        return -1;
+    }
+    if (!globe_valid_) {
+        *why = "no valid globe";
+        return -7;
+    }
+    return 0;
+}
+
+int FisheyeHost::set_raymap(int width, int height, int platesize, const float *rays) {
+    const size_t W = static_cast<size_t>(width);
+    std::vector<uint32_t> packed(W * static_cast<size_t>(height));
+    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
+    const int threads = fallback_threads_;
+    const int band = threads > 1 ? 8 : height;  // one thread: the build's single bottom-up sweep
+    const int nbands = (height + band - 1) / band;
+    const int rc = run_inverse_workers(threads, nbands, display, [&](Worker &w, int b, int *disp) {
+        const int y0 = b * band;
+        for (int ly = std::min(height, y0 + band) - 1; ly >= y0; --ly) {
+            for (size_t lx = 0; lx < W; ++lx) {
+                const size_t at = static_cast<size_t>(ly) * W + lx;
+                float ray[3] = {rays[3 * at], rays[3 * at + 1], rays[3 * at + 2]};
+                normalize3(ray);
+                packed[at] = ray_entry(w, ray, platesize, disp);
+            }
+        }
+        return 0;
+    });
+    if (rc != 0) return -2;
+    width_px_ = width;
+    height_px_ = height;
+    platesize_ = platesize;
+    unpack_map(packed.data());
+    map_plates_ = numplates_;
+    finish_build();
+    for (int i = 0; i < kMaxPlates; ++i) plates_[i].display = display[i];
+    lens_changed_ = globe_changed_ = zoom_changed_ = false;
+    built_w_ = width;
+    built_h_ = height;
+    built_ps_ = platesize;
+    return 0;
+}
+
+bool FisheyeHost::raymap_device_source(bool cuda, std::string *source, std::string *why) {
+    if (fn_globe_plate_.is_function()) return globe_plate_device_source(cuda, source, why);
+    const char *ni = getenv("BLINKY_LENS_NOINLINE");
+    *source = transpile_prelude(cuda, ni && ni[0] == '1');
+    return true;
+}
+
+int FisheyeHost::raymap_device(int width, int height, int platesize, const float *d_rays, void *stream, uint32_t **d_map, size_t *settled,
+                               std::string *why) {
+    *settled = 0;
+    if (!device_builder_) {
+        *why = "no GPU lens builder installed";
+        return 1;
+    }
+    std::string src;
+    if (!raymap_device_source(true, &src, why)) return 1;
+    std::vector<uint32_t> flagged;
+    std::vector<float> flagged_rays;
+    if (!device_builder_->raymap(src, device_params(width, height, platesize), d_rays, stream, d_map, &flagged, &flagged_rays, why)) return 1;
+    // the interpreter decides what the device could not
+    std::vector<RayPatch> patches(flagged.size());
+    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};  // (the planner derives the display flags from the finished map)
+    const int chunk = 256;
+    const int nitems = static_cast<int>((flagged.size() + chunk - 1) / chunk);
+    const int threads = flagged.size() >= 4096 ? fallback_threads_ : 1;
+    const int rc = run_inverse_workers(threads, nitems, display, [&](Worker &w, int i, int *disp) {
+        const size_t b = static_cast<size_t>(i) * chunk, e = std::min(flagged.size(), b + chunk);
+        for (size_t k = b; k < e; ++k) {
+            float ray[3] = {flagged_rays[3 * k], flagged_rays[3 * k + 1], flagged_rays[3 * k + 2]};
+            normalize3(ray);
+            patches[k] = RayPatch{flagged[k], ray_entry(w, ray, platesize, disp)};
+        }
+        return 0;
+    });
+    if (rc != 0) return -2;
+    if (!device_builder_->patch_entries(patches, stream, why)) return 1;
+    *settled = patches.size();
+    return 0;
 }
 
 }  // namespace blinky

@@ -95,6 +95,25 @@ public:
     // plates of the current lensmap: the globe's at a build, the caller's for a supplied map
     int map_numplates() const { return map_plates_; }
 
+    // ---- ray maps ------------------------------------------------------------------
+    // A field of view rays in place of the lens: width * height float32 triples, row-major, each lens_inverse's result
+    // narrowed to float and NOT normalised (normalize3 is applied here, as the build applies it; the zero vector is a
+    // pixel the lens leaves empty).  The rays go through the current globe (plate choice or globe_plate, stale plate
+    // slots, rubix grid) exactly as a build's rays do.  The lens, zoom and scale stay; the lens / globe / zoom change
+    // flags are consumed.  check_raymap: 0, or -1 for a bad size / -7 without a valid globe (reason in *why);
+    // platesize <= 0 becomes min(width, height).
+    int check_raymap(int width, int height, int *platesize, std::string *why) const;
+    // the host path on the worker threads: 0 ok; -2, changing nothing, when globe_plate raises an error
+    int set_raymap(int width, int height, int platesize, const float *rays);
+    // The device path (sizes checked): the map of the rays at d_rays (device memory, read on `stream`) in the device
+    // builder's map (*d_map), with the pixels the device could not decide settled here (*settled).  0 ok; 1 = not
+    // possible on the device (why): take the host path; -2 = globe_plate raised an error.  Changes no host state.
+    int raymap_device(int width, int height, int platesize, const float *d_rays, void *stream, uint32_t **d_map, size_t *settled,
+                      std::string *why);
+    // C++ / CUDA source the ray-map kernel is appended to: the globe's globe_plate translated alone, or the bare
+    // prelude for globes without one; false + reason when globe_plate does not translate
+    bool raymap_device_source(bool cuda, std::string *source, std::string *why);
+
     // ---- results -------------------------------------------------------------
     int width() const { return width_px_; }
     int height() const { return height_px_; }
@@ -176,8 +195,11 @@ private:
 
     int ray_to_plate_index(Worker &w, const float ray[3]);
     bool ray_to_plate_uv(int plate, const float ray[3], double *u, double *v) const;
+    bool on_rubix_grid(int px, int py, int ps) const;
     void set_from_plate(int lx, int ly, int px, int py, int plate, int *display);
+    bool ray_to_texel(Worker &w, const float ray[3], int ps, int *plate, int *px, int *py);
     void set_from_ray(Worker &w, int lx, int ly, const float ray[3], int *display);
+    uint32_t ray_entry(Worker &w, const float ray[3], int ps, int *display);
     int call_inverse(Worker &w, double x, double y, float ray[3]);
     int call_forward(Worker &w, const float ray[3], double *x, double *y);
     int build_inverse_rows(Worker &w, int y_begin, int y_end, int *display);  // rows [y_begin,y_end), bottom-up
@@ -188,7 +210,7 @@ private:
     int build_inverse(int threads);
     int build_inverse_device(int *display, std::string *why);  // 0 ok, -1 script failure, 1 = not possible (why)
     int build_forward_device(std::string *why);                // same convention
-    LensBuildParams device_params() const;
+    LensBuildParams device_params(int width, int height, int platesize) const;
     int build_forward(int threads);
     int uv_to_screen(Worker &w, int plate, double u, double v, int *lx, int *ly);
     void draw_quad(const int *tl, const int *tr, const int *bl, const int *br, int plate, int px, int py, int *display);

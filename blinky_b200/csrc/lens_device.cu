@@ -24,8 +24,9 @@ namespace {
 // bit-identical to the host.
 //
 // The text is kept in pieces so that a globe with a globe_plate script can replace the plate argmax
-// (kernel_tail): every other globe gets exactly kKernelHead + kKernelArgmax + kKernelTexel + kKernelEnd.
-const char *kKernelHead = R"KRN(
+// (kernel_tail): every other globe gets exactly kKernelParams + kKernelHead + kKernelNormalize + kKernelArgmax + kKernelTexel +
+// kKernelEnd.  The ray-map unit (raymap_tail) wraps the same pieces from kKernelNormalize on.
+const char *kKernelParams = R"KRN(
 struct LtParams {
     int width, height, platesize, numplates;
     double scale;
@@ -35,7 +36,9 @@ struct LtParams {
 };
 
 static __device__ __forceinline__ float lt_dot3(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+)KRN";
 
+const char *kKernelHead = R"KRN(
 extern "C" __global__ void __launch_bounds__(128) lt_build(const __grid_constant__ LtParams P, unsigned *__restrict__ cand) {
     const int lx = blockIdx.x * blockDim.x + threadIdx.x, ly = blockIdx.y;
     if (lx >= P.width) return;
@@ -51,7 +54,10 @@ extern "C" __global__ void __launch_bounds__(128) lt_build(const __grid_constant
     unsigned out = 0;
     if (lt_entry(c, x, y, r)) {
         float ray[3] = {lt_f32(c, r[0]), lt_f32(c, r[1]), lt_f32(c, r[2])};
-        float len = ray[0] * ray[0] + ray[1] * ray[1] + ray[2] * ray[2];
+)KRN";
+
+// normalize3 of fisheye_host.cpp (VectorNormalize)
+const char *kKernelNormalize = R"KRN(        float len = ray[0] * ray[0] + ray[1] * ray[1] + ray[2] * ray[2];
         len = (float)sqrt((double)len);
         if (len) {
             const float inv = 1 / len;
@@ -102,6 +108,39 @@ const char *kKernelGlobePlateClose = R"KRN(#ifdef LT_HAS_GLOBE_PLATE
 const char *kKernelEnd = R"KRN(    }
     if (c.flag) out |= 0x20000000u;
     cand[(size_t)ly * P.width + lx] = out;
+}
+)KRN";
+
+// The ray-map kernel (blinky_set_raymap_device): pixel `at` reads the caller's float32 ray instead of evaluating a lens,
+// and writes its packed lensmap entry (BLINKY_LM_*) straight away: a map built in one pass gives an on-grid pixel no
+// tint.  A pixel whose globe_plate decision carries a risk flag is written unmapped and listed in `flagged` for the host.
+const char *kRaymapHead = R"KRN(
+extern "C" __global__ void __launch_bounds__(256) lt_raymap(const __grid_constant__ LtParams P, const float *__restrict__ rays,
+                                                            unsigned *__restrict__ map, unsigned *__restrict__ flagged,
+                                                            unsigned *__restrict__ nflagged, unsigned flagged_cap) {
+    const size_t at = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (at >= (size_t)P.width * P.height) return;
+    Ctx c;
+    c.flag = 0;
+    c.steps = 0;
+    c.plates = P.plates;
+    c.numplates = P.numplates;
+#ifdef LT_HAS_GLOBE_PLATE
+    lt_init_mut(c);
+#endif
+    unsigned out = 0;
+    {
+        float ray[3] = {rays[3 * at], rays[3 * at + 1], rays[3 * at + 2]};
+)KRN";
+
+const char *kRaymapEnd = R"KRN(        if (out) out = (out & 0x8FFFFFFFu) | ((out & 0x40000000u) ? 7u : (unsigned)best) << 28;
+    }
+    if (c.flag) {
+        out = 0;
+        const unsigned k = atomicAdd(nflagged, 1u);
+        if (k < flagged_cap) flagged[k] = (unsigned)at;
+    }
+    map[at] = out ? out : 0x70000000u;
 }
 )KRN";
 
@@ -308,6 +347,19 @@ __global__ void fwd_owner_patch_kernel(unsigned char *owner, const uint32_t *pat
     if (k < n) fwd_apply_owner_patch(owner, patches[k]);
 }
 
+// the rays of the listed pixels, for the host to settle (ray maps)
+__global__ void gather_rays_kernel(const float *__restrict__ rays, const unsigned *__restrict__ pixels, unsigned n, float *__restrict__ out) {
+    const unsigned k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const size_t at = pixels[k];
+    for (int i = 0; i < 3; ++i) out[3 * k + i] = rays[3 * at + i];
+}
+
+__global__ void scatter_entries_kernel(uint32_t *__restrict__ map, const RayPatch *__restrict__ patches, unsigned n) {
+    const unsigned k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) map[patches[k].pixel] = patches[k].entry;
+}
+
 __global__ void __launch_bounds__(128) fwd_raster_kernel(const __grid_constant__ FwdGeom g, const FwdPoint *__restrict__ grid, FwdOut o,
                                                          const unsigned char *__restrict__ owner) {
     const int px = blockIdx.x * blockDim.x + threadIdx.x;
@@ -324,6 +376,8 @@ __global__ void fwd_resolve_kernel(const unsigned *__restrict__ idxkey, const un
 
 LensDevice::~LensDevice() {
     drop_forward_state();
+    cudaFree(ray_flagged_);
+    cudaFree(ray_map_);
     for (auto &kv : cache_) {
         if (kv.second->mod && driver().ok) driver().ModuleUnload(kv.second->mod);
         delete kv.second;
@@ -344,17 +398,27 @@ void LensDevice::drop_forward_state() {
 
 std::string LensDevice::kernel_tail(bool forward, bool globe_plate) {
     if (forward) return globe_plate ? std::string(kForwardKernelSource) + kForwardOwnerKernelSource : std::string(kForwardKernelSource);
-    if (!globe_plate) return std::string(kKernelHead) + kKernelArgmax + kKernelTexel + kKernelEnd;
-    return std::string(kKernelHead) + kKernelGlobePlateOpen + kKernelArgmax + "#endif\n" + kKernelTexel + kKernelGlobePlateClose + kKernelEnd;
+    const std::string head = std::string(kKernelParams) + kKernelHead + kKernelNormalize;
+    if (!globe_plate) return head + kKernelArgmax + kKernelTexel + kKernelEnd;
+    return head + kKernelGlobePlateOpen + kKernelArgmax + "#endif\n" + kKernelTexel + kKernelGlobePlateClose + kKernelEnd;
+}
+
+std::string LensDevice::raymap_tail(bool globe_plate) {
+    const std::string head = std::string(kKernelParams) + kRaymapHead + kKernelNormalize;
+    if (!globe_plate) return head + kKernelArgmax + kKernelTexel + kRaymapEnd;
+    return head + kKernelGlobePlateOpen + kKernelArgmax + "#endif\n" + kKernelTexel + kKernelGlobePlateClose + kRaymapEnd;
 }
 
 bool LensDevice::compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log) {
+    return compile_unit(lens_source + kernel_tail(forward, source_has_globe_plate(lens_source)), cubin, log);
+}
+
+bool LensDevice::compile_unit(const std::string &src, std::vector<char> *cubin, std::string *log) {
     Nvrtc &n = nvrtc();
     if (!n.why.empty()) {
         *log = n.why;
         return false;
     }
-    const std::string src = lens_source + kernel_tail(forward, source_has_globe_plate(lens_source));
     nvrtcProgram prog;
     nvrtcResult rc = n.CreateProgram(&prog, src.c_str(), "lens.cu", 0, nullptr, nullptr);
     if (rc != NVRTC_SUCCESS) {
@@ -383,7 +447,7 @@ bool LensDevice::compile(const std::string &lens_source, bool forward, std::vect
     return sz > 0;
 }
 
-LensDevice::Module *LensDevice::module_for(const std::string &lens_source, bool forward, std::string *err) {
+LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit, std::string *err) {
     compile_ms_ = 0;
     if (cudaSetDevice(device_) != cudaSuccess) {
         *err = "cudaSetDevice failed";
@@ -394,21 +458,24 @@ LensDevice::Module *LensDevice::module_for(const std::string &lens_source, bool 
         *err = "CUDA driver entry points unavailable";
         return nullptr;
     }
-    const std::string cache_key = (forward ? "F" : "I") + lens_source;
+    const std::string cache_key = "IFR"[unit] + source;
     auto it = cache_.find(cache_key);
     if (it != cache_.end()) return it->second;
     auto t0 = std::chrono::steady_clock::now();
     std::vector<char> cubin;
     std::string log;
-    if (!compile(lens_source, forward, &cubin, &log)) {
+    const bool compiled = unit == kRaymapUnit ? compile_unit(source + raymap_tail(source_has_globe_plate(source)), &cubin, &log)
+                                              : compile(source, unit == kForwardUnit, &cubin, &log);
+    if (!compiled) {
         *err = log;
         return nullptr;
     }
     cudaFree(nullptr);  // make sure the primary context is current
     Module *m = new Module;
     CUresult cr = d.ModuleLoadData(&m->mod, cubin.data());
-    if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, forward ? "lt_forward_points" : "lt_build");
-    if (cr == CUDA_SUCCESS && forward && source_has_globe_plate(lens_source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
+    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : "lt_build";
+    if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, entry);
+    if (cr == CUDA_SUCCESS && unit == kForwardUnit && source_has_globe_plate(source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
     if (cr != CUDA_SUCCESS) {
         if (m->mod) d.ModuleUnload(m->mod);
         delete m;
@@ -433,7 +500,7 @@ bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p,
         *err = "screen taller than 65535 rows, the device lens kernel's grid limit";
         return false;
     }
-    Module *m = module_for(lens_source, false, err);
+    Module *m = module_for(lens_source, kInverseUnit, err);
     if (!m) return false;
     Driver &d = driver();
     const size_t npix = static_cast<size_t>(p.width) * p.height;
@@ -472,12 +539,131 @@ bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p,
     return ok;
 }
 
+bool LensDevice::raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
+                        std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) {
+    kernel_ms_ = 0;
+    const size_t npix = static_cast<size_t>(p.width) * p.height;
+    if (npix >= 0xFFFFFFFFull) {   // the flagged list holds 32-bit pixel numbers
+        *err = "screen of 2^32 pixels or more";
+        return false;
+    }
+    Module *m = module_for(globe_source, kRaymapUnit, err);
+    if (!m) return false;
+    // kept for the context's later ray maps: the look-around loop makes one per frame
+    cudaError_t ce = cudaSuccess;
+    if (!ray_flagged_) ce = cudaMalloc(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned));
+    if (ce == cudaSuccess && ray_map_pixels_ < npix) {
+        cudaFree(ray_map_);
+        ray_map_ = nullptr;
+        ray_map_pixels_ = 0;
+        ce = cudaMalloc(&ray_map_, npix * sizeof(uint32_t));
+        if (ce == cudaSuccess) ray_map_pixels_ = npix;
+    }
+    if (ce != cudaSuccess) {
+        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
+        return false;
+    }
+    *d_map = ray_map_;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    LensBuildParams params = p;
+    unsigned *count = ray_flagged_, *list = ray_flagged_ + 1;
+    unsigned cap = kUndecidedCap;
+    void *args[] = {&params, &d_rays, &ray_map_, &list, &count, &cap};
+    const unsigned block = 256;
+    unsigned n = 0;
+    bool ok = true;
+    ce = cudaMemsetAsync(count, 0, sizeof(unsigned), s);
+    if (ce == cudaSuccess) {
+        cudaEventRecord(e0, s);
+        const CUresult cr = driver().LaunchKernel(m->fn, static_cast<unsigned>((npix + block - 1) / block), 1, 1, block, 1, 1, 0, s, args, nullptr);
+        cudaEventRecord(e1, s);
+        if (cr != CUDA_SUCCESS) {
+            *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
+            ok = false;
+        }
+    }
+    if (ok) {
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&n, count, sizeof n, cudaMemcpyDeviceToHost, s);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+        if (ce != cudaSuccess) {
+            *err = std::string("ray map kernel: ") + cudaGetErrorString(ce);
+            ok = false;
+        }
+    }
+    if (ok && n > kUndecidedCap) {
+        *err = "too many pixels need the interpreter (" + std::to_string(n) + ")";
+        ok = false;
+    }
+    if (ok) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, e0, e1);
+        kernel_ms_ = ms;
+        ++launches_;
+        flagged->resize(n);
+        flagged_rays->resize(3 * static_cast<size_t>(n));
+    }
+    if (ok && n) {
+        // only the flagged pixels' rays come back
+        float *d_gathered = nullptr;
+        ce = cudaMalloc(&d_gathered, 3 * static_cast<size_t>(n) * sizeof(float));
+        if (ce == cudaSuccess) {
+            gather_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, list, n, d_gathered);
+            ++launches_;
+            ce = cudaMemcpyAsync(flagged->data(), list, n * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
+            if (ce == cudaSuccess) ce = cudaMemcpyAsync(flagged_rays->data(), d_gathered, flagged_rays->size() * sizeof(float), cudaMemcpyDeviceToHost, s);
+            if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+            cudaFree(d_gathered);
+        }
+        if (ce != cudaSuccess) {
+            *err = std::string("ray map gather: ") + cudaGetErrorString(ce);
+            ok = false;
+        }
+    }
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    return ok;
+}
+
+bool LensDevice::patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) {
+    if (patches.empty()) return true;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    RayPatch *d_patches = nullptr;
+    cudaError_t ce = cudaMalloc(&d_patches, patches.size() * sizeof(RayPatch));
+    if (ce == cudaSuccess) {
+        ce = cudaMemcpyAsync(d_patches, patches.data(), patches.size() * sizeof(RayPatch), cudaMemcpyHostToDevice, s);
+        if (ce == cudaSuccess) {
+            const unsigned n = static_cast<unsigned>(patches.size());
+            scatter_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(ray_map_, d_patches, n);
+            ++launches_;
+            ce = cudaStreamSynchronize(s);  // (patches is pageable host memory the copy may still read)
+        }
+        cudaFree(d_patches);
+    }
+    if (ce != cudaSuccess) {
+        *err = std::string("ray map patch: ") + cudaGetErrorString(ce);
+        return false;
+    }
+    return true;
+}
+
+bool LensDevice::copy_to_host(void *dst, const void *d_src, size_t bytes, void *stream, std::string *err) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    cudaError_t ce = cudaSetDevice(device_);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, s);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+    if (ce != cudaSuccess) *err = std::string("copying the rays to the host: ") + cudaGetErrorString(ce);
+    return ce == cudaSuccess;
+}
+
 bool LensDevice::forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
                                 std::vector<uint32_t> *undecided_texels, std::string *err) {
     undecided_texels->clear();
     kernel_ms_ = 0;
     drop_forward_state();
-    Module *m = module_for(lens_source, true, err);
+    Module *m = module_for(lens_source, kForwardUnit, err);
     if (!m) return false;
     Driver &d = driver();
     const size_t n1 = static_cast<size_t>(p.platesize) + 1;

@@ -59,6 +59,12 @@ constexpr uint8_t kOwnerRisk = 2u;   // not provably the host's answer: the host
 // a texel owner the host decided: the texel index, | kOwnerPatchOwned when the texel is owned
 constexpr uint32_t kOwnerPatchOwned = 0x80000000u;
 
+// a ray-map entry the host settled: pixel number (ly * width + lx) and packed lensmap entry
+struct RayPatch {
+    uint32_t pixel;
+    uint32_t entry;
+};
+
 // True when a translated source defines lt_globe_plate (lua_transpile.h).
 inline bool source_has_globe_plate(const std::string &lens_source) { return lens_source.find("\n#define LT_HAS_GLOBE_PLATE 1\n") != std::string::npos; }
 
@@ -79,6 +85,15 @@ public:
     // reference prints.
     virtual bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
                                 uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) = 0;
+    // ray maps: the packed lensmap entry of each of the width * height float32 rays at d_rays (unnormalised, three per
+    // pixel), on `stream` (a cudaStream_t) after the work already there, into a device map the builder keeps until its
+    // next ray map (*d_map).  globe_source: the globe's globe_plate translated alone, or the bare prelude for argmax
+    // globes.  Pixels whose plate decision is not provably the host's are written unmapped; *flagged receives them and
+    // *flagged_rays their rays, for the host to settle.
+    virtual bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
+                        std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) = 0;
+    // writes the settled entries into that map on `stream`; returns once they are there
+    virtual bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) = 0;
 };
 
 class LensDevice : public DeviceLensBuilder {
@@ -94,12 +109,19 @@ public:
                         std::vector<uint32_t> *undecided_texels, std::string *err) override;
     bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx, uint8_t *tint,
                         int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) override;
+    bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
+                std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) override;
+    bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) override;
+    // bytes from device memory on `stream`, after the work already there (a ray map that takes the host path)
+    bool copy_to_host(void *dst, const void *d_src, size_t bytes, void *stream, std::string *err);
 
     // the fixed CUDA source appended to a translated lens (the per-pixel / per-grid-point tail);
     // exposed so that the CPU test-suite can run the very same text through a host shim.
     // globe_plate: the source defines lt_globe_plate — the inverse tail then lets it pick the plate and
     // the forward tail gains the owner kernel; without it the tails are unchanged.
     static std::string kernel_tail(bool forward, bool globe_plate = false);
+    // the same for the ray-map kernel, appended to the globe's translated globe_plate (or the bare prelude)
+    static std::string raymap_tail(bool globe_plate);
 
     // compile only (no GPU needed): used by the CPU test-suite and by build()
     static bool compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log);
@@ -111,11 +133,16 @@ public:
 private:
     struct Module;
     struct ForwardState;
-    Module *module_for(const std::string &lens_source, bool forward, std::string *err);
+    enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit };
+    static bool compile_unit(const std::string &src, std::vector<char> *cubin, std::string *log);
+    Module *module_for(const std::string &source, Unit unit, std::string *err);
     void drop_forward_state();
     int device_;
-    std::map<std::string, Module *> cache_;  // by flavour + source text
+    std::map<std::string, Module *> cache_;  // by unit + source text
     ForwardState *fwd_ = nullptr;
+    unsigned *ray_flagged_ = nullptr;  // ray maps: [0] the flagged count, then the flagged pixels
+    uint32_t *ray_map_ = nullptr;      // ray maps: the last map, ray_map_pixels_ entries
+    size_t ray_map_pixels_ = 0;
     double compile_ms_ = 0, kernel_ms_ = 0;
     int64_t launches_ = 0;
 };

@@ -169,6 +169,35 @@ int blinky_set_lensmap(blinky_ctx *ctx, int width, int height, int platesize, in
 int blinky_set_lensmap_device(blinky_ctx *ctx, int width, int height, int platesize, int numplates, const uint32_t *d_packed,
                               void *stream);
 
+/* Ray maps: the lens supplied as data.  A lens is one view ray per screen pixel (lens_inverse,
+ * fisheye.c:2084-2124); the globe maps each ray to a plate texel and a rubix tint (:1922-2066).  These
+ * calls take the rays and do the globe's half, so a lens that is a table, a calibrated dome or
+ * projector warp, a camera model fitted elsewhere or a view turned by head tracking needs no script.
+ * rays: width*height float32 triples, row-major, dense: pixel (lx, ly) at rays[3*(ly*width + lx) + k],
+ * ly = 0 the top row, in the globe's frame.  Each triple is what lens_inverse returns, narrowed to
+ * float and NOT normalised: the library normalises it as the build does (VectorNormalize), and
+ * normalising twice is not exact, so a caller that normalises first gets a slightly different map.  A
+ * pixel the lens leaves empty is the zero vector (it maps to nothing, as in the reference); NaN and
+ * infinite components follow the reference's arithmetic.  The rays go through the current globe: its
+ * plates, its globe_plate script if it has one (with the plate slots an earlier globe left, as in a
+ * build), and the current f_rubixgrid; the result equals what blinky_build_lensmap makes of a lens
+ * returning these rays.  platesize <= 0 means min(width, height), and 6 * platesize^2 must stay below
+ * 2^28.  The lens, zoom and blinky_scale are untouched; like a build, the call consumes the lens, globe
+ * and zoom changes.  The map is installed as blinky_set_lensmap installs one (every query and warp
+ * then reads it; a graph captured before keeps its map until blinky_release_captures).  On failure
+ * nothing changes: BLINKY_E_INVALID for NULL or misaligned rays or a bad size, BLINKY_E_STATE without
+ * a valid globe, BLINKY_E_SCRIPT when globe_plate raises an error.
+ * blinky_set_raymap reads host memory on the worker threads and works on host-only contexts.
+ * blinky_set_raymap_device reads d_rays (4-byte aligned device memory) on `stream` (a cudaStream_t,
+ * NULL = the default stream) after the work already there, maps and plans on the GPU, and returns once
+ * the map is resident: the caller may then reuse d_rays.  Pixels whose globe_plate decision the GPU
+ * cannot prove are settled by the interpreter; when that is not possible (globe_plate outside the
+ * translatable subset, no NVRTC, too many such pixels) the rays are copied to the host and take the
+ * host path.  blinky_build_info says which path ran and how many pixels the interpreter settled.  Not
+ * while a stream is capturing.  BLINKY_E_NODEVICE on a host-only context. */
+int blinky_set_raymap(blinky_ctx *ctx, int width, int height, int platesize, const float *rays);
+int blinky_set_raymap_device(blinky_ctx *ctx, int width, int height, int platesize, const float *d_rays, void *stream);
+
 /* ---- state queries ------------------------------------------------------ */
 int blinky_fisheye_enabled(blinky_ctx *ctx);          /* fisheye_enabled, :293 */
 int blinky_lens_valid(blinky_ctx *ctx);
@@ -215,7 +244,9 @@ int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate
  * lens_inverse), bit 2 = append the fixed kernel (the per-pixel / per-grid-point tail) and, when
  * the globe has a globe_plate script, translate it into the same unit — with bits 0 and 2 this is
  * exactly what NVRTC is given.  bit 3 = the globe's globe_plate translated alone (bit 0 still picks
- * CUDA; bits 1 and 2 are ignored).  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT
+ * CUDA; bits 1 and 2 are ignored).  bit 4 = the ray-map unit of blinky_set_raymap_device: the globe's
+ * globe_plate translated alone (nothing for globes without one) and the ray-map kernel; with bit 0
+ * this is exactly what NVRTC is given (bits 1 to 3 are ignored).  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT
  * when the lens (or globe_plate) is missing or outside the translatable subset (reason:
  * blinky_last_error). */
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize);
