@@ -63,6 +63,8 @@ _SIGNATURES = [
     ("blinky_set_lensmap_device", c_int, [_CTX, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_set_raymap", c_int, [_CTX, c_int, c_int, c_int, c_void_p]),
     ("blinky_set_raymap_device", c_int, [_CTX, c_int, c_int, c_int, c_void_p, c_void_p]),
+    ("blinky_get_raymap", c_int, [_CTX, c_int, c_int, c_void_p]),
+    ("blinky_get_raymap_device", c_int, [_CTX, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_build_info", c_char_p, [_CTX]),
     ("blinky_plan_digest", ctypes.c_uint64, [_CTX, c_int]),
     ("blinky_get_tile_plan", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
@@ -303,6 +305,23 @@ class Fisheye:
             raise ValueError(f"set_raymap: expected a contiguous [H, W, 3] float32 tensor, got {rays.dtype} {tuple(rays.shape)}")
         self._check(self._lib.blinky_set_raymap_device(self._ctx, rays.shape[1], rays.shape[0], platesize, rays.data_ptr(), stream))
 
+    def raymap(self, width: int, height: int, out=None, stream: int | None = None):
+        """The view rays a width x height build of the current lens evaluates, as set_raymap reads them: [height,
+        width, 3] float32, lens_inverse at ((lx - width//2) * scale, -(ly - height//2) * scale) narrowed to float and not
+        normalised, the zero vector for nil.  No `out`: a new numpy array (blinky_get_raymap, on the worker threads).
+        `out`, a contiguous CUDA float32 [height, width, 3] tensor: filled on `stream` after the work already there
+        (blinky_get_raymap_device, evaluated on the GPU) and returned once complete."""
+        if out is None:
+            rays = np.empty((height, width, 3), np.float32)
+            self._check(self._lib.blinky_get_raymap(self._ctx, width, height, rays.ctypes.data))
+            return rays
+        if not (hasattr(out, "is_cuda") and out.is_cuda):
+            raise TypeError("raymap: out must be a CUDA tensor")
+        if tuple(out.shape) != (height, width, 3) or str(out.dtype) != "torch.float32" or not out.is_contiguous():
+            raise ValueError(f"raymap: expected a contiguous [{height}, {width}, 3] float32 tensor, got {out.dtype} {tuple(out.shape)}")
+        self._check(self._lib.blinky_get_raymap_device(self._ctx, width, height, out.data_ptr(), stream))
+        return out
+
     @property
     def build_info(self) -> str:
         """How the last lensmap was built ("device: ..." or "host ...")."""
@@ -415,12 +434,14 @@ class Fisheye:
         return st, plate.value
 
     def lens_source(self, cuda: bool = False, forward: bool = False, with_kernel: bool = False, globe_plate: bool = False,
-                    raymap: bool = False) -> str:
+                    raymap: bool = False, rays: bool = False) -> str:
         """The current ``lens_inverse`` (or ``lens_forward``) translated to C++/CUDA (raises when not translatable);
         ``with_kernel`` appends the fixed kernel the device builder launches and translates the globe's
         ``globe_plate`` into the same unit when there is one.  ``globe_plate``: that function translated alone.
-        ``raymap``: the unit of the ray-map kernel (set_raymap on a CUDA tensor), globe_plate and kernel."""
-        flavour = int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0) | (8 if globe_plate else 0) | (16 if raymap else 0)
+        ``raymap``: the unit of the ray-map kernel (set_raymap on a CUDA tensor), globe_plate and kernel.
+        ``rays``: the unit of the ray-export kernel (raymap into a CUDA tensor), lens_inverse and kernel."""
+        flavour = (int(cuda) | (2 if forward else 0) | (4 if with_kernel else 0) | (8 if globe_plate else 0) | (16 if raymap else 0)
+                   | (32 if rays else 0))
         n = self._lib.blinky_lens_source(self._ctx, flavour, None, 0)
         if n < 0:
             self._check(n)

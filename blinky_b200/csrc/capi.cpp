@@ -301,6 +301,28 @@ int check_raymap(blinky_ctx *ctx, const char *who, int width, int height, int *p
     return BLINKY_OK;
 }
 
+// the checks both ray-export entry points make before anything runs; *scale: the zoom of a width x height build
+int check_export(blinky_ctx *ctx, const char *who, int width, int height, const float *rays, double *scale) {
+    if (!rays || reinterpret_cast<uintptr_t>(rays) % 4 != 0) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": rays must be a non-NULL, 4-byte aligned pointer");
+    if (width <= 0 || height <= 0) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": width and height must be positive");
+    std::string why;
+    const int rc = ctx->host.check_rays(width, height, scale, &why);
+    if (rc == -7) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": " + why);
+    if (rc != 0) return set_err(ctx, BLINKY_E_ZOOM, std::string(who) + ": zoom could not be computed for this lens: " + ctx->host.log());
+    return BLINKY_OK;
+}
+
+// blinky_get_raymap and the host path of blinky_get_raymap_device: the rays into host memory on the worker threads
+int get_raymap_host(blinky_ctx *ctx, const char *who, int width, int height, double scale, float *rays, const std::string &path) {
+    auto t0 = std::chrono::steady_clock::now();
+    if (ctx->host.export_rays(width, height, scale, rays) != 0)
+        return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": lens_inverse failed: " + ctx->host.log());
+    char t[64];
+    snprintf(t, sizeof t, "; rays %.1f ms", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+    ctx->build_info = "ray export, " + path + t;
+    return BLINKY_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -309,6 +331,13 @@ int blinky_set_raymap(blinky_ctx *ctx, int width, int height, int platesize, con
     const char *who = "blinky_set_raymap";
     const int rc = check_raymap(ctx, who, width, height, &platesize, rays);
     return rc != BLINKY_OK ? rc : set_raymap_host(ctx, who, width, height, platesize, rays, "host");
+}
+
+int blinky_get_raymap(blinky_ctx *ctx, int width, int height, float *rays) {
+    const char *who = "blinky_get_raymap";
+    double scale;
+    const int rc = check_export(ctx, who, width, height, rays, &scale);
+    return rc != BLINKY_OK ? rc : get_raymap_host(ctx, who, width, height, scale, rays, "host");
 }
 
 const char *blinky_build_info(blinky_ctx *ctx) { return ctx->build_info.c_str(); }
@@ -406,7 +435,10 @@ int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate
 
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize) {
     std::string s, why;
-    if (flavour & 16) {
+    if (flavour & 32) {
+        if (!ctx->host.lens_device_source((flavour & 1) != 0, &s, &why)) return set_err(ctx, BLINKY_E_SCRIPT, why);
+        s += LensDevice::rays_tail();
+    } else if (flavour & 16) {
         if (!ctx->host.raymap_device_source((flavour & 1) != 0, &s, &why)) return set_err(ctx, BLINKY_E_SCRIPT, why);
         s += LensDevice::raymap_tail(blinky::source_has_globe_plate(s));
     } else if (flavour & 8) {
@@ -536,6 +568,32 @@ int blinky_set_raymap_device(blinky_ctx *ctx, int width, int height, int platesi
     char t[256];
     snprintf(t, sizeof t, "ray map, device: %zu of %zu pixels settled by the interpreter; map %.3f ms (NVRTC %.0f ms, kernel %.3f ms), plan+adopt %.3f ms",
              settled, npix, ms_map, ctx->lens_dev->last_compile_ms(), ctx->lens_dev->last_kernel_ms(), ms_since(t0));
+    ctx->build_info = t;
+    return BLINKY_OK;
+}
+
+int blinky_get_raymap_device(blinky_ctx *ctx, int width, int height, float *d_rays, void *stream) {
+    NEED_DEVICE(ctx);
+    const char *who = "blinky_get_raymap_device";
+    double scale;
+    int rc = check_export(ctx, who, width, height, d_rays, &scale);
+    if (rc != BLINKY_OK) return rc;
+    // the host settles flagged pixels and the call returns with the field complete: nothing here can be captured
+    if (LensDevice::capturing(stream)) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": the stream is capturing a graph");
+    const size_t npix = static_cast<size_t>(width) * height;
+    std::string why;
+    size_t settled = 0;
+    rc = ctx->host.export_rays_device(width, height, scale, d_rays, stream, &settled, &why);
+    if (rc == -2) return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": lens_inverse failed: " + ctx->host.log());
+    if (rc == 1) {
+        std::vector<float> rays(3 * npix);
+        rc = get_raymap_host(ctx, who, width, height, scale, rays.data(), "host (" + why + ")");
+        if (rc != BLINKY_OK) return rc;
+        return ctx->lens_dev->copy_to_device(d_rays, rays.data(), rays.size() * sizeof(float), stream, &ctx->err) ? BLINKY_OK : BLINKY_E_CUDA;
+    }
+    char t[192];
+    snprintf(t, sizeof t, "ray export, device: %zu of %zu pixels settled by the interpreter; NVRTC %.0f ms, kernel %.3f ms", settled, npix,
+             ctx->lens_dev->last_compile_ms(), ctx->lens_dev->last_kernel_ms());
     ctx->build_info = t;
     return BLINKY_OK;
 }

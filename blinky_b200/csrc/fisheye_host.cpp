@@ -794,6 +794,13 @@ bool FisheyeHost::load_globe() {
 // ---------------------------------------------------------------------------
 
 int FisheyeHost::call_inverse(Worker &w, double x, double y, float ray[3]) {
+    const int status = eval_inverse(w, x, y, ray);
+    if (status == 1) normalize3(ray);
+    return status;
+}
+
+// lens_inverse(x, y) narrowed to float, not normalised: 1 = a ray, 0 = nil, -1 = a bad result (message printed)
+int FisheyeHost::eval_inverse(Worker &w, double x, double y, float ray[3]) {
     Value args[2] = {Value(x), Value(y)};
     ValueList ret;
     w.L->call(w.inverse, args, 2, ret);  // LuaError propagates to the builder
@@ -803,7 +810,6 @@ int FisheyeHost::call_inverse(Worker &w, double x, double y, float ray[3]) {
             ray[0] = static_cast<float>(a);
             ray[1] = static_cast<float>(b);
             ray[2] = static_cast<float>(c);
-            normalize3(ray);
             return 1;
         }
         print("lens_inverse returned a non-number value for x,y,z\n");
@@ -920,8 +926,8 @@ int FisheyeHost::globe_plate(double x, double y, double z, int *plate) {
 // zoom (fisheye.c:1293-1386)
 // ---------------------------------------------------------------------------
 
-bool FisheyeHost::calc_zoom() {
-    scale_ = -1;
+bool FisheyeHost::calc_zoom(int width, int height, double *scale) {
+    *scale = -1;
     if (zoom_type_ == ZOOM_FOV || zoom_type_ == ZOOM_VFOV) {
         if (max_fov_ <= 0 || max_vfov_ <= 0) {
             print("max_fov & max_vfov not specified, try \"f_cover\"\n");
@@ -958,28 +964,28 @@ bool FisheyeHost::calc_zoom() {
             print("ray_to_xy did not return a valid r value for determining FOV scale\n");
             return false;
         }
-        scale_ = zoom_type_ == ZOOM_FOV ? x / (width_px_ * 0.5) : y / (height_px_ * 0.5);
+        *scale = zoom_type_ == ZOOM_FOV ? x / (width * 0.5) : y / (height * 0.5);
     } else if (zoom_type_ == ZOOM_CONTAIN || zoom_type_ == ZOOM_COVER) {
-        double fit_w = lens_width_ / width_px_;
-        double fit_h = lens_height_ / height_px_;
+        double fit_w = lens_width_ / width;
+        double fit_h = lens_height_ / height;
         bool have_w = lens_width_ > 0, have_h = lens_height_ > 0;
         if (!have_w && have_h) {
-            scale_ = fit_h;
+            *scale = fit_h;
         } else if (have_w && !have_h) {
-            scale_ = fit_w;
+            *scale = fit_w;
         } else if (!have_w && !have_h) {
             print("neither lens_height nor lens_width are valid/specified.  Try f_fov instead.\n");
             return false;
         } else {
             double lens_aspect = lens_width_ / lens_height_;
-            double screen_aspect = static_cast<double>(width_px_) / height_px_;
+            double screen_aspect = static_cast<double>(width) / height;
             bool lens_wider = lens_aspect > screen_aspect;
-            if (zoom_type_ == ZOOM_CONTAIN) scale_ = lens_wider ? fit_w : fit_h;
-            else scale_ = lens_wider ? fit_h : fit_w;
+            if (zoom_type_ == ZOOM_CONTAIN) *scale = lens_wider ? fit_w : fit_h;
+            else *scale = lens_wider ? fit_h : fit_w;
         }
     }
-    if (scale_ <= 0) {
-        print("init returned a scale of %f, which is  <= 0\n", scale_);
+    if (*scale <= 0) {
+        print("init returned a scale of %f, which is  <= 0\n", *scale);
         return false;
     }
     return true;
@@ -1528,7 +1534,7 @@ int FisheyeHost::build_lensmap(int width, int height, int platesize, int threads
         rc = -7;
     } else {
         t0 = clk::now();
-        const bool zoom_ok = calc_zoom();
+        const bool zoom_ok = calc_zoom(width_px_, height_px_, &scale_);
         ms_zoom = ms_since(t0);
         t0 = clk::now();
         if (!zoom_ok) {
@@ -1847,6 +1853,77 @@ int FisheyeHost::raymap_device(int width, int height, int platesize, const float
     if (rc != 0) return -2;
     if (!device_builder_->patch_entries(patches, stream, why)) return 1;
     *settled = patches.size();
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// ray export: the lens half of a build (fisheye.c:2084-2124) without the globe, as set_raymap reads it
+// ---------------------------------------------------------------------------
+
+int FisheyeHost::check_rays(int width, int height, double *scale, std::string *why) {
+    if (!lens_valid_) {
+        *why = "no valid lens";
+        return -7;
+    }
+    if (map_type_ != MAP_INVERSE || !fn_inverse_.is_function()) {
+        *why = "the lens maps with lens_forward and has no per-pixel ray";
+        return -7;
+    }
+    return calc_zoom(width, height, scale) ? 0 : -3;
+}
+
+int FisheyeHost::export_rays(int width, int height, double scale, float *rays) {
+    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};  // (no globe is involved)
+    const int band = 8;
+    const int nbands = (height + band - 1) / band;
+    const int rc = run_inverse_workers(fallback_threads_, nbands, display, [&](Worker &w, int b, int *) {
+        for (int ly = b * band; ly < std::min(height, (b + 1) * band); ++ly) {
+            const double y = -(ly - height / 2) * scale;
+            for (int lx = 0; lx < width; ++lx) {
+                float *o = rays + 3 * (static_cast<size_t>(ly) * width + lx);
+                const int status = eval_inverse(w, (lx - width / 2) * scale, y, o);
+                if (status == -1) return -1;
+                if (status == 0) o[0] = o[1] = o[2] = 0;
+            }
+        }
+        return 0;
+    });
+    return rc == 0 ? 0 : -2;
+}
+
+int FisheyeHost::export_rays_device(int width, int height, double scale, float *d_rays, void *stream, size_t *settled, std::string *why) {
+    *settled = 0;
+    if (!device_builder_) {
+        *why = "no GPU lens builder installed";
+        return 1;
+    }
+    std::string src;
+    if (!lens_device_source(true, &src, why)) return 1;
+    LensBuildParams p = device_params(width, height, platesize_);
+    p.scale = scale;
+    std::vector<uint32_t> flagged;
+    if (!device_builder_->rays(src, p, d_rays, stream, &flagged, why)) return 1;
+    // the interpreter evaluates what the device could not
+    std::vector<RaySample> samples(flagged.size());
+    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
+    const int chunk = 256;
+    const int nitems = static_cast<int>((flagged.size() + chunk - 1) / chunk);
+    const int threads = flagged.size() >= 4096 ? fallback_threads_ : 1;
+    const int rc = run_inverse_workers(threads, nitems, display, [&](Worker &w, int i, int *) {
+        const size_t b = static_cast<size_t>(i) * chunk, e = std::min(flagged.size(), b + chunk);
+        for (size_t k = b; k < e; ++k) {
+            const int ly = static_cast<int>(flagged[k] / static_cast<uint32_t>(width)), lx = static_cast<int>(flagged[k] % static_cast<uint32_t>(width));
+            RaySample &s = samples[k];
+            s.pixel = flagged[k];
+            const int status = eval_inverse(w, (lx - width / 2) * scale, -(ly - height / 2) * scale, s.ray);
+            if (status == -1) return -1;
+            if (status == 0) s.ray[0] = s.ray[1] = s.ray[2] = 0;
+        }
+        return 0;
+    });
+    if (rc != 0) return -2;
+    if (!device_builder_->patch_rays(samples, d_rays, stream, why)) return 1;
+    *settled = samples.size();
     return 0;
 }
 

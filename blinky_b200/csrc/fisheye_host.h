@@ -114,6 +114,21 @@ public:
     // prelude for globes without one; false + reason when globe_plate does not translate
     bool raymap_device_source(bool cuda, std::string *source, std::string *why);
 
+    // ---- ray export ------------------------------------------------------------------
+    // The view rays a width x height build evaluates, as set_raymap reads them: pixel (lx, ly) gets
+    // lens_inverse((lx - width/2) * scale, -(ly - height/2) * scale) (integer /2) narrowed to float and not normalised,
+    // (0, 0, 0) for nil, at rays[3 * (ly * width + lx)].  The loaded lens_inverse is evaluated (the script is not re-run)
+    // and no globe is needed.  Nothing of the context changes: not the map, the scale or the change flags.
+    // check_rays: 0 with the scale calc_zoom gives for width x height in *scale; -7 without a valid lens that has a
+    // per-pixel ray (reason in *why); -3 when the zoom fails (the build's console message is printed).
+    int check_rays(int width, int height, double *scale, std::string *why);
+    // the host path on the worker threads: 0 ok; -2 when lens_inverse raises an error or returns a bad result
+    int export_rays(int width, int height, double scale, float *rays);
+    // The device path: the rays into d_rays (device memory) on `stream`, the pixels the device could not decide evaluated
+    // here (*settled).  0 ok, the field complete; 1 = not possible on the device (why): take the host path; -2 as
+    // export_rays.
+    int export_rays_device(int width, int height, double scale, float *d_rays, void *stream, size_t *settled, std::string *why);
+
     // ---- results -------------------------------------------------------------
     int width() const { return width_px_; }
     int height() const { return height_px_; }
@@ -189,7 +204,7 @@ private:
     void clear_lens_vars();
     void clear_globe_vars();
     bool run_script(const std::string &kind, const std::string &name, const std::string *source);
-    bool calc_zoom();
+    bool calc_zoom(int width, int height, double *scale);  // the scale of a width x height build; false + console message
     void create_palmap();
     int find_closest_pal_index(int r, int g, int b) const;
 
@@ -201,6 +216,7 @@ private:
     void set_from_ray(Worker &w, int lx, int ly, const float ray[3], int *display);
     uint32_t ray_entry(Worker &w, const float ray[3], int ps, int *display);
     int call_inverse(Worker &w, double x, double y, float ray[3]);
+    int eval_inverse(Worker &w, double x, double y, float ray[3]);
     int call_forward(Worker &w, const float ray[3], double *x, double *y);
     int build_inverse_rows(Worker &w, int y_begin, int y_end, int *display);  // rows [y_begin,y_end), bottom-up
     int build_inverse_pixels(Worker &w, const int32_t *pixels, size_t n, int *display);

@@ -24,8 +24,9 @@ namespace {
 // bit-identical to the host.
 //
 // The text is kept in pieces so that a globe with a globe_plate script can replace the plate argmax
-// (kernel_tail): every other globe gets exactly kKernelParams + kKernelHead + kKernelNormalize + kKernelArgmax + kKernelTexel +
-// kKernelEnd.  The ray-map unit (raymap_tail) wraps the same pieces from kKernelNormalize on.
+// (kernel_tail): every other globe gets exactly kKernelParams + kKernelSignature + kKernelHead + kKernelNormalize + kKernelArgmax +
+// kKernelTexel + kKernelEnd.  The ray-map unit (raymap_tail) wraps the same pieces from kKernelNormalize on; the
+// ray-export unit (rays_tail) puts kKernelHead, the lens half, under its own signature and end.
 const char *kKernelParams = R"KRN(
 struct LtParams {
     int width, height, platesize, numplates;
@@ -38,9 +39,12 @@ struct LtParams {
 static __device__ __forceinline__ float lt_dot3(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 )KRN";
 
-const char *kKernelHead = R"KRN(
+const char *kKernelSignature = R"KRN(
 extern "C" __global__ void __launch_bounds__(128) lt_build(const __grid_constant__ LtParams P, unsigned *__restrict__ cand) {
-    const int lx = blockIdx.x * blockDim.x + threadIdx.x, ly = blockIdx.y;
+)KRN";
+
+// the pixel's coordinates (fisheye.c:2100-2105, integer /2) and the lens's ray, narrowed to float
+const char *kKernelHead = R"KRN(    const int lx = blockIdx.x * blockDim.x + threadIdx.x, ly = blockIdx.y;
     if (lx >= P.width) return;
     const double x = (lx - P.width / 2) * P.scale;
     const double y = -(ly - P.height / 2) * P.scale;
@@ -141,6 +145,30 @@ const char *kRaymapEnd = R"KRN(        if (out) out = (out & 0x8FFFFFFFu) | ((ou
         if (k < flagged_cap) flagged[k] = (unsigned)at;
     }
     map[at] = out ? out : 0x70000000u;
+}
+)KRN";
+
+// The ray-export kernel (blinky_get_raymap_device): the build's lens half (kKernelHead) for pixel (lx, ly), whose
+// narrowed ray, or the zero vector for nil, goes straight into the caller's float32[height][width][3] field.  A pixel
+// with a risk flag is listed in `flagged`; the host evaluates it and overwrites its ray.
+const char *kRaysSignature = R"KRN(
+extern "C" __global__ void __launch_bounds__(128) lt_rays(const __grid_constant__ LtParams P, float *__restrict__ rays,
+                                                          unsigned *__restrict__ flagged, unsigned *__restrict__ nflagged,
+                                                          unsigned flagged_cap) {
+)KRN";
+
+const char *kRaysEnd = R"KRN(        float *o = rays + 3 * ((size_t)ly * P.width + lx);
+        o[0] = ray[0];
+        o[1] = ray[1];
+        o[2] = ray[2];
+        out = 1;
+    }
+    const size_t at = (size_t)ly * P.width + lx;
+    if (!out) rays[3 * at] = rays[3 * at + 1] = rays[3 * at + 2] = 0.0f;
+    if (c.flag) {
+        const unsigned k = atomicAdd(nflagged, 1u);
+        if (k < flagged_cap) flagged[k] = (unsigned)at;
+    }
 }
 )KRN";
 
@@ -360,6 +388,14 @@ __global__ void scatter_entries_kernel(uint32_t *__restrict__ map, const RayPatc
     if (k < n) map[patches[k].pixel] = patches[k].entry;
 }
 
+// the rays the host evaluated, into the exported field (ray export)
+__global__ void scatter_rays_kernel(float *__restrict__ rays, const RaySample *__restrict__ samples, unsigned n) {
+    const unsigned k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const size_t at = samples[k].pixel;
+    for (int i = 0; i < 3; ++i) rays[3 * at + i] = samples[k].ray[i];
+}
+
 __global__ void __launch_bounds__(128) fwd_raster_kernel(const __grid_constant__ FwdGeom g, const FwdPoint *__restrict__ grid, FwdOut o,
                                                          const unsigned char *__restrict__ owner) {
     const int px = blockIdx.x * blockDim.x + threadIdx.x;
@@ -398,10 +434,12 @@ void LensDevice::drop_forward_state() {
 
 std::string LensDevice::kernel_tail(bool forward, bool globe_plate) {
     if (forward) return globe_plate ? std::string(kForwardKernelSource) + kForwardOwnerKernelSource : std::string(kForwardKernelSource);
-    const std::string head = std::string(kKernelParams) + kKernelHead + kKernelNormalize;
+    const std::string head = std::string(kKernelParams) + kKernelSignature + kKernelHead + kKernelNormalize;
     if (!globe_plate) return head + kKernelArgmax + kKernelTexel + kKernelEnd;
     return head + kKernelGlobePlateOpen + kKernelArgmax + "#endif\n" + kKernelTexel + kKernelGlobePlateClose + kKernelEnd;
 }
+
+std::string LensDevice::rays_tail() { return std::string(kKernelParams) + kRaysSignature + kKernelHead + kRaysEnd; }
 
 std::string LensDevice::raymap_tail(bool globe_plate) {
     const std::string head = std::string(kKernelParams) + kRaymapHead + kKernelNormalize;
@@ -458,13 +496,14 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
         *err = "CUDA driver entry points unavailable";
         return nullptr;
     }
-    const std::string cache_key = "IFR"[unit] + source;
+    const std::string cache_key = "IFRE"[unit] + source;
     auto it = cache_.find(cache_key);
     if (it != cache_.end()) return it->second;
     auto t0 = std::chrono::steady_clock::now();
     std::vector<char> cubin;
     std::string log;
     const bool compiled = unit == kRaymapUnit ? compile_unit(source + raymap_tail(source_has_globe_plate(source)), &cubin, &log)
+                          : unit == kRaysUnit ? compile_unit(source + rays_tail(), &cubin, &log)
                                               : compile(source, unit == kForwardUnit, &cubin, &log);
     if (!compiled) {
         *err = log;
@@ -473,7 +512,7 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
     cudaFree(nullptr);  // make sure the primary context is current
     Module *m = new Module;
     CUresult cr = d.ModuleLoadData(&m->mod, cubin.data());
-    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : "lt_build";
+    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : unit == kRaysUnit ? "lt_rays" : "lt_build";
     if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, entry);
     if (cr == CUDA_SUCCESS && unit == kForwardUnit && source_has_globe_plate(source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
     if (cr != CUDA_SUCCESS) {
@@ -656,6 +695,113 @@ bool LensDevice::copy_to_host(void *dst, const void *d_src, size_t bytes, void *
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
     if (ce != cudaSuccess) *err = std::string("copying the rays to the host: ") + cudaGetErrorString(ce);
     return ce == cudaSuccess;
+}
+
+bool LensDevice::copy_to_device(void *d_dst, const void *src, size_t bytes, void *stream, std::string *err) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    cudaError_t ce = cudaSetDevice(device_);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_dst, src, bytes, cudaMemcpyHostToDevice, s);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);  // (src is pageable host memory the copy may still read)
+    if (ce != cudaSuccess) *err = std::string("copying the rays to the device: ") + cudaGetErrorString(ce);
+    return ce == cudaSuccess;
+}
+
+bool LensDevice::capturing(void *stream) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    // an error (the legacy stream while another stream captures) counts as capturing: the call could not synchronise
+    return cudaStreamIsCapturing(static_cast<cudaStream_t>(stream), &st) != cudaSuccess || st != cudaStreamCaptureStatusNone;
+}
+
+bool LensDevice::rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
+                      std::string *err) {
+    kernel_ms_ = 0;
+    if (p.height > 65535) {   // one row of blocks per screen row, as lt_build
+        *err = "screen taller than 65535 rows, the device lens kernel's grid limit";
+        return false;
+    }
+    if (static_cast<size_t>(p.width) * p.height >= 0xFFFFFFFFull) {   // the flagged list holds 32-bit pixel numbers
+        *err = "screen of 2^32 pixels or more";
+        return false;
+    }
+    Module *m = module_for(lens_source, kRaysUnit, err);
+    if (!m) return false;
+    cudaError_t ce = cudaSuccess;
+    if (!ray_flagged_) ce = cudaMalloc(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned));
+    if (ce != cudaSuccess) {
+        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
+        return false;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    LensBuildParams params = p;
+    unsigned *count = ray_flagged_, *list = ray_flagged_ + 1;
+    unsigned cap = kUndecidedCap;
+    void *args[] = {&params, &d_rays, &list, &count, &cap};
+    const unsigned block = 128;
+    unsigned n = 0;
+    bool ok = true;
+    ce = cudaMemsetAsync(count, 0, sizeof(unsigned), s);
+    if (ce == cudaSuccess) {
+        cudaEventRecord(e0, s);
+        const CUresult cr = driver().LaunchKernel(m->fn, (p.width + block - 1) / block, static_cast<unsigned>(p.height), 1, block, 1, 1, 0, s, args, nullptr);
+        cudaEventRecord(e1, s);
+        if (cr != CUDA_SUCCESS) {
+            *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
+            ok = false;
+        }
+    }
+    if (ok) {
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&n, count, sizeof n, cudaMemcpyDeviceToHost, s);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+        if (ce != cudaSuccess) {
+            *err = std::string("ray export kernel: ") + cudaGetErrorString(ce);
+            ok = false;
+        }
+    }
+    if (ok && n > kUndecidedCap) {
+        *err = "too many pixels need the interpreter (" + std::to_string(n) + ")";
+        ok = false;
+    }
+    if (ok) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, e0, e1);
+        kernel_ms_ = ms;
+        ++launches_;
+        flagged->resize(n);
+        if (n) ce = cudaMemcpyAsync(flagged->data(), list, n * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
+        if (n && ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+        if (ce != cudaSuccess) {
+            *err = std::string("ray export flagged list: ") + cudaGetErrorString(ce);
+            ok = false;
+        }
+    }
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    return ok;
+}
+
+bool LensDevice::patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) {
+    if (samples.empty()) return true;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    RaySample *d_samples = nullptr;
+    cudaError_t ce = cudaMalloc(&d_samples, samples.size() * sizeof(RaySample));
+    if (ce == cudaSuccess) {
+        ce = cudaMemcpyAsync(d_samples, samples.data(), samples.size() * sizeof(RaySample), cudaMemcpyHostToDevice, s);
+        if (ce == cudaSuccess) {
+            const unsigned n = static_cast<unsigned>(samples.size());
+            scatter_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, d_samples, n);
+            ++launches_;
+            ce = cudaStreamSynchronize(s);  // (samples is pageable host memory the copy may still read)
+        }
+        cudaFree(d_samples);
+    }
+    if (ce != cudaSuccess) {
+        *err = std::string("ray export patch: ") + cudaGetErrorString(ce);
+        return false;
+    }
+    return true;
 }
 
 bool LensDevice::forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,

@@ -65,6 +65,12 @@ struct RayPatch {
     uint32_t entry;
 };
 
+// an exported ray the host evaluated: pixel number (ly * width + lx) and the narrowed, unnormalised ray
+struct RaySample {
+    uint32_t pixel;
+    float ray[3];
+};
+
 // True when a translated source defines lt_globe_plate (lua_transpile.h).
 inline bool source_has_globe_plate(const std::string &lens_source) { return lens_source.find("\n#define LT_HAS_GLOBE_PLATE 1\n") != std::string::npos; }
 
@@ -94,6 +100,14 @@ public:
                         std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) = 0;
     // writes the settled entries into that map on `stream`; returns once they are there
     virtual bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) = 0;
+    // ray export: lens_inverse's ray at each of the p.width * p.height pixels of a build at p.scale, narrowed to float and
+    // not normalised (zeros for nil), into d_rays (float32[height][width][3], device memory) on `stream` after the work
+    // already there.  lens_source: the lens translated alone.  *flagged receives the pixels whose ray is not provably
+    // the host's, for the host to evaluate; returns once the kernel has finished.
+    virtual bool rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
+                      std::string *err) = 0;
+    // writes the host's rays into that field on `stream`; returns once they are there
+    virtual bool patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) = 0;
 };
 
 class LensDevice : public DeviceLensBuilder {
@@ -112,8 +126,16 @@ public:
     bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
                 std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) override;
     bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) override;
+    bool rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
+              std::string *err) override;
+    bool patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) override;
     // bytes from device memory on `stream`, after the work already there (a ray map that takes the host path)
     bool copy_to_host(void *dst, const void *d_src, size_t bytes, void *stream, std::string *err);
+    // bytes to device memory on `stream`, after the work already there; returns once they are there (a ray export
+    // that takes the host path)
+    bool copy_to_device(void *d_dst, const void *src, size_t bytes, void *stream, std::string *err);
+    // true while `stream` (a cudaStream_t) is capturing a graph, or when that cannot be asked
+    static bool capturing(void *stream);
 
     // the fixed CUDA source appended to a translated lens (the per-pixel / per-grid-point tail);
     // exposed so that the CPU test-suite can run the very same text through a host shim.
@@ -122,6 +144,8 @@ public:
     static std::string kernel_tail(bool forward, bool globe_plate = false);
     // the same for the ray-map kernel, appended to the globe's translated globe_plate (or the bare prelude)
     static std::string raymap_tail(bool globe_plate);
+    // the same for the ray-export kernel, appended to the lens translated alone
+    static std::string rays_tail();
 
     // compile only (no GPU needed): used by the CPU test-suite and by build()
     static bool compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log);
@@ -133,7 +157,7 @@ public:
 private:
     struct Module;
     struct ForwardState;
-    enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit };
+    enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit, kRaysUnit };
     static bool compile_unit(const std::string &src, std::vector<char> *cubin, std::string *log);
     Module *module_for(const std::string &source, Unit unit, std::string *err);
     void drop_forward_state();

@@ -198,6 +198,36 @@ int blinky_set_lensmap_device(blinky_ctx *ctx, int width, int height, int plates
 int blinky_set_raymap(blinky_ctx *ctx, int width, int height, int platesize, const float *rays);
 int blinky_set_raymap_device(blinky_ctx *ctx, int width, int height, int platesize, const float *d_rays, void *stream);
 
+/* Ray export: the other half of a ray map.  Writes the view rays a width x height build of the current
+ * lens evaluates, in the layout blinky_set_raymap reads: float32[height][width][3], dense, ly = 0 the
+ * top row.  Pixel (lx, ly) gets lens_inverse((lx - width/2) * scale, -(ly - height/2) * scale), with
+ * integer /2 as in the build (fisheye.c:2100-2105) and scale what the current zoom gives for width x
+ * height; each component narrowed with static_cast<float> and NOT normalised; (0, 0, 0) where
+ * lens_inverse returns nil; NaN and infinities pass through the narrowing.  So for every inverse lens
+ * on every globe, with or without a rubix grid, blinky_set_raymap(width, height, platesize, rays) after
+ * an export installs the lensmap blinky_build_lensmap(width, height, platesize, ...) installs: the
+ * packed map, the display flags, the mapped count and the tile plan.  A head-tracked view exports once,
+ * turns the rays each frame (its own kernel) and sets them with blinky_set_raymap_device.  The loaded
+ * lens_inverse is evaluated; the lens script is not run again (the purity every threaded or device
+ * build assumes).  No globe is needed.  Nothing of the context changes: not the installed lensmap, its
+ * plan or generation, blinky_scale, blinky_width/height/platesize, blinky_needs_rebuild or the lens /
+ * globe / zoom change flags; blinky_build_info reports the export ("ray export, device: ..." or "ray
+ * export, host ...").  On failure the context does not change and the buffer's contents are
+ * unspecified: BLINKY_E_INVALID for NULL or misaligned rays or width / height <= 0; BLINKY_E_STATE
+ * without a valid lens or for a lens that maps with lens_forward (it has no per-pixel ray);
+ * BLINKY_E_ZOOM when the zoom cannot be computed (the build's console message is printed);
+ * BLINKY_E_SCRIPT when lens_inverse raises an error or returns anything but three numbers or one nil.
+ * blinky_get_raymap writes host memory on the worker threads and works on host-only contexts.
+ * blinky_get_raymap_device writes d_rays (4-byte aligned device memory) on `stream` (a cudaStream_t,
+ * NULL = the default stream) after the work already there, evaluating the translated lens on the GPU;
+ * pixels whose ray the GPU cannot prove equal to the interpreter's are evaluated by the interpreter and
+ * written in stream order.  When that is not possible (a lens outside the translatable subset, no
+ * NVRTC, too many such pixels) the rays are made on the host and copied to d_rays in stream order.  It
+ * returns once d_rays holds the complete field.  BLINKY_E_STATE while `stream` is capturing a graph
+ * (nothing is launched); BLINKY_E_NODEVICE on a host-only context. */
+int blinky_get_raymap(blinky_ctx *ctx, int width, int height, float *rays);
+int blinky_get_raymap_device(blinky_ctx *ctx, int width, int height, float *d_rays, void *stream);
+
 /* ---- state queries ------------------------------------------------------ */
 int blinky_fisheye_enabled(blinky_ctx *ctx);          /* fisheye_enabled, :293 */
 int blinky_lens_valid(blinky_ctx *ctx);
@@ -246,7 +276,9 @@ int blinky_globe_plate(blinky_ctx *ctx, double x, double y, double z, int *plate
  * exactly what NVRTC is given.  bit 3 = the globe's globe_plate translated alone (bit 0 still picks
  * CUDA; bits 1 and 2 are ignored).  bit 4 = the ray-map unit of blinky_set_raymap_device: the globe's
  * globe_plate translated alone (nothing for globes without one) and the ray-map kernel; with bit 0
- * this is exactly what NVRTC is given (bits 1 to 3 are ignored).  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT
+ * this is exactly what NVRTC is given (bits 1 to 3 are ignored).  bit 5 = the ray-export unit of
+ * blinky_get_raymap_device: lens_inverse translated alone and the ray-export kernel; with bit 0 this is
+ * exactly what NVRTC is given (bits 1 to 4 are ignored).  Returns the bytes needed (excluding NUL), or BLINKY_E_SCRIPT
  * when the lens (or globe_plate) is missing or outside the translatable subset (reason:
  * blinky_last_error). */
 int blinky_lens_source(blinky_ctx *ctx, int flavour, char *buf, size_t bufsize);
