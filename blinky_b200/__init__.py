@@ -69,6 +69,7 @@ _SIGNATURES = [
     ("blinky_plan_digest", ctypes.c_uint64, [_CTX, c_int]),
     ("blinky_get_tile_plan", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
     ("blinky_compile_lens", c_int, [_CTX, c_int, POINTER(c_size_t)]),
+    ("blinky_probe_math", c_int, [_CTX, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("blinky_fisheye_enabled", c_int, [_CTX]),
     ("blinky_lens_valid", c_int, [_CTX]),
     ("blinky_globe_valid", c_int, [_CTX]),
@@ -347,6 +348,30 @@ class Fisheye:
         n = c_size_t()
         self._check(self._lib.blinky_compile_lens(self._ctx, int(forward), ctypes.byref(n)))
         return n.value
+
+    # blinky_probe_math's ops, in BLINKY_PROBE_* order
+    PROBE_OPS = ("sin", "cos", "tan", "asin", "acos", "atan", "atan2", "exp", "log", "log10", "logb", "sinh", "cosh", "tanh", "pow",
+                 "sqrt", "fmod", "floor", "ceil", "trunc", "modf", "div", "f32", "int")
+    PROBE_BINARY = ("atan2", "logb", "pow", "fmod", "div")
+
+    def probe_math(self, op: str, a=None, b=None, stream: int | None = None):
+        """Test hook (blinky_probe_math): the translated lenses' wrapper for `op` (a PROBE_OPS name) on the GPU, as every
+        lens unit compiles it.  a, b: contiguous CUDA float64 tensors of one length (b only for PROBE_BINARY ops).
+        Returns (value, bound) as new CUDA float64 tensors, complete on return; modf gives (fractional part, integral
+        part).  a=None only compiles the unit (works without a GPU)."""
+        code = self.PROBE_OPS.index(op)
+        if a is None:
+            self._check(self._lib.blinky_probe_math(self._ctx, code, None, None, None, None, 0, None))
+            return None
+        import torch
+        for t in (a,) + ((b,) if op in self.PROBE_BINARY else ()):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.is_contiguous() and t.shape == a.shape):
+                raise ValueError("probe_math: expected contiguous CUDA float64 tensors of one shape")
+        v, e = torch.empty_like(a), torch.empty_like(a)
+        if a.numel():
+            self._check(self._lib.blinky_probe_math(self._ctx, code, a.data_ptr(), b.data_ptr() if op in self.PROBE_BINARY else None,
+                                                    v.data_ptr(), e.data_ptr(), a.numel(), stream))
+        return v, e
 
     def needs_rebuild(self, width: int, height: int, platesize: int = 0) -> bool:
         return bool(self._lib.blinky_needs_rebuild(self._ctx, width, height, platesize))

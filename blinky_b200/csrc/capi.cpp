@@ -16,6 +16,7 @@
 
 #include "fisheye_host.h"
 #include "lens_device.h"
+#include "lua_transpile.h"
 #include "shard.h"
 #include "tile_plan.h"
 #include "tile_plan_device.h"
@@ -350,6 +351,26 @@ int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes) {
     if (!LensDevice::compile(src, forward != 0, &cubin, &log)) return set_err(ctx, BLINKY_E_CUDA, log);
     if (cubin_bytes) *cubin_bytes = cubin.size();
     return BLINKY_OK;
+}
+
+int blinky_probe_math(blinky_ctx *ctx, int op, const double *d_a, const double *d_b, double *d_v, double *d_e, size_t n, void *stream) {
+    const bool binary = op == BLINKY_PROBE_ATAN2 || op == BLINKY_PROBE_LOGB || op == BLINKY_PROBE_POW || op == BLINKY_PROBE_FMOD ||
+                        op == BLINKY_PROBE_DIV;
+    if (op < 0 || op >= BLINKY_PROBE_COUNT) return set_err(ctx, BLINKY_E_INVALID, "blinky_probe_math: unknown op");
+    const std::string prelude = blinky::transpile_prelude(true, false);
+    if (n == 0) {
+        std::vector<char> cubin;
+        std::string log;
+        return LensDevice::compile_unit(prelude + LensDevice::probe_tail(), &cubin, &log) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, log);
+    }
+    if (!ctx->lens_dev) return set_err(ctx, BLINKY_E_NODEVICE, "blinky_probe_math: this context has no GPU");
+    for (const void *p : {static_cast<const void *>(d_a), static_cast<const void *>(d_v), static_cast<const void *>(d_e),
+                          binary ? static_cast<const void *>(d_b) : static_cast<const void *>(d_a)})
+        if (!p || reinterpret_cast<uintptr_t>(p) % 8 != 0)
+            return set_err(ctx, BLINKY_E_INVALID, "blinky_probe_math: arguments and results must be non-NULL, 8-byte aligned pointers");
+    if (LensDevice::capturing(stream)) return set_err(ctx, BLINKY_E_STATE, "blinky_probe_math: the stream is capturing a graph");
+    std::string why;
+    return ctx->lens_dev->probe_math(prelude, op, d_a, d_b, d_v, d_e, n, stream, &why) ? BLINKY_OK : set_err(ctx, BLINKY_E_CUDA, why);
 }
 
 int blinky_needs_rebuild(blinky_ctx *ctx, int w, int h, int ps) { return ctx->host.needs_rebuild(w, h, ps) ? 1 : 0; }

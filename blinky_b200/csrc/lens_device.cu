@@ -172,6 +172,47 @@ const char *kRaysEnd = R"KRN(        float *o = rays + 3 * ((size_t)ly * P.width
 }
 )KRN";
 
+// The math probe (blinky_probe_math, a test hook): one prelude wrapper or IEEE operation per launch, on exact
+// arguments a[i] (and b[i] for the binary ones), with the prelude's value and bound.  The op numbers are
+// BLINKY_PROBE_* in blinky_b200.h; modf's integral part goes to e.
+const char *kProbeSource = R"KRN(
+extern "C" __global__ void __launch_bounds__(256) lt_probe(int op, const double *__restrict__ a, const double *__restrict__ b,
+                                                           double *__restrict__ v, double *__restrict__ e, unsigned long long n) {
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const LtD x(a[i]);
+    LtD r(0.0);
+    switch (op) {
+        case 0: r = lt_sin(x); break;
+        case 1: r = lt_cos(x); break;
+        case 2: r = lt_tan(x); break;
+        case 3: r = lt_asin(x); break;
+        case 4: r = lt_acos(x); break;
+        case 5: r = lt_atan(x); break;
+        case 6: r = lt_atan2(x, LtD(b[i])); break;
+        case 7: r = lt_exp(x); break;
+        case 8: r = lt_log(x); break;
+        case 9: r = lt_log10(x); break;
+        case 10: r = lt_logb(x, LtD(b[i])); break;
+        case 11: r = lt_sinh(x); break;
+        case 12: r = lt_cosh(x); break;
+        case 13: r = lt_tanh(x); break;
+        case 14: r = lt_pow(x, LtD(b[i])); break;
+        case 15: r = LtD(sqrt(x.v)); break;
+        case 16: r = LtD(fmod(x.v, b[i])); break;
+        case 17: r = LtD(floor(x.v)); break;
+        case 18: r = LtD(ceil(x.v)); break;
+        case 19: r = LtD(trunc(x.v)); break;
+        case 20: { double ip; const double f = modf(x.v, &ip); r = LtD(f, ip); break; }
+        case 21: r = LtD(x.v / b[i]); break;
+        case 22: r = LtD((double)(float)x.v); break;
+        case 23: r = LtD((double)(int)x.v); break;
+    }
+    v[i] = r.v;
+    e[i] = r.e;
+}
+)KRN";
+
 // Forward builder, step 1 (fisheye.c:2227-2243 uv_to_screen over the grid of fisheye.c:2151-2189):
 // grid point (plate, j, i) sits at u = (i - 0.5)/ps, v = (j - 0.5)/ps.
 const char *kForwardKernelSource = R"KRN(
@@ -441,6 +482,8 @@ std::string LensDevice::kernel_tail(bool forward, bool globe_plate) {
 
 std::string LensDevice::rays_tail() { return std::string(kKernelParams) + kRaysSignature + kKernelHead + kRaysEnd; }
 
+std::string LensDevice::probe_tail() { return kProbeSource; }
+
 std::string LensDevice::raymap_tail(bool globe_plate) {
     const std::string head = std::string(kKernelParams) + kRaymapHead + kKernelNormalize;
     if (!globe_plate) return head + kKernelArgmax + kKernelTexel + kRaymapEnd;
@@ -496,7 +539,7 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
         *err = "CUDA driver entry points unavailable";
         return nullptr;
     }
-    const std::string cache_key = "IFRE"[unit] + source;
+    const std::string cache_key = "IFREP"[unit] + source;
     auto it = cache_.find(cache_key);
     if (it != cache_.end()) return it->second;
     auto t0 = std::chrono::steady_clock::now();
@@ -504,6 +547,7 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
     std::string log;
     const bool compiled = unit == kRaymapUnit ? compile_unit(source + raymap_tail(source_has_globe_plate(source)), &cubin, &log)
                           : unit == kRaysUnit ? compile_unit(source + rays_tail(), &cubin, &log)
+                          : unit == kProbeUnit ? compile_unit(source + probe_tail(), &cubin, &log)
                                               : compile(source, unit == kForwardUnit, &cubin, &log);
     if (!compiled) {
         *err = log;
@@ -512,7 +556,8 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
     cudaFree(nullptr);  // make sure the primary context is current
     Module *m = new Module;
     CUresult cr = d.ModuleLoadData(&m->mod, cubin.data());
-    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : unit == kRaysUnit ? "lt_rays" : "lt_build";
+    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : unit == kRaysUnit ? "lt_rays"
+                        : unit == kProbeUnit ? "lt_probe" : "lt_build";
     if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, entry);
     if (cr == CUDA_SUCCESS && unit == kForwardUnit && source_has_globe_plate(source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
     if (cr != CUDA_SUCCESS) {
@@ -710,6 +755,25 @@ bool LensDevice::capturing(void *stream) {
     cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
     // an error (the legacy stream while another stream captures) counts as capturing: the call could not synchronise
     return cudaStreamIsCapturing(static_cast<cudaStream_t>(stream), &st) != cudaSuccess || st != cudaStreamCaptureStatusNone;
+}
+
+bool LensDevice::probe_math(const std::string &prelude, int op, const double *d_a, const double *d_b, double *d_v, double *d_e, size_t n,
+                            void *stream, std::string *err) {
+    Module *m = module_for(prelude, kProbeUnit, err);
+    if (!m) return false;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    unsigned long long count = n;
+    void *args[] = {&op, &d_a, &d_b, &d_v, &d_e, &count};
+    const unsigned block = 256;
+    const CUresult cr = driver().LaunchKernel(m->fn, static_cast<unsigned>((n + block - 1) / block), 1, 1, block, 1, 1, 0, s, args, nullptr);
+    if (cr != CUDA_SUCCESS) {
+        *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
+        return false;
+    }
+    ++launches_;
+    const cudaError_t ce = cudaStreamSynchronize(s);
+    if (ce != cudaSuccess) *err = std::string("math probe: ") + cudaGetErrorString(ce);
+    return ce == cudaSuccess;
 }
 
 bool LensDevice::rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,

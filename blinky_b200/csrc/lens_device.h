@@ -146,9 +146,19 @@ public:
     static std::string raymap_tail(bool globe_plate);
     // the same for the ray-export kernel, appended to the lens translated alone
     static std::string rays_tail();
+    // the math probe kernel (blinky_probe_math), appended to the bare prelude
+    static std::string probe_tail();
+
+    // test hook: one prelude wrapper or IEEE operation (BLINKY_PROBE_*) on n exact arguments in device memory, value
+    // and bound into d_v and d_e, on `stream` after the work already there; returns once they are written.
+    // prelude: transpile_prelude(true), the text every lens unit starts with.
+    bool probe_math(const std::string &prelude, int op, const double *d_a, const double *d_b, double *d_v, double *d_e, size_t n,
+                    void *stream, std::string *err);
 
     // compile only (no GPU needed): used by the CPU test-suite and by build()
     static bool compile(const std::string &lens_source, bool forward, std::vector<char> *cubin, std::string *log);
+    // a complete unit, with the NVRTC options of every lens unit (no GPU needed)
+    static bool compile_unit(const std::string &src, std::vector<char> *cubin, std::string *log);
 
     double last_compile_ms() const { return compile_ms_; }
     double last_kernel_ms() const { return kernel_ms_; }
@@ -157,8 +167,7 @@ public:
 private:
     struct Module;
     struct ForwardState;
-    enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit, kRaysUnit };
-    static bool compile_unit(const std::string &src, std::vector<char> *cubin, std::string *log);
+    enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit, kRaysUnit, kProbeUnit };
     Module *module_for(const std::string &source, Unit unit, std::string *err);
     void drop_forward_state();
     int device_;

@@ -1077,8 +1077,10 @@ std::string transpile_prelude(bool cuda, bool noinline_user_functions) {
 #define LT_RISK_F32 32u     /* a value sits on a float32 rounding boundary */
 #define LT_MAX_MUT 32
 
-/* A double that went through a libm function, with a first-order bound `e` on
- * |value computed here - value the host's libm would give|.  e == 0: provably identical. */
+/* A double that went through a libm function, with a bound `e` on |value computed here - value the
+ * host's libm would give| that holds to all orders: every rule below bounds the change of its function
+ * over the whole input interval [v - e, v + e] (box, for two operands), and gives an infinite bound
+ * when that interval reaches a pole, a domain edge or a NaN region.  e == 0: provably identical. */
 struct LtD {
     double v, e;
     LT_HD LtD() {}
@@ -1087,6 +1089,7 @@ struct LtD {
 };
 #define LT_U 0x1p-52            /* one rounding */
 #define LT_KU (8.0 * LT_U)      /* libm results: CUDA <= 2 ulp + glibc <= 2 ulp (documented), doubled */
+#define LT_FINITE(x) (fabs(x) <= 1.79769313486231570815e308)
 
 struct LtPlate { float forward[3], right[3], up[3]; float dist; };
 
@@ -1106,56 +1109,112 @@ LT_FN LtD lt_fn(double r, double prop) {
     if (prop == 0.0 && !(fabs(r) <= 1.79769313486231570815e308)) return LtD(r);
     return LtD(r, prop + LT_KU * fabs(r));
 }
+/* result r of exp, sinh, cosh, pow or atan2, whose finite arguments can put it at a range edge where LT_KU * |r|
+ * says nothing: within a few ulp of the overflow threshold one libm may give the largest double and the other inf,
+ * and below the normal range (an ulp is 2^-1074 there) one may give 0 and the other a subnormal.  edge: the
+ * arguments are finite and not ones that make the result exact (sinh(0), pow(0, y), atan2(0, x), ...) */
+LT_FN LtD lt_fn_edge(double r, double prop, bool edge) {
+    if (edge && fabs(r) < 0x1p-1022) return LtD(r, prop + LT_KU * 0x1p-1022);
+    if (edge && fabs(r) > 0x1.ffffffffffff0p1023) return LtD(r, LT_INF);
+    return lt_fn(r, prop);
+}
+/* exp(e) - 1 <= e / (1 - e) for 0 <= e < 1: the relative change of exp over [v - e, v + e] */
+LT_FN double lt_expm1_bound(double e) { return e < 1.0 ? e / (1.0 - e) : LT_INF; }
 
 LT_FN LtD operator+(LtD a, LtD b) { return lt_mk(a.v + b.v, a.e + b.e); }
 LT_FN LtD operator-(LtD a, LtD b) { return lt_mk(a.v - b.v, a.e + b.e); }
 LT_FN LtD operator*(LtD a, LtD b) {
     const double r = a.v * b.v;
     if (a.e == 0.0 && b.e == 0.0) return LtD(r);
-    return lt_mk(r, fabs(a.v) * b.e + fabs(b.v) * a.e);
+    return lt_mk(r, fabs(a.v) * b.e + fabs(b.v) * a.e + a.e * b.e);
 }
 LT_FN LtD operator/(LtD a, LtD b) {
     const double r = a.v / b.v;
     if (a.e == 0.0 && b.e == 0.0) return LtD(r);
-    return lt_mk(r, (a.e + fabs(r) * b.e) / fabs(b.v));
+    /* |a'/b' - a/b| <= (a.e + |a/b| b.e) / (|b| - b.e); unbounded once the divisor's interval reaches 0 */
+    const double d = fabs(b.v) - b.e;
+    return lt_mk(r, d > 0.0 ? (a.e + fabs(r) * b.e) / d : LT_INF);
 }
 LT_FN LtD operator-(LtD a) { return LtD(-a.v, a.e); }
 LT_FN LtD lt_fabs(LtD a) { return LtD(fabs(a.v), a.e); }
 LT_FN LtD lt_sqrt(LtD a) {
     const double r = sqrt(a.v);
     if (a.e == 0.0) return LtD(r);
-    return lt_mk(r, a.e / (2.0 * r));
+    /* sqrt(v) - sqrt(v - e) = e / (r + sqrt(v - e)) <= e / (2r - e/r), as sqrt(1 - t) >= 1 - t; NaN below 0 */
+    return lt_mk(r, a.e < a.v ? a.e / (2.0 * r - a.e / r) : LT_INF);
 }
 LT_FN LtD lt_sin(LtD a) { return lt_fn(sin(a.v), a.e); }
 LT_FN LtD lt_cos(LtD a) { return lt_fn(cos(a.v), a.e); }
-LT_FN LtD lt_tan(LtD a) { const double r = tan(a.v); return lt_fn(r, (1.0 + r * r) * a.e); }
-LT_FN LtD lt_asin(LtD a) { return lt_fn(asin(a.v), a.e == 0.0 ? 0.0 : a.e / sqrt(fmax(1.0 - a.v * a.v, 0.0))); }
-LT_FN LtD lt_acos(LtD a) { return lt_fn(acos(a.v), a.e == 0.0 ? 0.0 : a.e / sqrt(fmax(1.0 - a.v * a.v, 0.0))); }
-LT_FN LtD lt_atan(LtD a) { return lt_fn(atan(a.v), a.e / (1.0 + a.v * a.v)); }
+LT_FN LtD lt_tan(LtD a) {
+    const double r = tan(a.v);
+    if (a.e == 0.0) return lt_fn(r, 0.0);
+    /* tan(v + s) - tan(v) = (1 + r^2) tan(s) / (1 - r tan(s)), and tan(s) <= s / (1 - s^2/2) for s < sqrt(2);
+     * the denominator reaching 0 means the interval reaches a pole */
+    const double t = a.e * a.e < 2.0 ? a.e / (1.0 - 0.5 * a.e * a.e) : LT_INF;
+    const double d = 1.0 - fabs(r) * t;
+    return lt_fn(r, d > 0.0 ? (1.0 + r * r) * t / d : LT_INF);
+}
+/* asin, acos: the derivative at the end of the interval nearer +-1; NaN beyond */
+LT_FN double lt_asin_bound(LtD a) {
+    const double m = fabs(a.v) + a.e;
+    return a.e == 0.0 ? 0.0 : m < 1.0 ? a.e / sqrt((1.0 - m) * (1.0 + m)) : LT_INF;
+}
+LT_FN LtD lt_asin(LtD a) { return lt_fn(asin(a.v), lt_asin_bound(a)); }
+LT_FN LtD lt_acos(LtD a) { return lt_fn(acos(a.v), lt_asin_bound(a)); }
+LT_FN LtD lt_atan(LtD a) {
+    const double m = fmax(fabs(a.v) - a.e, 0.0);   /* the derivative at the end of the interval nearer 0 */
+    return lt_fn(atan(a.v), a.e / (1.0 + m * m));
+}
 LT_FN LtD lt_atan2(LtD y, LtD x) {
     const double r = atan2(y.v, x.v);
-    if (y.e == 0.0 && x.e == 0.0) return lt_fn(r, 0.0);
-    return lt_fn(r, (fabs(x.v) * y.e + fabs(y.v) * x.e) / (x.v * x.v + y.v * y.v));
+    const bool edge = y.v != 0.0 && LT_FINITE(y.v) && LT_FINITE(x.v);   /* atan2(tiny, huge) underflows */
+    if (y.e == 0.0 && x.e == 0.0) return lt_fn_edge(r, 0.0, edge);
+    /* along a path inside the error box, |d atan2| = |x dy - y dx| / (x^2 + y^2), the box's nearest point to the
+     * origin bounding the denominator; a box holding the origin, or one that can move y across 0 where x < 0
+     * (atan2 jumps by 2 pi there), has no bound */
+    const double dy = fmax(fabs(y.v) - y.e, 0.0), dx = fmax(fabs(x.v) - x.e, 0.0);
+    const bool jump = dy == 0.0 && (dx == 0.0 || (y.e > 0.0 && x.v - x.e < 0.0));
+    return lt_fn_edge(r, jump ? LT_INF : (fabs(x.v) * y.e + fabs(y.v) * x.e + 2.0 * x.e * y.e) / (dx * dx + dy * dy), edge);
 }
-LT_FN LtD lt_exp(LtD a) { const double r = exp(a.v); return lt_fn(r, a.e == 0.0 ? 0.0 : r * a.e); }
-LT_FN LtD lt_log(LtD a) { return lt_fn(log(a.v), a.e == 0.0 ? 0.0 : a.e / fabs(a.v)); }
-LT_FN LtD lt_log10(LtD a) { return lt_fn(log10(a.v), a.e == 0.0 ? 0.0 : a.e / (fabs(a.v) * 2.302585092994046)); }
+LT_FN LtD lt_exp(LtD a) {
+    const double r = exp(a.v);
+    return lt_fn_edge(r, a.e == 0.0 ? 0.0 : r * lt_expm1_bound(a.e), LT_FINITE(a.v));
+}
+/* log(v) - log(v - e) = -log(1 - t) <= t / (1 - t), t = e / v; unbounded once the interval reaches 0 */
+LT_FN double lt_log_bound(LtD a) {
+    const double t = a.e / fabs(a.v);
+    return a.e == 0.0 ? 0.0 : t < 1.0 ? t / (1.0 - t) : LT_INF;
+}
+LT_FN LtD lt_log(LtD a) { return lt_fn(log(a.v), lt_log_bound(a)); }
+LT_FN LtD lt_log10(LtD a) { return lt_fn(log10(a.v), lt_log_bound(a) / 2.302585092994046); }
 LT_FN LtD lt_logb(LtD x, LtD base) {   /* lmathlib.c math_log with a base */
     if (base.e == 0.0 && base.v == 10.0) return lt_log10(x);
     return lt_log(x) / lt_log(base);
 }
-LT_FN LtD lt_sinh(LtD a) { const double r = sinh(a.v); return lt_fn(r, a.e == 0.0 ? 0.0 : (fabs(r) + 1.0) * a.e); }
-LT_FN LtD lt_cosh(LtD a) { const double r = cosh(a.v); return lt_fn(r, a.e == 0.0 ? 0.0 : r * a.e); }
+/* sinh(v + s) - sinh(v) = sinh(v) (cosh(s) - 1) + cosh(v) sinh(s), cosh(v) <= |r| + 1: at most (|r| + 1) (exp(e) - 1) */
+LT_FN LtD lt_sinh(LtD a) {
+    const double r = sinh(a.v);
+    return lt_fn_edge(r, a.e == 0.0 ? 0.0 : (fabs(r) + 1.0) * lt_expm1_bound(a.e), a.v != 0.0 && LT_FINITE(a.v));
+}
+LT_FN LtD lt_cosh(LtD a) {
+    const double r = cosh(a.v);
+    return lt_fn_edge(r, a.e == 0.0 ? 0.0 : r * lt_expm1_bound(a.e), LT_FINITE(a.v));
+}
 LT_FN LtD lt_tanh(LtD a) { return lt_fn(tanh(a.v), a.e); }
 LT_FN LtD lt_pow(LtD a, LtD b) {
     const double r = pow(a.v, b.v);
-    if (a.e == 0.0 && b.e == 0.0) return lt_fn(r, 0.0);
-    if (b.e == 0.0) {   /* exact exponent (x^2, x^0.5, ...): d(a^b) = b a^(b-1) da, any sign of a */
-        if (a.v != 0.0) return lt_fn(r, fabs(r * b.v / a.v) * a.e);
-        return lt_fn(r, b.v > 0.0 ? pow(a.e, b.v) : LT_INF);
-    }
-    /* d(a^b) = a^b (b/a da + ln a db); outside a > 0 the bound turns NaN/inf and flags */
-    return lt_fn(r, fabs(r) * (fabs(b.v / a.v) * a.e + fabs(log(a.v)) * b.e));
+    const bool edge = a.v != 0.0 && LT_FINITE(a.v) && LT_FINITE(b.v);
+    if (a.e == 0.0 && b.e == 0.0) return lt_fn_edge(r, 0.0, edge);
+    const bool int_b = b.e == 0.0 && b.v == floor(b.v);
+    if (a.v == 0.0)   /* |a'^b| <= a.e^b for a positive exponent; a negative base gives NaN unless b is an integer */
+        return lt_fn(r, b.e == 0.0 && b.v > 0.0 && int_b ? pow(a.e, b.v) : LT_INF);
+    /* a'^b' = r exp(b (log a' - log a) + (b' - b) log a'), |log a' - log a| <= l = t / (1 - t), t = a.e / |a|: the
+     * base keeps its sign (only an integer exponent is defined for a negative one), then |exp(w) - 1| <= z / (1 - z) */
+    const double t = a.e / fabs(a.v);
+    if (!(t < 1.0) || (b.e != 0.0 && !(a.v > 0.0))) return lt_fn(r, LT_INF);
+    const double l = t / (1.0 - t);
+    const double z = fabs(b.v) * l + (b.e == 0.0 ? 0.0 : b.e * (fabs(log(a.v)) + l));
+    return lt_fn_edge(r, fabs(r) * lt_expm1_bound(z), edge);
 }
 
 /* ---- decisions: flag when the outcome is not certain within the bounds (x2 safety) ---- */

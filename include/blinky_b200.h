@@ -141,6 +141,32 @@ const char *blinky_build_info(blinky_ctx *ctx);
 /* Translate + NVRTC-compile the current lens_inverse (forward = 0) or lens_forward (forward = 1)
  * kernel without running it (works without a GPU). */
 int blinky_compile_lens(blinky_ctx *ctx, int forward, size_t *cubin_bytes);
+/* Test hook, not for applications: runs one of the translated lenses' math wrappers on the GPU, as every
+ * lens unit compiles it (the same prelude text, NVRTC and options), so a test can hold the device's
+ * libm and the error bound the prelude charges against the host's libm.  For i < n: v[i] and e[i] are
+ * the value and the bound of op on the exact arguments a[i] (and b[i] for the two-argument ops; d_b may
+ * be NULL otherwise).  For the IEEE operations e[i] is 0, except BLINKY_PROBE_MODF, which writes the
+ * fractional part to v and the integral part to e.  d_a, d_b, d_v, d_e: 8-byte aligned device memory,
+ * read and written on `stream` (a cudaStream_t, NULL = the default stream) after the work already there;
+ * the call returns once the results are written.  n = 0 only compiles the unit (no GPU needed; also on
+ * host-only contexts).  BLINKY_E_INVALID for an unknown op or a NULL / misaligned pointer, BLINKY_E_STATE
+ * while `stream` is capturing a graph, BLINKY_E_NODEVICE for n > 0 on a host-only context, BLINKY_E_CUDA
+ * when NVRTC is missing or the unit does not compile. */
+enum {
+    BLINKY_PROBE_SIN = 0, BLINKY_PROBE_COS, BLINKY_PROBE_TAN, BLINKY_PROBE_ASIN, BLINKY_PROBE_ACOS, BLINKY_PROBE_ATAN,
+    BLINKY_PROBE_ATAN2,   /* atan2(a, b) */
+    BLINKY_PROBE_EXP, BLINKY_PROBE_LOG, BLINKY_PROBE_LOG10,
+    BLINKY_PROBE_LOGB,    /* Lua's math.log(a, b) */
+    BLINKY_PROBE_SINH, BLINKY_PROBE_COSH, BLINKY_PROBE_TANH,
+    BLINKY_PROBE_POW,     /* pow(a, b) */
+    /* the operations the device computes exactly as the host does (IEEE) */
+    BLINKY_PROBE_SQRT, BLINKY_PROBE_FMOD, BLINKY_PROBE_FLOOR, BLINKY_PROBE_CEIL, BLINKY_PROBE_TRUNC, BLINKY_PROBE_MODF,
+    BLINKY_PROBE_DIV,     /* a / b */
+    BLINKY_PROBE_F32,     /* (double)(float)a */
+    BLINKY_PROBE_INT,     /* (double)(int)a, for a in int range */
+    BLINKY_PROBE_COUNT
+};
+int blinky_probe_math(blinky_ctx *ctx, int op, const double *d_a, const double *d_b, double *d_v, double *d_e, size_t n, void *stream);
 /* 1 if a lens/globe/zoom/rubixgrid/size change since the last build requires a rebuild (:730) */
 int blinky_needs_rebuild(blinky_ctx *ctx, int width, int height, int platesize);
 

@@ -378,14 +378,37 @@ PERTURBED_LT_FN = """LT_FN LtD lt_fn(double r, double prop) {
 }"""
 
 
+EXACT_LT_FN_EDGE = """LT_FN LtD lt_fn_edge(double r, double prop, bool edge) {
+    if (edge && fabs(r) < 0x1p-1022) return LtD(r, prop + LT_KU * 0x1p-1022);
+    if (edge && fabs(r) > 0x1.ffffffffffff0p1023) return LtD(r, LT_INF);
+    return lt_fn(r, prop);
+}"""
+
+# the range edges as another libm may round them: an underflowed 0 becomes the smallest subnormal, a subnormal moves
+# by up to 3 of its ulps, and an overflowed inf becomes the largest double (lt_fn moves every other result)
+PERTURBED_LT_FN_EDGE = """LT_FN LtD lt_fn_edge(double r, double prop, bool edge) {
+    if (edge && fabs(r) < 0x1p-1022) {
+        union { double d; unsigned long long u; } b;
+        b.d = r;
+        const unsigned long long h = (b.u ^ (b.u >> 29)) * 0x9E3779B97F4A7C15ull;
+        const long long k = (long long)((h >> 40) % 4ull);   /* 0 .. 3 ulp of 2^-1074 away from 0 */
+        b.u = (b.u & 0x8000000000000000ull) | ((b.u & 0x7FFFFFFFFFFFFFFFull) + k);
+        if (r == 0.0) b.u |= 1ull;
+        return LtD(b.d, prop + LT_KU * 0x1p-1022);
+    }
+    if (edge && fabs(r) > 0x1.ffffffffffff0p1023) return LtD(fabs(r) > 1.79769313486231570815e308 ? copysign(1.79769313486231570815e308, r) : r, LT_INF);
+    return lt_fn(r, prop);
+}"""
+
+
 def perturbed(src, scale=1):
     """scale > 1 magnifies both the libm disagreement and the per-call bound by the same factor: the
-    propagation rules are first order, so they must hold at any (small) scale, and at 2^20 ulp the rare
+    propagation rules hold to all orders, so they must hold at any scale, and at 2^20 ulp the rare
     events (a float32 rounding boundary inside the error interval) become frequent enough to be tested."""
-    assert EXACT_LT_FN in src, "lt_fn changed: update the test's copy"
+    assert EXACT_LT_FN in src and EXACT_LT_FN_EDGE in src, "lt_fn / lt_fn_edge changed: update the test's copy"
     assert "#define LT_KU (8.0 * LT_U)" in src
     src = src.replace("#define LT_KU (8.0 * LT_U)", f"#define PERT_SCALE {scale}LL\n#define LT_KU (8.0 * PERT_SCALE * LT_U)")
-    return src.replace(EXACT_LT_FN, PERTURBED_LT_FN)
+    return src.replace(EXACT_LT_FN, PERTURBED_LT_FN).replace(EXACT_LT_FN_EDGE, PERTURBED_LT_FN_EDGE)
 
 
 def f32bits(vals):
@@ -418,3 +441,31 @@ def test_error_bounds_are_sound_under_a_different_libm(host, tmp_path, lens, sca
     pts = _points(2500)
     decided = check_bounds_sound(host, lib, pts, (lens, scale))
     assert decided >= (0.4 if scale == 1 else 0.05) * len(pts), (lens, scale, decided, len(pts))
+
+
+EDGES = """
+function lens_inverse(x, y)
+  local t = math.exp(x * 200 - 745)      -- 0, a subnormal or a normal number around x = 0
+  local s = math.exp(709.78 + y * 0.01)  -- finite below y = 0.27, inf above
+  local p = 2 ^ (1023.99 + x * 0.01)     -- the same for pow
+  local lat, lon = y * 0.3, x * 0.3
+  if t > 0 then lon = lon + 0.1 end
+  if s < math.huge then lat = lat - 0.05 end
+  if p == math.huge then lon = lon - 0.2 end
+  return latlon_to_ray(lat, lon)
+end"""
+
+
+@pytest.mark.parametrize("scale", [1, 1 << 20])
+def test_error_bounds_are_sound_at_the_range_edges(host, tmp_path, scale):
+    """exp and pow at their underflow and overflow thresholds, where another libm may give 0 for a subnormal or inf
+    for the largest double: the perturbed build moves those results too, and every decision it leaves unflagged must
+    still be the interpreter's"""
+    host.command("f_globe cube")
+    host.load_lens("edges", EDGES)
+    lib = _compile_host(perturbed(host.lens_source(cuda=False), scale), str(tmp_path / f"edges{scale}"))
+    xs = np.concatenate([np.linspace(-0.05, 0.3, 71), [-4.0, -1.0, 1.0, 4.0]])
+    ys = np.concatenate([np.linspace(0.2, 0.35, 61), [-3.0, 0.0, 3.0]])
+    pts = [(x, y) for x in xs for y in ys]
+    decided = check_bounds_sound(host, lib, pts, ("edges", scale))
+    assert decided >= (0.3 if scale == 1 else 0.1) * len(pts), (scale, decided, len(pts))
