@@ -111,6 +111,10 @@ _SIGNATURES = [
     ("blinky_warp_device_view_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     ("blinky_warp_device_view_rgba_tables", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int,
                                                     c_void_p, c_size_t, c_void_p]),
+    ("blinky_warp_device_rays", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int,
+                                        c_int, c_int, c_void_p]),
+    ("blinky_warp_device_rays_rgba", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int,
+                                             c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_host", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int]),
     ("blinky_upload_bytes_per_frame", c_int64, [_CTX]),
     ("blinky_alloc_pinned", c_int, [_CTX, c_size_t, POINTER(c_void_p)]),
@@ -595,6 +599,57 @@ class Fisheye:
         fn = self._lib.blinky_warp_device_view_rgba if rgba else self._lib.blinky_warp_device_view
         self._check(fn(self._ctx, _ptr(d_faces), face_stride, _ptr(d_screen), screen_stride, rowbytes, x0, y0, nframes,
                        1 if keep_unmapped else 0, _warp_stream(stream)))
+
+    def warp_rays(self, d_faces, d_screen, rays, xforms=None, *, x0: int = 0, y0: int = 0, rowbytes: int | None = None,
+                  nframes: int | None = None, keep_unmapped: bool = False, rgba: bool = False, tables=None,
+                  face_stride: int | None = None, screen_stride: int | None = None, stream: int | None = None):
+        """warp_view with each pixel's texel computed on the GPU from its view ray, turned by a per-frame 3x3 matrix,
+        through the current globe (blinky_warp_device_rays[_rgba]): frame f equals set_raymap of the turned field
+        followed by a one-frame warp_view, without changing the installed lensmap, whose size and background it uses.
+        rays: a CUDA float32 tensor [H, W, 3] (one field for every frame) or [N, H, W, 3] (one per frame); xforms: a
+        CUDA float32 tensor [3, 3] or [N, 3, 3] of row-major matrices, or None for the rays as they are.  nframes
+        defaults to N of whichever is per-frame (else 1).  The other arguments are warp_view's (tables: RGBA only).
+        May be captured into a CUDA graph; a replay reads the rays and matrices as they are then."""
+        if not (hasattr(rays, "is_cuda") and rays.is_cuda):
+            raise TypeError("warp_rays: rays must be a CUDA tensor")
+        W, H = self.width, self.height
+        if str(rays.dtype) != "torch.float32" or rays.dim() not in (3, 4) or tuple(rays.shape[-3:]) != (H, W, 3) or \
+                tuple(rays.stride()[-3:]) != (3 * W, 3, 1):
+            raise ValueError(f"warp_rays: rays must be float32 [{H}, {W}, 3] or [N, {H}, {W}, 3] with contiguous fields, got "
+                             f"{rays.dtype} {tuple(rays.shape)} strides {tuple(rays.stride())}")
+        if xforms is not None:
+            if not (hasattr(xforms, "is_cuda") and xforms.is_cuda):
+                raise TypeError("warp_rays: xforms must be a CUDA tensor")
+            if str(xforms.dtype) != "torch.float32" or xforms.dim() not in (2, 3) or tuple(xforms.shape[-2:]) != (3, 3) or \
+                    tuple(xforms.stride()[-2:]) != (3, 1):
+                raise ValueError(f"warp_rays: xforms must be float32 [3, 3] or [N, 3, 3] with contiguous matrices, got "
+                                 f"{xforms.dtype} {tuple(xforms.shape)} strides {tuple(xforms.stride())}")
+        per_frame = [t.shape[0] for t in (rays, xforms) if t is not None and t.dim() == (4 if t is rays else 3)]
+        if nframes is None:
+            nframes = min(per_frame) if per_frame else 1
+        if rays.dim() == 4 and rays.shape[0] < nframes:
+            raise ValueError(f"warp_rays: {rays.shape[0]} ray fields for {nframes} frames")
+        if xforms is not None and xforms.dim() == 3 and xforms.shape[0] < nframes:
+            raise ValueError(f"warp_rays: {xforms.shape[0]} matrices for {nframes} frames")
+        ray_stride = rays.stride(0) * 4 if rays.dim() == 4 else 0
+        d_xforms = None if xforms is None else xforms.data_ptr()
+        xform_stride = xforms.stride(0) * 4 if xforms is not None and xforms.dim() == 3 else 0
+        d_tables, table_stride = (None, 0) if tables is None else self._table_args(tables, rgba, nframes)
+        if face_stride is None:
+            face_stride = self._face_stride(d_faces)
+        bpp = 4 if rgba else 1
+        shape = getattr(d_screen, "shape", None)
+        if rowbytes is None:
+            rowbytes = d_screen.stride(-2) * d_screen.element_size() if shape is not None and len(shape) >= 2 else (x0 + W) * bpp
+        if screen_stride is None:
+            screen_stride = (d_screen.stride(-3) * d_screen.element_size() if shape is not None and len(shape) >= 3
+                             else (y0 + H) * rowbytes)
+        args = (self._ctx, _ptr(d_faces), face_stride, rays.data_ptr(), ray_stride, d_xforms, xform_stride, _ptr(d_screen), screen_stride,
+                rowbytes, x0, y0, nframes, 1 if keep_unmapped else 0)
+        if rgba:
+            self._check(self._lib.blinky_warp_device_rays_rgba(*args, d_tables, table_stride, _warp_stream(stream)))
+        else:
+            self._check(self._lib.blinky_warp_device_rays(*args, _warp_stream(stream)))
 
     def release_captures(self):
         """No CUDA graph that captured a warp of this context will run again (blinky_release_captures): frees the

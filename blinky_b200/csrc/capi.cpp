@@ -637,13 +637,9 @@ int warp_into_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0,
     return ctx->dev->warp(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
-// The view entry points: the warp r in keep_unmapped / rgba mode into the view rectangle at (x0, y0), checked first.
-// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose r.tables / r.table_stride are checked here too.
-int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba, bool with_tables = false) {
-    NEED_DEVICE(ctx);
-    r.keep_unmapped = keep_unmapped != 0;
-    r.rgba = rgba;
-    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : r.rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
+// The checks of the view entry points, r in keep_unmapped / rgba mode into the view rectangle at (x0, y0): BLINKY_OK or
+// the refusal.  with_tables: r.tables / r.table_stride are checked too.
+int check_view(blinky_ctx *ctx, const char *name, const blinky::WarpRequest &r, int rowbytes, int x0, int y0, bool with_tables) {
     auto invalid = [&](const char *why) { return set_err(ctx, BLINKY_E_INVALID, std::string(name) + ": " + why); };
     const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = r.rgba ? 4 : 1;
     if (!r.faces || !r.out) return invalid("NULL buffer");
@@ -660,7 +656,48 @@ int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x
         if (r.table_stride != 0 && (r.table_stride < 256 * sizeof(uint32_t) || r.table_stride % 16 != 0 || r.table_stride / 4 > UINT32_MAX))
             return invalid("table_stride must be 0 (one table for every frame) or at least 1024, a multiple of 16 and below 16 GB");
     }
-    return warp_into_view(ctx, r, rowbytes, x0, y0);
+    return BLINKY_OK;
+}
+
+// The view entry points: the warp r in keep_unmapped / rgba mode into the view rectangle at (x0, y0), checked first.
+// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose r.tables / r.table_stride are checked here too.
+int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba, bool with_tables = false) {
+    NEED_DEVICE(ctx);
+    r.keep_unmapped = keep_unmapped != 0;
+    r.rgba = rgba;
+    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : r.rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
+    const int rc = check_view(ctx, name, r, rowbytes, x0, y0, with_tables);
+    return rc != BLINKY_OK ? rc : warp_into_view(ctx, r, rowbytes, x0, y0);
+}
+
+// blinky_warp_device_rays[_rgba]: the view warp r with each pixel's texel computed from its ray in q, turned, through
+// the current globe.  Every refusal launches nothing.
+int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRequest &q, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba) {
+    NEED_DEVICE(ctx);
+    r.keep_unmapped = keep_unmapped != 0;
+    r.rgba = rgba;
+    const char *name = rgba ? "blinky_warp_device_rays_rgba" : "blinky_warp_device_rays";
+    auto refuse = [&](int code, const std::string &why) { return set_err(ctx, code, std::string(name) + ": " + why); };
+    const int W = ctx->dev->width(), H = ctx->dev->height(), ps = ctx->dev->platesize();
+    if (W <= 0) return refuse(BLINKY_E_STATE, "no lensmap installed (the view's size and background are the installed lensmap's)");
+    if (!ctx->host.globe_valid()) return refuse(BLINKY_E_STATE, "no valid globe");
+    if (ctx->host.has_globe_plate())
+        return refuse(BLINKY_E_STATE, "the globe picks its plates with a globe_plate script, whose decisions can need the interpreter: "
+                                      "map such rays with blinky_set_raymap_device and warp the installed lensmap");
+    if (!q.rays) return refuse(BLINKY_E_INVALID, "NULL rays");
+    if (reinterpret_cast<uintptr_t>(q.rays) % 4 != 0 || reinterpret_cast<uintptr_t>(q.xforms) % 4 != 0)
+        return refuse(BLINKY_E_INVALID, "d_rays and d_xforms must be 4-byte aligned");
+    if (q.ray_stride != 0 && (q.ray_stride < 12 * static_cast<size_t>(W) * static_cast<size_t>(H) || q.ray_stride % 4 != 0))
+        return refuse(BLINKY_E_INVALID, "ray_stride must be 0 (one field for every frame) or a multiple of 4 of at least 12 * width * height");
+    if (q.xform_stride != 0 && (q.xform_stride < 36 || q.xform_stride % 4 != 0))
+        return refuse(BLINKY_E_INVALID, "xform_stride must be 0 (one matrix for every frame) or a multiple of 4 of at least 36");
+    if (r.nframes > 65535) return refuse(BLINKY_E_INVALID, "at most 65535 frames per launch");
+    const int rc = check_view(ctx, name, r, rowbytes, x0, y0, rgba && r.tables);
+    if (rc != BLINKY_OK) return rc;
+    const blinky::LensBuildParams globe = ctx->host.device_params(W, H, ps);
+    r.out_pitch = static_cast<size_t>(rowbytes);
+    r.out = static_cast<uint8_t *>(r.out) + static_cast<size_t>(y0) * r.out_pitch + static_cast<size_t>(x0) * (rgba ? 4 : 1);
+    return ctx->dev->warp_rays(r, q, globe) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 }  // namespace
@@ -690,6 +727,22 @@ int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, si
     r.tables = d_tables;
     r.table_stride = table_stride;
     return warp_device_view(ctx, r, rowbytes, x0, y0, keep_unmapped, true, true);
+}
+
+int blinky_warp_device_rays(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride, const float *d_xforms,
+                            size_t xform_stride, void *d_screen, size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                            int keep_unmapped, void *stream) {
+    return warp_device_rays(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, {d_rays, ray_stride, d_xforms, xform_stride},
+                            rowbytes, x0, y0, keep_unmapped, false);
+}
+
+int blinky_warp_device_rays_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
+                                 const float *d_xforms, size_t xform_stride, void *d_screen_rgba, size_t screen_frame_stride, int rowbytes,
+                                 int x0, int y0, int nframes, int keep_unmapped, const uint32_t *d_tables, size_t table_stride, void *stream) {
+    blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
+    r.tables = d_tables;
+    r.table_stride = table_stride;
+    return warp_device_rays(ctx, r, {d_rays, ray_stride, d_xforms, xform_stride}, rowbytes, x0, y0, keep_unmapped, true);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,

@@ -152,6 +152,11 @@ public:
     bool fisheye_enabled() const { return fisheye_enabled_; }
     bool lens_valid() const { return lens_valid_; }
     bool globe_valid() const { return globe_valid_; }
+    // the globe picks its plates with a globe_plate script (whose decisions can need the interpreter)
+    bool has_globe_plate() const { return fn_globe_plate_.is_function(); }
+    // the globe's plates, rubix grid and uv scales (and the lens's scale) as the device kernels read them, for a
+    // width x height view on plates of platesize texels
+    LensBuildParams device_params(int width, int height, int platesize) const;
     const std::string &lens_name() const { return lens_name_; }
     const std::string &globe_name() const { return globe_name_; }
     const std::string &onload() const { return onload_; }
@@ -226,7 +231,6 @@ private:
     int build_inverse(int threads);
     int build_inverse_device(int *display, std::string *why);  // 0 ok, -1 script failure, 1 = not possible (why)
     int build_forward_device(std::string *why);                // same convention
-    LensBuildParams device_params(int width, int height, int platesize) const;
     int build_forward(int threads);
     int uv_to_screen(Worker &w, int plate, double u, double v, int *lx, int *ly);
     void draw_quad(const int *tl, const int *tr, const int *bl, const int *br, int plate, int px, int py, int *display);

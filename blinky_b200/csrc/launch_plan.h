@@ -52,6 +52,25 @@ inline WarpKernel choose_kernel(const WarpRequest &r, size_t pitch, const FaceLa
     return vector ? WarpKernel::Vector : WarpKernel::Scalar;
 }
 
+// The warp from a ray field (ray_warp_kernel): one thread per 4-pixel quad of a row, written as one word, when W % 4
+// == 0 and the view's origin, pitch and frame stride allow 4-pixel words; otherwise one thread per pixel.
+inline bool ray_warp_quads(const WarpRequest &r, size_t pitch, int width) {
+    const size_t word = 4 * (r.rgba ? 4 : 1);
+    const bool frames_aligned = reinterpret_cast<uintptr_t>(r.out) % word == 0 && (r.out_stride % word == 0 || r.nframes == 1);
+    return width % 4 == 0 && pitch % word == 0 && frames_aligned;
+}
+
+// Frames each thread of a ray warp carries.  With one ray field for every frame (ray_stride 0) a thread carries several,
+// so that the field is read once per launch rather than once per frame — but no more than leaves the launch at least
+// `resident_threads` threads (what the GPU holds at once: SMs x threads per SM), so that a small view in a large batch
+// does not leave most SMs idle.  nitems: threads per frame (quads or pixels).  Per-frame fields: one frame per thread.
+inline int ray_warp_frames_per_thread(size_t ray_stride, int nframes, uint32_t nitems, uint32_t resident_threads) {
+    if (ray_stride != 0 || nframes <= 1) return 1;
+    const uint64_t want = (static_cast<uint64_t>(resident_threads) + std::max<uint32_t>(nitems, 1u) - 1) / std::max<uint32_t>(nitems, 1u);
+    const uint64_t splits = std::min<uint64_t>(static_cast<uint64_t>(nframes), std::max<uint64_t>(want, 1u));
+    return static_cast<int>(static_cast<uint64_t>(nframes) / splits);   // (rounded down: at least `splits` rows of threads)
+}
+
 struct RingGeometry {
     int warps;            // resident ring warps per SM; 0: the plan's largest box does not fit a ring
     uint32_t ring_bytes;  // each warp's staging ring (a multiple of 128)

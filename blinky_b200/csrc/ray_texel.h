@@ -1,0 +1,87 @@
+// The per-ray arithmetic of a warp from a ray field (ray_warp.cu, blinky_warp_device_rays): a view ray turned by a 3x3
+// matrix, then mapped through the current globe exactly as FisheyeHost::set_raymap maps it — normalize3, the plate argmax
+// of ray_to_plate_index, ray_to_plate_uv, the texel and its range checks, and on_rubix_grid (fisheye_host.cpp), operation
+// by operation, with the globe's values as FisheyeHost::device_params computes them.
+//
+// This is a second copy of that arithmetic, kept apart from the NVRTC text of lens_device.cu on purpose: the warp
+// kernel must run without NVRTC and be capturable on its first call.  Host and device share this header; the CPU tests
+// compile it with g++ -ffp-contract=off and pin it to the host path, and ray_warp.cu is compiled with --fmad=false, so
+// every float and double operation here is one IEEE-rounded operation on both.
+#pragma once
+
+#include <math.h>
+
+#include <cstdint>
+
+#include "face_layout.h"   // BLINKY_HD
+#include "lens_device.h"   // LensBuildParams
+
+namespace blinky {
+
+// t = M ray, M row-major: t_k = (M[k][0] x + M[k][1] y) + M[k][2] z, every product and sum rounded to float
+BLINKY_HD void turn_ray(const float M[9], const float ray[3], float t[3]) {
+    for (int k = 0; k < 3; ++k) t[k] = (M[3 * k] * ray[0] + M[3 * k + 1] * ray[1]) + M[3 * k + 2] * ray[2];
+}
+
+BLINKY_HD float ray_dot3(const float a[3], const float b[3]) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+// normalize3 (VectorNormalize): a zero, NaN or overflowing length leaves what the division gives, as on the host
+BLINKY_HD void ray_normalize3(float v[3]) {
+    float len = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
+    len = static_cast<float>(sqrt(static_cast<double>(len)));
+    if (len) {
+        const float inv = 1 / len;
+        v[0] *= inv;
+        v[1] *= inv;
+        v[2] *= inv;
+    }
+}
+
+// The plate and texel set_raymap gives the unnormalised ray (normalised here, in place) on plates of P.platesize
+// texels: false when the ray maps to nothing.  The plate is the argmax over the globe's P.numplates plates (strict:
+// the lowest index wins ties, NaN never wins).
+BLINKY_HD bool ray_texel(const LensBuildParams &P, float ray[3], int *plate, int *px, int *py) {
+    ray_normalize3(ray);
+    int best = 0;
+    double best_dp = -2;
+    for (int i = 0; i < P.numplates; ++i) {
+        const double dp = ray_dot3(ray, P.plates[i].forward);   // float dot product, widened
+        if (dp > best_dp) {
+            best_dp = dp;
+            best = i;
+        }
+    }
+    const LensBuildParams::PlateF &p = P.plates[best];
+    const double x = ray_dot3(p.right, ray);
+    const double y = ray_dot3(p.up, ray);
+    const double z = ray_dot3(p.forward, ray);
+    const double u = x / z * P.uv_dist[best] + 0.5;
+    const double v = -y / z * P.uv_dist[best] + 0.5;
+    if (!(u >= 0 && u <= 1 && v >= 0 && v <= 1)) return false;
+    const int ps = P.platesize;
+    *plate = best;
+    *px = static_cast<int>(u * ps);
+    *py = static_cast<int>(v * ps);
+    return *px >= 0 && *px < ps && *py >= 0 && *py < ps;
+}
+
+// on_rubix_grid: texel (px, py) lies in the padding between the rubix cells
+BLINKY_HD bool ray_on_rubix_grid(const LensBuildParams &P, int px, int py) {
+    const double ux = static_cast<double>(px) / P.rubix_unit_px;
+    const double uy = static_cast<double>(py) / P.rubix_unit_px;
+    return fmod(ux, P.rubix_block) < P.rubix_pad || fmod(uy, P.rubix_block) < P.rubix_pad;
+}
+
+// The packed lensmap entry (BLINKY_LM_*) blinky_set_raymap installs for the ray turned by M (nullptr: the ray as it
+// is): a map made in one pass gives an on-grid texel no tint.
+BLINKY_HD uint32_t ray_entry(const LensBuildParams &P, const float *M, const float ray[3]) {
+    float t[3] = {ray[0], ray[1], ray[2]};
+    if (M) turn_ray(M, ray, t);
+    int plate, px, py;
+    if (!ray_texel(P, t, &plate, &px, &py)) return 7u << 28;
+    const uint32_t tint = ray_on_rubix_grid(P, px, py) ? 7u : static_cast<uint32_t>(plate);
+    const uint32_t ps = static_cast<uint32_t>(P.platesize);
+    return 0x80000000u | tint << 28 | (static_cast<uint32_t>(plate) * ps * ps + static_cast<uint32_t>(px) + static_cast<uint32_t>(py) * ps);
+}
+
+}  // namespace blinky

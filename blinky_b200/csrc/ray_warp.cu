@@ -1,0 +1,228 @@
+// The warp from a ray field turned by a per-frame matrix (blinky_warp_device_rays): each pixel's texel is computed on
+// the fly from its view ray, so a head-tracked look-around needs no lensmap, plan or install per frame — only the
+// matrix changes.  Frame f of the output equals blinky_set_raymap of the field turned by M_f followed by a one-frame
+// blinky_warp_device_view (ray_texel.h holds the per-ray arithmetic).
+//
+// Compiled with --fmad=false: the turn and the globe's float / double arithmetic must round operation by operation
+// as the host's -ffp-contract=off build does.
+#include "ray_warp.h"
+
+#include <cuda_runtime.h>
+
+#include <cstdio>
+
+#include "ray_texel.h"
+
+namespace blinky {
+
+namespace {
+
+constexpr int kRayThreads = 256;
+
+struct RayWarpParams {
+    const float *rays;
+    size_t ray_floats;          // floats between frames' fields (0: shared)
+    const float *xforms;
+    size_t xform_floats;        // floats between frames' matrices (0: shared)
+    const uint8_t *faces;
+    size_t face_stride;
+    const uint8_t *bg;
+    const uint8_t *lut;
+    const uint32_t *rgba;
+    size_t table_words;
+    uint8_t *out;
+    size_t out_stride;
+    uint32_t pitch;
+    uint32_t width;
+    uint32_t nitems;            // quads or pixels
+    int nframes;
+    int frames_per_thread;
+};
+
+__device__ __forceinline__ uint32_t ld_texel(const uint8_t *p) {
+    uint32_t v;
+    asm volatile("ld.global.nc.u8 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+
+__device__ __forceinline__ void st_cs_u8(uint8_t *p, uint32_t v) { asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ void st_cs_u32(void *p, uint32_t v) { asm volatile("st.global.cs.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ void st_cs_v4(void *p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+
+// --------------------------------------------------------------------------
+// One thread per item: a 4-pixel quad of a row (QUAD, W % 4 == 0) or one pixel.  The thread carries frames
+// [blockIdx.y * frames_per_thread, ...): with one shared field it reads its rays once, and with one shared matrix too
+// it maps them once; per frame it gathers the texels, tints, expands and stores like warp_gather_kernel (K1) /
+// warp_scalar_kernel (K0).  The texel of (plate, px, py) is lay.plate_base[plate] + py * lay.rowbytes + px: dense
+// faces are the layout with rowbytes = ps.
+// --------------------------------------------------------------------------
+template <bool QUAD, bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
+__global__ void __launch_bounds__(kRayThreads) ray_warp_kernel(const __grid_constant__ RayWarpParams p, const __grid_constant__ LensBuildParams P,
+                                                               const __grid_constant__ FaceLayoutParams lay) {
+    constexpr int NP = QUAD ? 4 : 1;
+    __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
+    __shared__ uint32_t s_rgba[RGBA && !TABLES ? 256 : 1];
+    if (RUBIX) {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.lut);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(s_lut);
+        for (int i = threadIdx.x; i < 6 * 256 / 4; i += kRayThreads) dst[i] = __ldg(src + i);
+    }
+    if (RGBA && !TABLES) {
+        for (int i = threadIdx.x; i < 256; i += kRayThreads) s_rgba[i] = __ldg(p.rgba + i);
+    }
+    if (RUBIX || (RGBA && !TABLES)) __syncthreads();
+
+    const uint32_t item = blockIdx.x * kRayThreads + threadIdx.x;
+    if (item >= p.nitems) return;
+    const uint32_t pix = item * NP;   // dense index y * W + x of the item's first pixel (a quad never straddles rows)
+    const uint32_t y = pix / p.width, x = pix - y * p.width;
+    const size_t out_at = static_cast<size_t>(y) * p.pitch + static_cast<size_t>(x) * (RGBA ? 4 : 1);
+    const int f0 = static_cast<int>(blockIdx.y) * p.frames_per_thread;
+    const int f1 = min(p.nframes, f0 + p.frames_per_thread);
+
+    // a pixel's texel, packed: px (bits 0-12), py (13-25), plate (26-28), on the rubix grid (29), mapped (31) —
+    // WarpDevice::warp_rays refuses a plate size beyond set_raymap's limit, 6 * ps^2 < 2^28, so ps <= 6688 < 2^13
+    constexpr uint32_t kMapped = 0x80000000u, kOnGrid = 0x20000000u;
+    float ray[NP][3];
+    uint32_t tx[NP];
+    uint32_t valid = 0;   // bit k: pixel k is mapped
+    for (int f = f0; f < f1; ++f) {
+        if (f == f0 || p.ray_floats) {
+            const float *r = p.rays + static_cast<size_t>(f) * p.ray_floats + 3 * static_cast<size_t>(pix);
+#pragma unroll
+            for (int k = 0; k < NP; ++k)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) ray[k][c] = __ldg(r + 3 * k + c);
+        }
+        if (f == f0 || p.ray_floats || p.xform_floats) {
+            float M[9] = {};
+            if (p.xforms) {
+                const float *m = p.xforms + static_cast<size_t>(f) * p.xform_floats;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) M[i] = __ldg(m + i);
+            }
+            valid = 0;
+#pragma unroll
+            for (int k = 0; k < NP; ++k) {
+                float t[3] = {ray[k][0], ray[k][1], ray[k][2]};
+                if (p.xforms) turn_ray(M, ray[k], t);
+                int plate = 0, px = 0, py = 0;
+                tx[k] = 0;
+                if (ray_texel(P, t, &plate, &px, &py)) {
+                    valid |= 1u << k;
+                    tx[k] = kMapped | static_cast<uint32_t>(plate) << 26 | static_cast<uint32_t>(py) << 13 | static_cast<uint32_t>(px);
+                }
+            }
+            // (the tint is read only with f_rubix: the grid test's two fmods are skipped otherwise)
+            if (RUBIX) {
+#pragma unroll
+                for (int k = 0; k < NP; ++k)
+                    if ((tx[k] & kMapped) && ray_on_rubix_grid(P, tx[k] & 0x1fffu, (tx[k] >> 13) & 0x1fffu)) tx[k] |= kOnGrid;
+            }
+        }
+        if (KEEP && valid == 0) continue;
+        const uint8_t *faces = p.faces + static_cast<size_t>(f) * p.face_stride;
+        const uint32_t *table = RGBA && TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : nullptr;
+        const bool all_valid = valid == (1u << NP) - 1;
+        uint32_t bgw = 0;
+        if (!KEEP && !all_valid) bgw = QUAD ? __ldg(reinterpret_cast<const uint32_t *>(p.bg) + item) : __ldg(p.bg + pix);
+        uint32_t px4[NP];
+#pragma unroll
+        for (int k = 0; k < NP; ++k) {
+            uint32_t b;
+            if (tx[k] & kMapped) {
+                const uint32_t plate = (tx[k] >> 26) & 7u;
+                b = ld_texel(faces + lay.plate_base[plate] + static_cast<size_t>((tx[k] >> 13) & 0x1fffu) * lay.rowbytes + (tx[k] & 0x1fffu));
+                if (RUBIX && !(tx[k] & kOnGrid)) b = s_lut[plate * 256 + b];
+            } else {
+                b = (bgw >> (8 * k)) & 0xffu;
+            }
+            if (RGBA) b = TABLES ? __ldg(table + b) : s_rgba[b];
+            px4[k] = b;
+        }
+        uint8_t *o = p.out + static_cast<size_t>(f) * p.out_stride + out_at;
+        if (QUAD && !(KEEP && !all_valid)) {
+            if (RGBA) st_cs_v4(o, px4[0], px4[NP > 1 ? 1 : 0], px4[NP > 2 ? 2 : 0], px4[NP > 3 ? 3 : 0]);
+            else st_cs_u32(o, px4[0] | (px4[NP > 1 ? 1 : 0] << 8) | (px4[NP > 2 ? 2 : 0] << 16) | (px4[NP > 3 ? 3 : 0] << 24));
+        } else {
+#pragma unroll
+            for (int k = 0; k < NP; ++k) {
+                if (KEEP && !((valid >> k) & 1u)) continue;
+                if (RGBA) st_cs_u32(o + 4 * k, px4[k]);
+                else st_cs_u8(o + k, px4[k]);
+            }
+        }
+    }
+}
+
+template <bool QUAD, bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
+void launch_instance(const RayWarpParams &p, const LensBuildParams &P, const FaceLayoutParams &lay, dim3 grid, cudaStream_t st) {
+    ray_warp_kernel<QUAD, RUBIX, RGBA, KEEP, TABLES><<<grid, kRayThreads, 0, st>>>(p, P, lay);
+}
+
+// the instance of (quads, rubix, rgba, keep, tables): per-frame tables exist only in RGBA, so 24 instances
+template <bool QUAD, bool RUBIX, bool RGBA, bool KEEP>
+void launch_tables(bool tables, const RayWarpParams &p, const LensBuildParams &P, const FaceLayoutParams &lay, dim3 grid, cudaStream_t st) {
+    if constexpr (RGBA) {
+        if (tables) return launch_instance<QUAD, RUBIX, RGBA, KEEP, true>(p, P, lay, grid, st);
+    }
+    launch_instance<QUAD, RUBIX, RGBA, KEEP, false>(p, P, lay, grid, st);
+}
+
+template <bool QUAD, bool RUBIX, bool RGBA>
+void launch_keep(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.keep) launch_tables<QUAD, RUBIX, RGBA, true>(L.tables, p, L.globe, L.layout, grid, st);
+    else launch_tables<QUAD, RUBIX, RGBA, false>(L.tables, p, L.globe, L.layout, grid, st);
+}
+
+template <bool QUAD, bool RUBIX>
+void launch_rgba(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.rgba) launch_keep<QUAD, RUBIX, true>(L, p, grid, st);
+    else launch_keep<QUAD, RUBIX, false>(L, p, grid, st);
+}
+
+template <bool QUAD>
+void launch_rubix(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.rubix) launch_rgba<QUAD, true>(L, p, grid, st);
+    else launch_rgba<QUAD, false>(L, p, grid, st);
+}
+
+}  // namespace
+
+bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
+    RayWarpParams p;
+    p.rays = L.rays;
+    p.ray_floats = L.ray_stride / 4;
+    p.xforms = L.xforms;
+    p.xform_floats = L.xform_stride / 4;
+    p.faces = static_cast<const uint8_t *>(L.faces);
+    p.face_stride = L.face_stride;
+    p.bg = L.bg;
+    p.lut = L.lut;
+    p.rgba = L.palette;
+    p.table_words = L.table_stride / 4;
+    p.out = static_cast<uint8_t *>(L.out);
+    p.out_stride = L.out_stride;
+    p.pitch = L.pitch;
+    p.width = static_cast<uint32_t>(L.width);
+    const size_t npix = static_cast<size_t>(L.width) * static_cast<size_t>(L.height);
+    p.nitems = static_cast<uint32_t>(L.quads ? npix / 4 : npix);
+    p.nframes = L.nframes;
+    p.frames_per_thread = L.frames_per_thread;
+    const dim3 grid(static_cast<unsigned>((p.nitems + kRayThreads - 1) / kRayThreads),
+                    static_cast<unsigned>((L.nframes + L.frames_per_thread - 1) / L.frames_per_thread));
+    cudaStream_t st = static_cast<cudaStream_t>(L.stream);
+    if (L.quads) launch_rubix<true>(L, p, grid, st);
+    else launch_rubix<false>(L, p, grid, st);
+    char buf[192];
+    snprintf(buf, sizeof buf, "ray_warp_kernel<quad=%d,rubix=%d,rgba=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d", L.quads, L.rubix,
+             L.rgba, L.keep, L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread);
+    *name = buf;
+    const cudaError_t e = cudaGetLastError();
+    *cuda_err = static_cast<int>(e);
+    return e == cudaSuccess;
+}
+
+}  // namespace blinky

@@ -1,0 +1,40 @@
+// The warp from a ray field turned by a per-frame matrix (blinky_warp_device_rays, ray_warp.cu): what one launch
+// needs, in host types, so that warp_device.cu can plan it without the kernel's translation unit.
+#pragma once
+
+#include <cstddef>
+#include <cstdint>
+#include <string>
+
+#include "face_layout.h"
+#include "lens_device.h"
+
+namespace blinky {
+
+struct RayWarpLaunch {
+    const float *rays;          // frame 0's field, float32[height][width][3]
+    size_t ray_stride;          // bytes between frames' fields (0: one field for every frame)
+    const float *xforms;        // frame 0's matrix, 9 floats row-major (nullptr: the rays as they are)
+    size_t xform_stride;        // bytes between frames' matrices (0: one matrix for every frame)
+    const void *faces;          // frame 0's faces, addressed through `layout`
+    size_t face_stride;
+    const uint8_t *bg;          // background, [height][width], padded like a lensmap to whole quads
+    const uint8_t *lut;         // [6][256] rubix tint LUTs
+    const uint32_t *palette;    // RGBA: the palette table (tables: frame 0's)
+    size_t table_stride;        // tables: bytes between frames' tables
+    void *out;                  // view origin of frame 0
+    size_t out_stride;          // bytes between frames
+    uint32_t pitch;             // bytes between output rows
+    int width, height, nframes;
+    int frames_per_thread;      // ray_warp_frames_per_thread (launch_plan.h)
+    bool quads;                 // ray_warp_quads (launch_plan.h)
+    bool rubix, rgba, keep, tables;
+    LensBuildParams globe;      // FisheyeHost::device_params of the current globe at the view's size
+    FaceLayoutParams layout;    // plate_base and rowbytes address every plate of the globe (dense faces included)
+    void *stream;               // cudaStream_t
+};
+
+// Launches ray_warp_kernel for L.  false with the CUDA error in *cuda_err; *name: the instance and launch shape (last_kernel).
+bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err);
+
+}  // namespace blinky

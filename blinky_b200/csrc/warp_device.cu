@@ -23,6 +23,8 @@
 #include "../../include/blinky_b200.h"
 #include "face_layout.h"
 #include "launch_plan.h"
+#include "lens_device.h"
+#include "ray_warp.h"
 #include "tile_plan.h"
 #include "tile_plan_device.h"
 
@@ -1024,6 +1026,7 @@ WarpDevice::WarpDevice(int device) : device_(device) {
         throw std::runtime_error(buf);
     }
     sm_count_ = prop.multiProcessorCount;
+    threads_per_sm_ = prop.maxThreadsPerMultiProcessor;
     smem_per_sm_ = prop.sharedMemPerMultiprocessor;
     if (const char *e = getenv("BLINKY_RING_BYTES")) ring_bytes_override_ = atoi(e);
     if (const char *e = getenv("BLINKY_RING_BOXES")) ring_boxes_ = atoi(e);
@@ -1051,6 +1054,7 @@ WarpDevice::~WarpDevice() {
 size_t WarpDevice::padded_pixels(size_t npix) { return round_up(npix, kPixelsPerBlock); }
 int WarpDevice::width() const { return cur_ ? cur_->width : 0; }
 int WarpDevice::height() const { return cur_ ? cur_->height : 0; }
+int WarpDevice::platesize() const { return cur_ ? cur_->platesize : 0; }
 size_t WarpDevice::plan_tiles() const { return cur_ && cur_->have_plan ? cur_->ntiles : 0; }
 size_t WarpDevice::plan_entry_bytes() const { return cur_ && cur_->have_plan ? cur_->entry_bytes : 0; }
 
@@ -1152,7 +1156,7 @@ void WarpDevice::set_face_layout(int rowbytes, const int32_t *origins, int nplat
 
 // The face layout against the current lensmap (the plate size and the plates it samples change with every build):
 // false, with err_code_ BLINKY_E_INVALID, when it does not fit; otherwise the kernels' view of it in *lay.
-bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay) {
+bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay, int globe_plates) {
     err_code_ = BLINKY_E_INVALID;
     const int n = static_cast<int>(layout_origins_.size() / 2);
     const uint64_t rb = static_cast<uint64_t>(layout_rowbytes_), ps = static_cast<uint64_t>(cur_->platesize);
@@ -1172,8 +1176,9 @@ bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *
     }
     for (int pl = n; pl < kLayoutPlates; ++pl) {
         const int *r = cur_->plate_rect[pl];
-        if (cur_->display[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
-            err_ = "face layout: the lensmap samples plate " + std::to_string(pl) + ", which has no origin (the layout has " + std::to_string(n) + ")";
+        if (globe_plates >= 0 ? pl < globe_plates : cur_->display[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
+            err_ = std::string(globe_plates >= 0 ? "face layout: the globe has plate " : "face layout: the lensmap samples plate ") + std::to_string(pl) +
+                   ", which has no origin (the layout has " + std::to_string(n) + ")";
             return false;
         }
     }
@@ -1192,13 +1197,7 @@ bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *
     return true;
 }
 
-bool WarpDevice::warp(const WarpRequest &r) {
-    err_code_ = BLINKY_E_CUDA;
-    if (!cur_) {
-        err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
-        return false;
-    }
-    if (r.nframes <= 0) return true;
+bool WarpDevice::check_output(const WarpRequest &r, size_t *pitch) {
     if (r.nframes > 65535) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp: at most 65535 frames per launch";
@@ -1211,34 +1210,120 @@ bool WarpDevice::warp(const WarpRequest &r) {
         return false;
     }
     const Generation &g = *cur_;
-    const size_t pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(g.width) * opx;
-    if (pitch < static_cast<size_t>(g.width) * opx || pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
+    *pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(g.width) * opx;
+    if (*pitch < static_cast<size_t>(g.width) * opx || *pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
         return false;
     }
+    return true;
+}
+
+bool WarpDevice::capture_info(void *stream, bool *capturing, unsigned long long *id) {
+    // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    *id = 0;
+    if (stream != nullptr && static_cast<cudaStream_t>(stream) != cudaStreamLegacy)
+        CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(stream), &cap, id));
+    *capturing = cap != cudaStreamCaptureStatusNone;
+    return true;
+}
+
+void WarpDevice::remember_capture(void *stream, unsigned long long id) {
+    if (held_.empty() || held_.back() != cur_) held_.push_back(cur_);
+    bool known = false;
+    for (CaptureStream &c : capture_streams_)
+        if (c.stream == stream) c.id = id, known = true;
+    if (!known) capture_streams_.push_back({stream, id});
+}
+
+bool WarpDevice::warp(const WarpRequest &r) {
+    err_code_ = BLINKY_E_CUDA;
+    if (!cur_) {
+        err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
+        return false;
+    }
+    if (r.nframes <= 0) return true;
+    size_t pitch = 0;
+    if (!check_output(r, &pitch)) return false;
+    const Generation &g = *cur_;
     const bool use_layout = layout_rowbytes_ > 0 && !r.dense_faces;
     FaceLayoutParams lay = {};   // (dense: the kernels' last argument, never read)
     if (use_layout && !make_layout(r.face_stride, r.nframes, &lay)) return false;
     const KernelVariant v = {rubix_, r.rgba, r.keep_unmapped, r.rgba && r.tables && r.table_stride != 0, use_layout};
     const WarpKernel k = choose_kernel(r, pitch, use_layout ? &lay : nullptr, g.width, g.height, g.have_plan, g.plan_has_box,
                                        variant_ == BLINKY_KERNEL_GATHER);
-    // (the legacy default stream cannot capture, and asking it while another stream captures is an error)
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    bool capturing = false;
     unsigned long long cap_id = 0;
-    if (r.stream != nullptr && static_cast<cudaStream_t>(r.stream) != cudaStreamLegacy)
-        CK(cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(r.stream), &cap, &cap_id));
-    const bool capturing = cap != cudaStreamCaptureStatusNone;
+    if (!capture_info(r.stream, &capturing, &cap_id)) return false;
     const bool ok = k == WarpKernel::Ring ? launch_ring(r, static_cast<uint32_t>(pitch), v, lay, capturing)
                                           : launch_flat(r, static_cast<uint32_t>(pitch), v, lay, k);
-    if (capturing) {
-        if (held_.empty() || held_.back() != cur_) held_.push_back(cur_);
-        bool known = false;
-        for (CaptureStream &c : capture_streams_)
-            if (c.stream == r.stream) c.id = cap_id, known = true;
-        if (!known) capture_streams_.push_back({r.stream, cap_id});
-    }
+    if (capturing) remember_capture(r.stream, cap_id);
     return ok;
+}
+
+bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe) {
+    err_code_ = BLINKY_E_CUDA;
+    if (!cur_) {
+        err_code_ = BLINKY_E_STATE;
+        err_ = "warp_rays: no lensmap on the device (its view size and background are the warp's)";
+        return false;
+    }
+    if (r.nframes <= 0) return true;
+    // (the kernel packs a texel's px and py into 13 bits each: set_raymap's own limit, 6 * ps^2 < 2^28, keeps ps <= 6688)
+    if (static_cast<uint64_t>(cur_->platesize) * static_cast<uint64_t>(cur_->platesize) * kLayoutPlates > 0x0FFFFFFFu) {
+        err_code_ = BLINKY_E_STATE;
+        err_ = "warp_rays: the installed lensmap's plate size " + std::to_string(cur_->platesize) +
+               " is beyond what a ray map takes (6 * platesize^2 must fit the 28-bit texel index)";
+        return false;
+    }
+    size_t pitch = 0;
+    if (!check_output(r, &pitch)) return false;
+    const Generation &g = *cur_;
+    FaceLayoutParams lay = {};
+    if (layout_rowbytes_ > 0) {
+        if (!make_layout(r.face_stride, r.nframes, &lay, globe.numplates)) return false;
+    } else {   // dense [plate][ps][ps] frames: the layout with rowbytes = ps
+        const uint64_t ps = static_cast<uint64_t>(g.platesize);
+        for (int i = 0; i < kLayoutPlates; ++i) lay.plate_base[i] = static_cast<uint64_t>(i) * ps * ps;
+        lay.rowbytes = static_cast<uint32_t>(ps);
+    }
+    bool capturing = false;
+    unsigned long long cap_id = 0;
+    if (!capture_info(r.stream, &capturing, &cap_id)) return false;
+    RayWarpLaunch L;
+    L.rays = q.rays;
+    L.ray_stride = q.ray_stride;
+    L.xforms = q.xforms;
+    L.xform_stride = q.xform_stride;
+    L.faces = r.faces;
+    L.face_stride = r.face_stride;
+    L.bg = g.bg->as<const uint8_t>();
+    L.lut = d_lut_.as<const uint8_t>();
+    L.palette = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
+    L.table_stride = r.table_stride;
+    L.out = r.out;
+    L.out_stride = r.out_stride;
+    L.pitch = static_cast<uint32_t>(pitch);
+    L.width = g.width;
+    L.height = g.height;
+    L.nframes = r.nframes;
+    L.quads = ray_warp_quads(r, pitch, g.width);
+    const size_t npix = static_cast<size_t>(g.width) * static_cast<size_t>(g.height);
+    L.frames_per_thread = ray_warp_frames_per_thread(q.ray_stride, r.nframes, static_cast<uint32_t>(L.quads ? npix / 4 : npix),
+                                                     static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
+    L.rubix = rubix_;
+    L.rgba = r.rgba;
+    L.keep = r.keep_unmapped;
+    L.tables = r.rgba && r.tables && r.table_stride != 0;
+    L.globe = globe;
+    L.layout = lay;
+    L.stream = r.stream;
+    int e = 0;
+    const bool ok = launch_ray_warp(L, &last_kernel_, &e);
+    ++launches_;
+    if (capturing) remember_capture(r.stream, cap_id);
+    return ok ? true : fail("ray_warp_kernel", e);
 }
 
 bool WarpDevice::release_captures() {

@@ -19,6 +19,7 @@ namespace blinky {
 
 struct DevicePlan;     // tile_plan_device.h
 struct KernelVariant;  // launch_plan.h
+struct LensBuildParams;  // lens_device.h
 enum class WarpKernel;
 
 // What WarpDevice::install keeps of a lensmap beside its device buffers (DevicePlan).
@@ -55,6 +56,14 @@ struct WarpRequest {
     bool dense_faces = false;          // the faces are dense [plate][ps][ps] frames whatever the face layout
 };
 
+// The ray field and matrices of a warp from rays (WarpDevice::warp_rays), device memory read when the launch runs.
+struct RayRequest {
+    const float *rays;          // frame 0's field, float32[height][width][3] as blinky_set_raymap reads it
+    size_t ray_stride;          // bytes between frames (0: one field for every frame)
+    const float *xforms;        // frame 0's 3x3 matrix, row-major (nullptr: the rays as they are)
+    size_t xform_stride;        // bytes between frames (0: one matrix for every frame)
+};
+
 class WarpDevice {
 public:
     // throws std::runtime_error on CUDA failure
@@ -80,6 +89,7 @@ public:
     // size of the resident lensmap's view (0 before the first install)
     int width() const;
     int height() const;
+    int platesize() const;
     // entries of a device lensmap buffer for npix pixels (the kernels read whole blocks; the padding is unmapped)
     static size_t padded_pixels(size_t npix);
     // copies of the resident map ([height][width] entries) and tile plan, synchronously
@@ -89,6 +99,11 @@ public:
     size_t plan_entry_bytes() const;
 
     bool warp(const WarpRequest &r);
+    // r (view, rgba, keep_unmapped, tables) with each pixel's texel computed from its ray in q, turned, through the
+    // globe `globe` (FisheyeHost::device_params at the resident view's size, no globe_plate script): the resident
+    // lensmap gives only the view's size and background.  Every plate of the globe must have an origin in the face
+    // layout.  Capturable like warp().
+    bool warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go
     // of the generations held for such graphs and returns every capture counter slot to the pool.
     bool release_captures();
@@ -115,11 +130,19 @@ private:
     struct Slot;
     bool ensure_slots();
     bool fail(const char *what, int cuda_err);
-    bool make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay);
+    // globe_plates >= 0: the plates 0..globe_plates-1 need an origin (a warp from rays may sample any of them), instead
+    // of the plates the lensmap samples
+    bool make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay, int globe_plates = -1);
+    // the checks every warp makes of its output; *pitch: the bytes between output rows
+    bool check_output(const WarpRequest &r, size_t *pitch);
+    // whether r.stream is capturing (and which capture); remember_capture: a warp was captured into it
+    bool capture_info(void *stream, bool *capturing, unsigned long long *id);
+    void remember_capture(void *stream, unsigned long long id);
     void finalize_slot(Slot &s);
 
     int device_ = 0;
     int sm_count_ = 132;
+    int threads_per_sm_ = 2048;
     bool batch_copies_ = true;   // plate rectangles of a frame in one cudaMemcpy3DBatchAsync (false once the driver refused it)
     const void *pin_src_ptr_ = nullptr, *pin_dst_ptr_ = nullptr;  // last buffers warp_host saw and whether they are pinned
     bool pin_src_ = false, pin_dst_ = false;

@@ -484,6 +484,50 @@ int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, si
                                         int y0, int nframes, int keep_unmapped, const uint32_t *d_tables,
                                         size_t table_stride, void *stream);
 
+/* Warp from a ray field turned by a per-frame 3x3 matrix: each pixel's texel is computed on the GPU
+ * from its view ray, so a head-tracked look-around needs no lensmap, plan or install per frame.
+ * W, H and ps are those of the installed lensmap (blinky_width, blinky_height, blinky_platesize), which
+ * also gives the background; without one the call fails with BLINKY_E_STATE.  Frame f reads
+ *   - the ray field at d_rays + f * ray_stride bytes: float32[H][W][3] as blinky_set_raymap reads it
+ *     (ray_stride 0: one field for every frame);
+ *   - the matrix M_f at d_xforms + f * xform_stride bytes: 9 floats, row-major (xform_stride 0: one
+ *     matrix for every frame; d_xforms NULL: no turn, the rays are used exactly as read);
+ *   - the faces at d_faces + f * face_stride, in the current face layout.  Without one they are dense
+ *     [numplates][ps][ps] frames of the GLOBE's numplates (blinky_numplates): after a turn any plate of
+ *     the globe may be sampled, not only those of the installed lensmap, so a frame must hold
+ *     numplates * ps^2 bytes even when a supplied lensmap has fewer plates.
+ * Each pixel's ray (x, y, z) is turned in float32 with round-to-nearest and no fused multiply-add:
+ * t_k = (M[k][0]*x + M[k][1]*y) + M[k][2]*z.  Any matrix is accepted, a rotation or not.  The pixel then
+ * gets the entry blinky_set_raymap(W, H, ps, t) installs for it through the CURRENT globe (normalised,
+ * plate argmax over the globe's plates, lowest index winning ties; an on-grid texel gets no tint), and
+ * is written as blinky_warp_device_view writes that entry (RGBA: as
+ * blinky_warp_device_view_rgba_tables, with d_tables NULL meaning the blinky_set_rgba_table table):
+ * same view rectangle, keep_unmapped, background, f_rubix LUTs and per-frame tables.  In short, frame f
+ * equals blinky_set_raymap of the turned field followed by a one-frame view warp.  Nothing outside the
+ * view rectangle is written, and no pixel is read back.  The context does not change (lensmap, its
+ * plan, blinky_needs_rebuild, display flags, build_info); blinky_launch_count and blinky_last_kernel do.
+ * Refusals launch nothing: BLINKY_E_NODEVICE on a host-only context; BLINKY_E_STATE without a valid
+ * globe, when the globe picks its plates with a globe_plate script (use blinky_set_raymap_device), or
+ * when the installed lensmap's ps is beyond what blinky_set_raymap takes (6 * ps^2 > 0x0FFFFFFF, i.e.
+ * ps > 6688, which a supplied lensmap of fewer plates may have);
+ * BLINKY_E_INVALID for NULL faces, rays or screen, rays or matrices not 4-byte aligned, a nonzero
+ * ray_stride below 12*W*H or not a multiple of 4, a nonzero xform_stride below 36 or not a multiple of
+ * 4, more than 65535 frames, any check blinky_warp_device_view[_rgba_tables] makes, and a face layout
+ * in which any plate of the globe (not only those the lensmap shows) has no origin or does not fit.
+ * Both calls may be captured like blinky_warp_device_view: a replay reads the rays, matrices, tables,
+ * faces and screen at the pointers given at capture with their contents at replay time, the globe's
+ * plates, rubix grid, f_rubix, face layout and view of the capture, and the background and LUTs as
+ * the other warps do; blinky_release_captures covers these graphs too. */
+int blinky_warp_device_rays(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays,
+                            size_t ray_stride, const float *d_xforms, size_t xform_stride, void *d_screen,
+                            size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                            int keep_unmapped, void *stream);
+int blinky_warp_device_rays_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays,
+                                 size_t ray_stride, const float *d_xforms, size_t xform_stride,
+                                 void *d_screen_rgba, size_t screen_frame_stride, int rowbytes, int x0, int y0,
+                                 int nframes, int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
+                                 void *stream);
+
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
 const char *blinky_plan_summary(blinky_ctx *ctx);
