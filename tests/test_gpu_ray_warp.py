@@ -2,11 +2,13 @@
 equals blinky_set_raymap of the field turned in numpy float32 by M_f, followed by a one-frame blinky_warp_device_view of
 that frame, on a second context with the same globe, palette, background, rubix state and face layout.  Every byte of
 each output buffer is compared, the bytes outside the view included.  Covered: every kernel instance, face layouts,
-the transform forms, CUDA graphs, refusals and a 4K look-around."""
+the transform forms, CUDA graphs, refusals, a 4K look-around, adversarial rays and matrices on every argmax globe, the
+exported fields of extreme zooms, and the largest plate size a ray map takes."""
 import numpy as np
 import pytest
 
 from conftest import ALL_LENSES
+from test_raymap_host_only import adversarial_rays, u_one_rays
 
 pytestmark = pytest.mark.gpu
 
@@ -480,3 +482,143 @@ def test_4k_look_around(bb, torch, pair):
         ref.warp(d_faces, want)
         torch.cuda.synchronize()
         assert torch.equal(out[f], want), f
+
+
+# ---- adversarial rays, matrices and fields -----------------------------------------------------------------------
+
+ARGMAX_GLOBES = ["cube", "cube_corner", "cube_edge", "tetra", "trism"]
+
+
+def adversarial_matrices():
+    """zero, singular, +-inf and NaN entries, 1e30 and subnormal 1e-40 entries, and exact 90-degree turns that take
+    rays on plate edges and corners onto other plates' edges and corners"""
+    inf, nan = np.float32(np.inf), np.float32(np.nan)
+    perm = np.array([[0, 0, 1], [1, 0, 0], [0, 1, 0]], np.float32)          # x -> y -> z -> x
+    quarter = np.array([[0, 0, 1], [0, 1, 0], [-1, 0, 0]], np.float32)      # 90 degree yaw
+    half_flip = np.array([[-1, 0, 0], [0, 0, -1], [0, -1, 0]], np.float32)  # reflection through a plate diagonal
+    singular = np.array([[1, 2, 3], [2, 4, 6], [-1, 0.5, 0]], np.float32)
+    with_inf = np.eye(3, dtype=np.float32)
+    with_inf[0, 2] = inf
+    with_inf[1, 1] = -inf
+    with_nan = np.eye(3, dtype=np.float32)
+    with_nan[2, 0] = nan
+    huge = (np.eye(3) * 1e30).astype(np.float32)
+    huge[0, 1] = -1e30
+    tiny = np.full((3, 3), 1e-40, np.float32)
+    tiny[2, 2] = 1
+    return np.stack([np.zeros((3, 3), np.float32), singular, with_inf, with_nan, huge, tiny, perm, quarter, half_flip,
+                     np.eye(3, dtype=np.float32)])
+
+
+def adversarial_field(fe, ps, w, h):
+    """test_raymap_host_only's adversarial rays (zeros, -0, NaN, +-inf, subnormals, +-3e38, u or v exactly 0 or 1, u * ps
+    reaching ps, cube-corner ties) for the globe on `fe`, then the lens's own rays, as a [h, w, 3] field"""
+    slots = np.zeros((6, 11), np.float32)
+    pl = fe.plates()
+    slots[: len(pl)] = pl
+    rays = adversarial_rays(slots, len(pl), ps)
+    extra = np.array([[-3e38, 3e38, 1], [-0.0, -0.0, 1], [1, -0.0, 0], [np.float32(1e-45), 1, 0], [1, 1, np.nan]], np.float32)
+    rays = np.vstack([rays, extra])
+    field = fe.raymap(w, h).reshape(-1, 3)
+    assert len(rays) <= len(field), len(rays)
+    field[: len(rays)] = rays
+    return field.reshape(h, w, 3)
+
+
+@pytest.mark.parametrize("quad", [True, False])
+@pytest.mark.parametrize("globe", ARGMAX_GLOBES)
+def test_adversarial_rays_and_matrices(bb, torch, pair, globe, quad):
+    fe, ref = pair
+    setup(pair, globe=globe, rubix=True, grid=(4, 3.0, 2.0))
+    rays = adversarial_field(fe, PS, W, H)
+    xs = adversarial_matrices()
+    n = len(xs)
+    d_faces = faces_for(torch, fe, n)
+    scr = Screens(torch, n, False, x0=8 if quad else 3, y0=2, extra=12 if quad else 13)
+    check_batch(torch, fe, ref, rays, xs, d_faces, scr, quad, False, expect_kernel=f"ray_warp_kernel<quad={int(quad)},rubix=1")
+    # and not turned at all
+    check_batch(torch, fe, ref, rays, None, d_faces, scr, not quad, False, expect_kernel=f"ray_warp_kernel<quad={int(quad)},rubix=1")
+
+
+def warp_dense_against_the_rule(torch, fe, ref, rays, xs, w, h, ps, rgba=False):
+    """warp_rays into dense [n, h, w] screens (quads where w allows) against set_raymap + warp_view, frame by frame"""
+    n = len(xs)
+    bpp = 4 if rgba else 1
+    d_faces = torch.randint(0, 256, (n, fe.numplates * ps * ps), dtype=torch.uint8, device="cuda")
+    out = torch.full((n * h * w * bpp,), 77, dtype=torch.uint8, device="cuda")
+    fe.warp_rays(d_faces, out.data_ptr(), torch.from_numpy(rays).cuda(), torch.from_numpy(xs).cuda(), rowbytes=w * bpp,
+                 screen_stride=w * h * bpp, nframes=n, rgba=rgba)
+    torch.cuda.synchronize()
+    kernel = fe.last_kernel
+    got = out.cpu().numpy().reshape(n, -1)
+    for f in range(n):
+        with np.errstate(all="ignore"):
+            ref.set_raymap(np.ascontiguousarray(turned(rays, xs[f])), ps)
+        want = torch.full((h * w * bpp,), 77, dtype=torch.uint8, device="cuda")
+        ref.warp_view(d_faces[f:f + 1], want.data_ptr(), rowbytes=w * bpp, screen_stride=w * h * bpp, nframes=1, rgba=rgba)
+        torch.cuda.synchronize()
+        bad = np.nonzero(got[f] != want.cpu().numpy())[0]
+        assert bad.size == 0, (kernel, f, bad.size, bad[:8].tolist())
+    return kernel
+
+
+@pytest.mark.parametrize("lens,zoom,w,h", [("panini", "f_fov 360", 96, 64), ("mercator", "f_vfov 180", 96, 64),
+                                           ("fisheye1", "f_contain", 8, 640), ("cylinder", "f_vfov 180", 1000, 8)])
+def test_exported_fields_of_extreme_zooms(bb, torch, pair, lens, zoom, w, h):
+    """the fields the exports give at the sweep's extreme zooms (panini at an infinite scale: lens_inverse of +-inf and
+    NaN) turned by ordinary and adversarial matrices, rubix on with a non-default grid"""
+    fe, ref = pair
+    ps = 48
+    for c in pair:
+        c.set_rubixgrid(4, 3.0, 2.0)
+        c.command("f_globe cube_corner")
+        c.command(f"f_lens {lens}")
+        c.command(zoom)
+        c.set_rubix(True)
+        c.build_lensmap(w, h, ps, threads=1)
+        c.set_rgba_table(np.random.default_rng(2).integers(0, 2**32, 256, dtype=np.uint32))
+    d = torch.empty((h, w, 3), dtype=torch.float32, device="cuda")
+    fe.raymap(w, h, out=d)
+    rays = d.cpu().numpy()
+    xs = np.concatenate([matrices(4), adversarial_matrices()])
+    for rgba in (False, True):
+        kernel = warp_dense_against_the_rule(torch, fe, ref, rays, xs, w, h, ps, rgba=rgba)
+        assert f"quad={int(w % 4 == 0)}" in kernel, kernel
+
+
+def test_plate_size_at_the_texel_packing_limit(bb, torch, pair):
+    """ps 6688, the largest plate a ray map takes: rays reaching u * ps = ps and the texels px, py = 6687 at every plate
+    edge, in quads and per pixel"""
+    fe, ref = pair
+    ps = 6688
+    for c in pair:
+        c.set_rubixgrid(4, 3.0, 2.0)
+        c.command("f_globe cube")
+        c.set_rubix(True)
+    slots = fe.plates()
+    edge = u_one_rays(slots, len(slots), ps)
+    # v = 1 too: the same rays with the plate's right and up exchanged
+    flipped = []
+    for plate in range(len(slots)):
+        f, rt, up = (slots[plate][k:k + 3].astype(np.float64) for k in (0, 3, 6))
+        t = np.tan(float(np.float32(slots[plate][9]) / np.float32(2)))
+        for a in np.linspace(-0.9, 0.9, 5):
+            base = f - up * t + rt * a * t
+            flipped += [(base * (1 + k * 2.0 ** -24)).astype(np.float32) for k in range(-6, 7)]
+    rays = np.vstack([edge, np.array(flipped, np.float32)])
+    for w in (64, 62):
+        h = -(-len(rays) // w)
+        field = np.zeros((h * w, 3), np.float32)
+        field[: len(rays)] = rays
+        field[len(rays):] = [0, 0, 1]
+        field = field.reshape(h, w, 3)
+        for c in pair:
+            c.set_raymap(field, ps)
+        entries = fe.lensmap_packed().reshape(-1)
+        texel = entries & 0x0FFFFFFF
+        mapped = (entries >> 31) == 1
+        px, py = texel % ps, texel // ps % ps
+        assert (mapped & (px == ps - 1)).any() and (mapped & (py == ps - 1)).any()
+        xs = np.stack([np.eye(3, dtype=np.float32), adversarial_matrices()[6], adversarial_matrices()[7]])
+        kernel = warp_dense_against_the_rule(torch, fe, ref, field, xs, w, h, ps)
+        assert f"quad={int(w % 4 == 0)}" in kernel, kernel
