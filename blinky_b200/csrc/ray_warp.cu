@@ -1,7 +1,9 @@
 // The warp from a ray field turned by a per-frame matrix (blinky_warp_device_rays): each pixel's texel is computed on
 // the fly from its view ray, so a head-tracked look-around needs no lensmap, plan or install per frame — only the
 // matrix changes.  Frame f of the output equals blinky_set_raymap of the field turned by M_f followed by a one-frame
-// blinky_warp_device_view (ray_texel.h holds the per-ray arithmetic).
+// blinky_warp_device_view (ray_texel.h holds the per-ray arithmetic).  The supersampled warp
+// (blinky_warp_device_rays_supersampled, ray_supersample_kernel) writes each RGBA pixel as the rounded mean of the
+// colours of k x k such rays.
 //
 // Compiled with --fmad=false: the turn and the globe's float / double arithmetic must round operation by operation
 // as the host's -ffp-contract=off build does.
@@ -157,6 +159,103 @@ __global__ void __launch_bounds__(kRayThreads) ray_warp_kernel(const __grid_cons
     }
 }
 
+// --------------------------------------------------------------------------
+// Supersampled RGBA (blinky_warp_device_rays_supersampled): one thread per output pixel, whose K x K samples are the
+// field pixels (K x + i, K y + j) of a dense K W x K H field, each turned and mapped as ray_warp_kernel maps a pixel's
+// ray.  Sample j's row is 12 K contiguous bytes of the field, so a warp reads 384 K contiguous bytes per sub-row.  The
+// samples' colours are summed in two SWAR words (bytes 0 and 2, bytes 1 and 3, in 16-bit lanes: 16 * 255 fits) and each
+// byte written is (sum + K^2 / 2) / K^2.  With one field and one matrix for every frame of the thread, the K^2 packed
+// texels are mapped once and carried; otherwise each frame re-reads its rays (a shared field of a small view from the
+// caches; at 4K from HBM, which the per-sample arithmetic outweighs).
+// (The minimum of one block per SM lets ptxas size the registers to the instance: with the default it held K = 2 with
+// f_rubix to 64 registers and spilled.)
+// --------------------------------------------------------------------------
+template <int K, bool RUBIX, bool KEEP, bool TABLES>
+__global__ void __launch_bounds__(kRayThreads, 1) ray_supersample_kernel(const __grid_constant__ RayWarpParams p, const __grid_constant__ LensBuildParams P,
+                                                                      const __grid_constant__ FaceLayoutParams lay) {
+    constexpr int S = K * K;
+    __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
+    __shared__ uint32_t s_rgba[TABLES ? 1 : 256];
+    if (RUBIX) {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.lut);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(s_lut);
+        for (int i = threadIdx.x; i < 6 * 256 / 4; i += kRayThreads) dst[i] = __ldg(src + i);
+    }
+    if (!TABLES) {
+        for (int i = threadIdx.x; i < 256; i += kRayThreads) s_rgba[i] = __ldg(p.rgba + i);
+    }
+    if (RUBIX || !TABLES) __syncthreads();
+
+    const uint32_t pix = blockIdx.x * kRayThreads + threadIdx.x;   // y * W + x (WarpDevice::warp_rays: K^2 W H < 2^31)
+    if (pix >= p.nitems) return;
+    const uint32_t y = pix / p.width, x = pix - y * p.width;
+    const uint32_t fw = K * p.width;                                // field row, in field pixels
+    const uint32_t first = K * y * fw + K * x;                      // field pixel of sample (0, 0)
+    const size_t out_at = static_cast<size_t>(y) * p.pitch + static_cast<size_t>(x) * 4;
+    const int f0 = static_cast<int>(blockIdx.y) * p.frames_per_thread;
+    const int f1 = min(p.nframes, f0 + p.frames_per_thread);
+    const bool carry = p.ray_floats == 0 && p.xform_floats == 0;   // the texels are the same in every frame
+
+    // a sample's texel, packed as in ray_warp_kernel: px (bits 0-12), py (13-25), plate (26-28), on the grid (29), mapped (31)
+    constexpr uint32_t kMapped = 0x80000000u, kOnGrid = 0x20000000u;
+    uint32_t tx[S];
+    int mapped = 0;
+    for (int f = f0; f < f1; ++f) {
+        if (f == f0 || !carry) {
+            float M[9] = {};
+            if (p.xforms) {
+                const float *m = p.xforms + static_cast<size_t>(f) * p.xform_floats;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) M[i] = __ldg(m + i);
+            }
+            const float *field = p.rays + static_cast<size_t>(f) * p.ray_floats;
+            mapped = 0;
+#pragma unroll
+            for (int j = 0; j < K; ++j) {
+#pragma unroll
+                for (int i = 0; i < K; ++i) {
+                    const float *r = field + 3 * static_cast<size_t>(first + j * fw + i);
+                    const float ray[3] = {__ldg(r), __ldg(r + 1), __ldg(r + 2)};
+                    float t[3] = {ray[0], ray[1], ray[2]};
+                    if (p.xforms) turn_ray(M, ray, t);
+                    int plate = 0, px = 0, py = 0;
+                    tx[j * K + i] = 0;
+                    if (ray_texel(P, t, &plate, &px, &py)) {
+                        ++mapped;
+                        tx[j * K + i] = kMapped | static_cast<uint32_t>(plate) << 26 | static_cast<uint32_t>(py) << 13 | static_cast<uint32_t>(px);
+                    }
+                }
+            }
+            if (RUBIX) {
+#pragma unroll
+                for (int s = 0; s < S; ++s)
+                    if ((tx[s] & kMapped) && ray_on_rubix_grid(P, tx[s] & 0x1fffu, (tx[s] >> 13) & 0x1fffu)) tx[s] |= kOnGrid;
+            }
+        }
+        if (KEEP && mapped == 0) continue;
+        const uint8_t *faces = p.faces + static_cast<size_t>(f) * p.face_stride;
+        const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : nullptr;
+        const uint32_t bgb = mapped < S ? __ldg(p.bg + pix) : 0u;
+        uint32_t lo = 0, hi = 0;   // bytes 0 and 2, bytes 1 and 3 of the sum, in 16-bit lanes
+#pragma unroll
+        for (int s = 0; s < S; ++s) {
+            uint32_t b = bgb;
+            if (tx[s] & kMapped) {
+                const uint32_t plate = (tx[s] >> 26) & 7u;
+                b = ld_texel(faces + lay.plate_base[plate] + static_cast<size_t>((tx[s] >> 13) & 0x1fffu) * lay.rowbytes + (tx[s] & 0x1fffu));
+                if (RUBIX && !(tx[s] & kOnGrid)) b = s_lut[plate * 256 + b];
+            }
+            const uint32_t c = TABLES ? __ldg(table + b) : s_rgba[b];
+            lo += c & 0x00ff00ffu;
+            hi += (c >> 8) & 0x00ff00ffu;
+        }
+        constexpr uint32_t half = S / 2;
+        const uint32_t rgba = ((lo & 0xffffu) + half) / S | (((hi & 0xffffu) + half) / S) << 8 | (((lo >> 16) + half) / S) << 16 |
+                              (((hi >> 16) + half) / S) << 24;
+        st_cs_u32(p.out + static_cast<size_t>(f) * p.out_stride + out_at, rgba);
+    }
+}
+
 template <bool QUAD, bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 void launch_instance(const RayWarpParams &p, const LensBuildParams &P, const FaceLayoutParams &lay, dim3 grid, cudaStream_t st) {
     ray_warp_kernel<QUAD, RUBIX, RGBA, KEEP, TABLES><<<grid, kRayThreads, 0, st>>>(p, P, lay);
@@ -189,6 +288,31 @@ void launch_rubix(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cud
     else launch_rgba<QUAD, false>(L, p, grid, st);
 }
 
+// the supersampled instance of (factor, rubix, keep, tables): 3 x 2 x 2 x 2 = 24 instances
+template <int K, bool RUBIX, bool KEEP>
+void launch_supersample_tables(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.tables) ray_supersample_kernel<K, RUBIX, KEEP, true><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.layout);
+    else ray_supersample_kernel<K, RUBIX, KEEP, false><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.layout);
+}
+
+template <int K, bool RUBIX>
+void launch_supersample_keep(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.keep) launch_supersample_tables<K, RUBIX, true>(L, p, grid, st);
+    else launch_supersample_tables<K, RUBIX, false>(L, p, grid, st);
+}
+
+template <int K>
+void launch_supersample_rubix(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.rubix) launch_supersample_keep<K, true>(L, p, grid, st);
+    else launch_supersample_keep<K, false>(L, p, grid, st);
+}
+
+void launch_supersample(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    if (L.factor == 2) launch_supersample_rubix<2>(L, p, grid, st);
+    else if (L.factor == 3) launch_supersample_rubix<3>(L, p, grid, st);
+    else launch_supersample_rubix<4>(L, p, grid, st);
+}
+
 }  // namespace
 
 bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
@@ -208,17 +332,23 @@ bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
     p.pitch = L.pitch;
     p.width = static_cast<uint32_t>(L.width);
     const size_t npix = static_cast<size_t>(L.width) * static_cast<size_t>(L.height);
-    p.nitems = static_cast<uint32_t>(L.quads ? npix / 4 : npix);
+    p.nitems = static_cast<uint32_t>(L.quads ? npix / 4 : npix);   // (supersampled: one item per output pixel, never quads)
     p.nframes = L.nframes;
     p.frames_per_thread = L.frames_per_thread;
     const dim3 grid(static_cast<unsigned>((p.nitems + kRayThreads - 1) / kRayThreads),
                     static_cast<unsigned>((L.nframes + L.frames_per_thread - 1) / L.frames_per_thread));
     cudaStream_t st = static_cast<cudaStream_t>(L.stream);
-    if (L.quads) launch_rubix<true>(L, p, grid, st);
-    else launch_rubix<false>(L, p, grid, st);
     char buf[192];
-    snprintf(buf, sizeof buf, "ray_warp_kernel<quad=%d,rubix=%d,rgba=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d", L.quads, L.rubix,
-             L.rgba, L.keep, L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread);
+    if (L.factor > 1) {
+        launch_supersample(L, p, grid, st);
+        snprintf(buf, sizeof buf, "ray_supersample_kernel<k=%d,rubix=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d", L.factor, L.rubix,
+                 L.keep, L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread);
+    } else {
+        if (L.quads) launch_rubix<true>(L, p, grid, st);
+        else launch_rubix<false>(L, p, grid, st);
+        snprintf(buf, sizeof buf, "ray_warp_kernel<quad=%d,rubix=%d,rgba=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d", L.quads,
+                 L.rubix, L.rgba, L.keep, L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread);
+    }
     *name = buf;
     const cudaError_t e = cudaGetLastError();
     *cuda_err = static_cast<int>(e);

@@ -528,6 +528,44 @@ int blinky_warp_device_rays_rgba(blinky_ctx *ctx, const void *d_faces, size_t fa
                                  int nframes, int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
                                  void *stream);
 
+/* Anti-aliased RGBA warp from a ray field: k x k view rays per pixel (k = factor, 2, 3 or 4),
+ * box-filtered.  W, H, ps and the background are the installed lensmap's, as for
+ * blinky_warp_device_rays_rgba.  Frame f reads
+ *   - the field at d_rays + f * ray_stride bytes, a dense float32[k*H][k*W][3] field (ray_stride 0: one
+ *     field for every frame);
+ *   - the matrices and faces as blinky_warp_device_rays_rgba reads them;
+ *   - the 256-entry table T_f at d_tables + f * table_stride bytes, or the blinky_set_rgba_table table
+ *     when d_tables is NULL.
+ * Output pixel (x, y) has k^2 samples s = (i, j), 0 <= i, j < k.  Sample s is field pixel
+ * (k*x + i, k*y + j), turned by M_f exactly as blinky_warp_device_rays turns a ray, and gets the entry
+ * blinky_set_raymap(k*W, k*H, ps, turned field) installs for it through the current globe, with ps the
+ * installed lensmap's.  From the entry: byte b_s = the face texel (through the plate's rubix LUT when
+ * f_rubix is on and the texel is off the grid) if mapped, else bg[y][x], the OUTPUT pixel's background;
+ * colour c_s = T_f[b_s].  Byte n (0..3, little-endian) of the output word is
+ * (sum_s byte_n(c_s) + k^2/2) / k^2 in integers (k^2/2 rounds down: 4 for k = 3): round-half-up per
+ * channel, alpha averaged like the others.  The average is of the table's bytes as they are (gamma-
+ * encoded, as the tables are), not in linear light: so the rule stays a pure integer function of the
+ * one-sample warp.  With keep_unmapped a pixel none of whose k^2 samples is mapped is not written, and a
+ * partly mapped pixel is written with its unmapped samples taking the background colour.  Nothing
+ * outside the view rectangle is written, and no pixel is read back.  Equivalently, frame f is the k x k
+ * box average of blinky_warp_device_rays_rgba at k*W x k*H whose background is bg with each byte
+ * repeated k x k.
+ * Fields: blinky_get_raymap_device(ctx, k*W, k*H, ...) exports the current lens at the k-fold size.
+ * Sample i of pixel x then lies at about (x + i/k - W/2) * scale, so the box spans [x, x + (k-1)/k] and
+ * sits less than half a pixel off the one-sample warp's (x - W/2) * scale; a caller wanting centred
+ * boxes supplies its own field.
+ * Refuses everything blinky_warp_device_rays_rgba refuses, with the same codes, and launches nothing
+ * when it does; BLINKY_E_INVALID also when factor is not 2, 3 or 4 (k = 1 is
+ * blinky_warp_device_rays_rgba), a nonzero ray_stride is below 12*k^2*W*H, or k^2*W*H is beyond the
+ * kernel's 31-bit pixel index (2^31 - 1).  Capturable like blinky_warp_device_rays_rgba, on the same
+ * terms; the context does not change, blinky_launch_count and blinky_last_kernel do. */
+int blinky_warp_device_rays_supersampled(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
+                                         const float *d_rays, size_t ray_stride, const float *d_xforms,
+                                         size_t xform_stride, int factor, void *d_screen_rgba,
+                                         size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                                         int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
+                                         void *stream);
+
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
 const char *blinky_plan_summary(blinky_ctx *ctx);
