@@ -8,6 +8,7 @@ sentinels that differ.  Every byte of each output buffer is compared, the bytes 
 import numpy as np
 import pytest
 
+import ray_reference as rr
 from test_gpu_ray_warp import Screens, layouts, matrices, yaw
 
 pytestmark = pytest.mark.gpu
@@ -118,8 +119,28 @@ def run(torch, fe, k, d_faces, d_rays, d_x, scr, n, keep, tables=None):
     return out, fe.last_kernel
 
 
-def check(torch, fe, k, bg, d_faces, d_rays, d_x, scr, n, keep, tables=None, expect_kernel=None):
-    """the new call against the oracle, every byte of the screens; the kernel's description"""
+def by_reference(torch, host, k, bg, d_faces, d_rays, d_x, n, keep, tables=None, w=W, h=H, ps=PS, band=None):
+    """(avg, mapped) as oracle() gives them, by tests/ray_reference.py (no project kernel); host: its HostGlobe on the
+    globe, rubix state and grid of fe.  band: output rows at a time (the 4K fields)"""
+    faces, field = d_faces.cpu().numpy(), d_rays.cpu().numpy()
+    xs = None if d_x is None else d_x.cpu().numpy()
+    tabs = None if tables is None else tables.cpu().numpy().view(np.uint32)
+    band = band or h
+    avg = np.empty((n, h, w, 4), np.uint8)
+    mapped = np.empty((n, h, w), bool)
+    for f in range(n):
+        fld = field if field.ndim == 3 else field[f]
+        M = None if xs is None else (xs if xs.ndim == 2 else xs[f])
+        tab = TABLE if tabs is None else (tabs if tabs.ndim == 1 else tabs[f])
+        for y in range(0, h, band):
+            avg[f, y:y + band], mapped[f, y:y + band] = rr.frame(host, fld[k * y:k * (y + band)], M, faces[min(f, len(faces) - 1)],
+                                                                 bg.reshape(h, w)[y:y + band], k, ps, table=tab)
+    return torch.from_numpy(avg).cuda(), torch.from_numpy(mapped).cuda() if keep else None
+
+
+def check(torch, fe, k, bg, d_faces, d_rays, d_x, scr, n, keep, tables=None, expect_kernel=None, host=None):
+    """the new call against the oracle (and, given host, tests/ray_reference.py), every byte of the screens; the
+    kernel's description"""
     got, kernel = run(torch, fe, k, d_faces, d_rays, d_x, scr, n, keep, tables)
     if expect_kernel:
         assert kernel.startswith(expect_kernel), kernel
@@ -129,6 +150,10 @@ def check(torch, fe, k, bg, d_faces, d_rays, d_x, scr, n, keep, tables=None, exp
     want = expected(scr, avg, mapped, n)
     bad = (got != want).nonzero().flatten()
     assert bad.numel() == 0, (kernel, bad.numel(), bad[:8].tolist())
+    if host is not None:
+        want = expected(scr, *by_reference(torch, host, k, bg, d_faces, d_rays, d_x, n, keep, tables), n)
+        bad = (got != want).nonzero().flatten()
+        assert bad.numel() == 0, ("ray_reference", kernel, bad.numel(), bad[:8].tolist())
     return kernel
 
 
@@ -138,8 +163,9 @@ def check(torch, fe, k, bg, d_faces, d_rays, d_x, scr, n, keep, tables=None, exp
 @pytest.mark.parametrize("keep", [False, True])
 @pytest.mark.parametrize("rubix", [False, True])
 @pytest.mark.parametrize("k", [2, 3, 4])
-def test_every_instance_follows_the_rule(bb, torch, fe, k, rubix, keep, mode):
+def test_every_instance_follows_the_rule(bb, palette, torch, fe, k, rubix, keep, mode):
     bg = setup(fe, rubix=rubix)
+    host = rr.HostGlobe(bb, palette, "cube", rubix=rubix)
     n = 3
     d_rays = torch.from_numpy(field(fe, k)).cuda()
     d_x = torch.from_numpy(np.stack([yaw(0), yaw(29), yaw(-71)])).cuda()
@@ -150,7 +176,10 @@ def test_every_instance_follows_the_rule(bb, torch, fe, k, rubix, keep, mode):
         tables = torch.from_numpy(np.random.default_rng(8).integers(0, 2**31, 256).astype(np.int32)).cuda()
     scr = Screens(torch, n, True, x0=3, y0=5, extra=13)
     tag = f"ray_supersample_kernel<k={k},rubix={int(rubix)},keep={int(keep)},tables={int(mode == 'frames')}>"
-    check(torch, fe, k, bg, faces_for(torch, fe, n), d_rays, d_x, scr, n, keep, tables, expect_kernel=tag)
+    try:
+        check(torch, fe, k, bg, faces_for(torch, fe, n), d_rays, d_x, scr, n, keep, tables, expect_kernel=tag, host=host)
+    finally:
+        host.close()
 
 
 @pytest.mark.parametrize("keep", [False, True])
@@ -194,14 +223,15 @@ def test_per_frame_fields_one_matrix_and_no_matrix(bb, torch, fe):
 
 @pytest.mark.parametrize("form", ["per-frame-matrices", "one-matrix"])
 def test_small_view_large_batch_splits_the_frames(bb, torch, fe, form):
-    """400 frames of a 96 x 64 view sharing one field: the frames are split over rows of threads"""
+    """400 frames of a 96 x 64 view sharing one field: the frames are split over rows of threads.  Each frame has its
+    own faces (the warp and the oracle step through them by the dense frame size)."""
     bg = setup(fe)
     n = 400
     d_rays = torch.from_numpy(field(fe, 3)).cuda()
     distinct = matrices(5)
     d_x = torch.from_numpy(distinct[np.arange(n) % 5] if form == "per-frame-matrices" else distinct[1]).cuda()
     scr = Screens(torch, n, True, x0=3, y0=2, extra=13)
-    kernel = check(torch, fe, 3, bg, faces_for(torch, fe, 1), d_rays, d_x, scr, n, form == "one-matrix")
+    kernel = check(torch, fe, 3, bg, faces_for(torch, fe, n), d_rays, d_x, scr, n, form == "one-matrix")
     fpt = int(kernel.split("frames/thread=")[1])
     assert 1 < fpt < n, kernel
 
@@ -317,7 +347,7 @@ def test_refusals_launch_nothing(bb, torch, fe, palette, cuda_device):
 
 # ---- 4K ----------------------------------------------------------------------------------------------------------
 
-def test_4k_look_around_at_k2(bb, torch, fe):
+def test_4k_look_around_at_k2(bb, palette, torch, fe):
     """a 3-frame 4K look-around from the exported panini field at 7680 x 4320 (~400 MB)"""
     W4, H4, P4, k, n = 3840, 2160, 2048, 2, 3
     fe.command("f_globe cube")
@@ -336,3 +366,9 @@ def test_4k_look_around_at_k2(bb, torch, fe):
     assert fe.last_kernel.startswith("ray_supersample_kernel<k=2,rubix=0,keep=0,tables=0>"), fe.last_kernel
     avg, _ = oracle(torch, fe, k, bg, d_faces, d_rays, d_x, n, False, w=W4, h=H4, ps=P4)
     assert torch.equal(out, avg), int((out != avg).any(-1).sum())
+    host = rr.HostGlobe(bb, palette, "cube")
+    try:
+        avg, _ = by_reference(torch, host, k, bg, d_faces, d_rays, d_x, n, False, w=W4, h=H4, ps=P4, band=270)
+    finally:
+        host.close()
+    assert torch.equal(out, avg), ("ray_reference", int((out != avg).any(-1).sum()))
