@@ -1175,6 +1175,17 @@ int FisheyeHost::run_inverse_workers(int threads, int nitems, int *display, F it
     return rc;
 }
 
+template <class F>
+int FisheyeHost::settle_flagged(size_t n, int *display, F chunk) {
+    const size_t size = 256;
+    const int nchunks = static_cast<int>((n + size - 1) / size);
+    const int threads = n >= 4096 ? fallback_threads_ : 1;
+    return run_inverse_workers(threads, nchunks, display, [&](Worker &w, int i, int *disp) {
+        const size_t b = static_cast<size_t>(i) * size;
+        return chunk(w, b, std::min(n, b + size), disp);
+    });
+}
+
 LensBuildParams FisheyeHost::device_params(int width, int height, int platesize) const {
     LensBuildParams p;
     memset(&p, 0, sizeof p);
@@ -1243,12 +1254,8 @@ int FisheyeHost::build_inverse_device(int *display, std::string *why) {
         }
     }
     // the interpreter decides what the device could not
-    const int chunk = 256;
-    const int nitems = static_cast<int>((undecided.size() + chunk - 1) / chunk);
-    const int threads = undecided.size() >= 4096 ? fallback_threads_ : 1;
-    int rc = run_inverse_workers(threads, nitems, display, [&](Worker &w, int i, int *disp) {
-        const size_t b = static_cast<size_t>(i) * chunk;
-        return build_inverse_pixels(w, undecided.data() + b, std::min<size_t>(chunk, undecided.size() - b), disp);
+    int rc = settle_flagged(undecided.size(), display, [&](Worker &w, size_t b, size_t e, int *disp) {
+        return build_inverse_pixels(w, undecided.data() + b, e - b, disp);
     });
     char info[160];
     snprintf(info, sizeof info, "device: %zu of %zu pixels re-evaluated by the interpreter", undecided.size(), area);
@@ -1358,15 +1365,12 @@ int FisheyeHost::build_forward_device(std::string *why) {
     if (!device_builder_->forward_points(src, p, &undecided, &undecided_texels, why)) return 1;
     std::vector<ForwardPatch> patches(undecided.size());
     const int n1 = platesize_ + 1;
-    const int chunk = 256;
-    const int nitems = static_cast<int>((undecided.size() + chunk - 1) / chunk);
     int display_unused[kMaxPlates] = {0, 0, 0, 0, 0, 0};
     std::atomic<int> bad(0);
     // the workers only need lens_forward; the generic worker setup parks lens_inverse (may be nil: fine)
     lua_->set_global("__blinky_forward", fn_forward_);
-    int rc = run_inverse_workers(undecided.size() >= 4096 ? fallback_threads_ : 1, nitems, display_unused, [&](Worker &w, int item, int *) {
+    int rc = settle_flagged(undecided.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
         if (!w.forward.is_function()) w.forward = w.L->get_global("__blinky_forward");
-        const size_t b = static_cast<size_t>(item) * chunk, e = std::min(undecided.size(), b + chunk);
         for (size_t k = b; k < e; ++k) {
             const uint32_t pt = undecided[k];
             const int i = static_cast<int>(pt % n1), j = static_cast<int>(pt / n1 % n1), plate = static_cast<int>(pt / n1 / n1);
@@ -1386,9 +1390,7 @@ int FisheyeHost::build_forward_device(std::string *why) {
     std::vector<uint32_t> owner_patches(undecided_texels.size());
     if (!undecided_texels.empty()) {
         const int ps = platesize_;
-        const int ntexel_items = static_cast<int>((undecided_texels.size() + chunk - 1) / chunk);
-        rc = run_inverse_workers(undecided_texels.size() >= 4096 ? fallback_threads_ : 1, ntexel_items, display_unused, [&](Worker &w, int item, int *) {
-            const size_t b = static_cast<size_t>(item) * chunk, e = std::min(undecided_texels.size(), b + chunk);
+        rc = settle_flagged(undecided_texels.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
             for (size_t k = b; k < e; ++k) {
                 const uint32_t t = undecided_texels[k];
                 const int px = static_cast<int>(t % ps), py = static_cast<int>(t / ps % ps), plate = static_cast<int>(t / ps / ps);
@@ -1838,11 +1840,7 @@ int FisheyeHost::raymap_device(int width, int height, int platesize, const float
     // the interpreter decides what the device could not
     std::vector<RayPatch> patches(flagged.size());
     int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};  // (the planner derives the display flags from the finished map)
-    const int chunk = 256;
-    const int nitems = static_cast<int>((flagged.size() + chunk - 1) / chunk);
-    const int threads = flagged.size() >= 4096 ? fallback_threads_ : 1;
-    const int rc = run_inverse_workers(threads, nitems, display, [&](Worker &w, int i, int *disp) {
-        const size_t b = static_cast<size_t>(i) * chunk, e = std::min(flagged.size(), b + chunk);
+    const int rc = settle_flagged(flagged.size(), display, [&](Worker &w, size_t b, size_t e, int *disp) {
         for (size_t k = b; k < e; ++k) {
             float ray[3] = {flagged_rays[3 * k], flagged_rays[3 * k + 1], flagged_rays[3 * k + 2]};
             normalize3(ray);
@@ -1906,11 +1904,7 @@ int FisheyeHost::export_rays_device(int width, int height, double scale, float *
     // the interpreter evaluates what the device could not
     std::vector<RaySample> samples(flagged.size());
     int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
-    const int chunk = 256;
-    const int nitems = static_cast<int>((flagged.size() + chunk - 1) / chunk);
-    const int threads = flagged.size() >= 4096 ? fallback_threads_ : 1;
-    const int rc = run_inverse_workers(threads, nitems, display, [&](Worker &w, int i, int *) {
-        const size_t b = static_cast<size_t>(i) * chunk, e = std::min(flagged.size(), b + chunk);
+    const int rc = settle_flagged(flagged.size(), display, [&](Worker &w, size_t b, size_t e, int *) {
         for (size_t k = b; k < e; ++k) {
             const int ly = static_cast<int>(flagged[k] / static_cast<uint32_t>(width)), lx = static_cast<int>(flagged[k] % static_cast<uint32_t>(width));
             RaySample &s = samples[k];

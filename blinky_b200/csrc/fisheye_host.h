@@ -70,7 +70,7 @@ public:
     // lens translates (lua_transpile.h); pixels the device cannot decide exactly, and lenses
     // outside the translatable subset, go through the interpreter on `fallback_threads`.
     int build_lensmap(int width, int height, int platesize, int threads);
-    void set_device_builder(DeviceLensBuilder *b) { device_builder_ = b; }
+    void set_device_builder(LensDevice *b) { device_builder_ = b; }
     // host threads for the fallback evaluation and for the per-pixel passes after the map is known
     void set_worker_threads(int n) { fallback_threads_ = n < 1 ? 1 : n; }
     int worker_threads() const { return fallback_threads_; }
@@ -228,6 +228,10 @@ private:
     // runs item(w, i, display) for i in [0, nitems) over `threads` cloned script states
     template <class F>
     int run_inverse_workers(int threads, int nitems, int *display, F item);
+    // the interpreter's share of a device build: chunk(w, b, e, display) for the items [b, e) of n the device left to
+    // the host, 256 at a time, on one thread below 4096 items and on the fallback threads from there
+    template <class F>
+    int settle_flagged(size_t n, int *display, F chunk);
     int build_inverse(int threads);
     int build_inverse_device(int *display, std::string *why);  // 0 ok, -1 script failure, 1 = not possible (why)
     int build_forward_device(std::string *why);                // same convention
@@ -246,7 +250,7 @@ private:
     std::unique_ptr<minilua::State> lua_;
     minilua::Value fn_inverse_, fn_forward_, fn_globe_plate_;  // registry refs, :328-332
 
-    DeviceLensBuilder *device_builder_ = nullptr;  // not owned
+    LensDevice *device_builder_ = nullptr;  // not owned
     int fallback_threads_ = 1;
     std::string build_info_;
 

@@ -373,23 +373,29 @@ Driver &driver() {
 
 }  // namespace
 
+// one loaded unit, unloaded when its owner goes
 struct LensDevice::Module {
     CUmodule mod = nullptr;
     CUfunction fn = nullptr;
     CUfunction owner_fn = nullptr;  // forward modules of globes with a globe_plate script
+    Module() = default;
+    Module(const Module &) = delete;
+    Module &operator=(const Module &) = delete;
+    ~Module() {
+        if (mod) driver().ModuleUnload(mod);
+    }
 };
 
 // device buffers that live between forward_points() and forward_finish()
 struct LensDevice::ForwardState {
     LensBuildParams p;
-    size_t npoints = 0;
-    FwdPoint *grid = nullptr;
-    unsigned char *status = nullptr;
-    unsigned *undecided = nullptr;
-    unsigned *counters = nullptr;  // [0] undecided points, [1] nil results, [2] messages, [3..8] display flags, [9] undecided owners
+    DeviceBuffer grid;       // FwdPoint[npoints]
+    DeviceBuffer status;     // unsigned char[npoints]
+    DeviceBuffer undecided;  // unsigned[kUndecidedCap]
+    DeviceBuffer counters;   // unsigned[16]: [0] undecided points, [1] nil results, [2] messages, [3..8] display flags, [9] undecided owners
     unsigned nil_count = 0;
-    unsigned char *owner = nullptr;       // [numplates * ps * ps] texel owners; nullptr: the plate argmax decides
-    unsigned *owner_undecided = nullptr;
+    DeviceBuffer owner;            // [numplates * ps * ps] texel owners; empty: the plate argmax decides
+    DeviceBuffer owner_undecided;  // unsigned[kUndecidedCap]
 };
 
 namespace {
@@ -449,29 +455,83 @@ __global__ void fwd_resolve_kernel(const unsigned *__restrict__ idxkey, const un
     if (at < npix) fwd_resolve_pixel(idxkey, tintkey, idx, tint, at, ps);
 }
 
+// true when ce is cudaSuccess; otherwise false with "what: <CUDA error>" in *err
+bool checked(cudaError_t ce, const char *what, std::string *err) {
+    if (ce != cudaSuccess) *err = std::string(what) + ": " + cudaGetErrorString(ce);
+    return ce == cudaSuccess;
+}
+
+cudaError_t allocate(DeviceBuffer *b, size_t bytes) { return static_cast<cudaError_t>(b->alloc(bytes)); }
+
+// a device copy of v, copied on `s`: the caller synchronises `s` before v may change or go
+template <typename T>
+DeviceBuffer upload(const std::vector<T> &v, cudaStream_t s, cudaError_t *ce) {
+    DeviceBuffer d;
+    *ce = allocate(&d, v.size() * sizeof(T));
+    if (*ce == cudaSuccess) *ce = cudaMemcpyAsync(d.get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, s);
+    return d;
+}
+
+// launches a kernel of a compiled unit, `block` threads per block, on `s`
+bool launch(CUfunction fn, dim3 grid, unsigned block, cudaStream_t s, void **args, std::string *err) {
+    const CUresult cr = driver().LaunchKernel(fn, grid.x, grid.y, grid.z, block, 1, 1, 0, s, args, nullptr);
+    if (cr != CUDA_SUCCESS) *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
+    return cr == CUDA_SUCCESS;
+}
+
+// A list a kernel filled for the host, read back on `s`: the count at d_count, then that many entries of d_list, into
+// *out.  False with the reason in *err on a CUDA error (what: the kernel, for the message) or when more than
+// kUndecidedCap items (a plural noun) need the interpreter.
+bool read_list(const unsigned *d_count, const unsigned *d_list, cudaStream_t s, const char *what, const char *items,
+               std::vector<uint32_t> *out, std::string *err) {
+    unsigned n = 0;
+    cudaError_t ce = cudaMemcpyAsync(&n, d_count, sizeof n, cudaMemcpyDeviceToHost, s);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+    if (!checked(ce, what, err)) return false;
+    if (n > kUndecidedCap) {
+        *err = std::string("too many ") + items + " need the interpreter (" + std::to_string(n) + ")";
+        return false;
+    }
+    out->resize(n);
+    if (n == 0) return true;
+    ce = cudaMemcpyAsync(out->data(), d_list, n * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+    return checked(ce, what, err);
+}
+
+// two events around a window of work on one stream
+class EventTimer {
+public:
+    EventTimer() {
+        created_ = cudaEventCreate(&begin_);
+        if (created_ == cudaSuccess) created_ = cudaEventCreate(&end_);
+    }
+    EventTimer(const EventTimer &) = delete;
+    EventTimer &operator=(const EventTimer &) = delete;
+    ~EventTimer() {
+        if (begin_) cudaEventDestroy(begin_);
+        if (end_) cudaEventDestroy(end_);
+    }
+    // opens the window: the error of creating the events or of recording the first
+    cudaError_t start(cudaStream_t s) { return created_ == cudaSuccess ? cudaEventRecord(begin_, s) : created_; }
+    void stop(cudaStream_t s) { cudaEventRecord(end_, s); }
+    // the window's milliseconds, once the stream is past stop()
+    float ms() const {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, begin_, end_);
+        return ms;
+    }
+
+private:
+    cudaEvent_t begin_ = nullptr, end_ = nullptr;
+    cudaError_t created_;
+};
+
 }  // namespace
 
-LensDevice::~LensDevice() {
-    drop_forward_state();
-    cudaFree(ray_flagged_);
-    cudaFree(ray_map_);
-    for (auto &kv : cache_) {
-        if (kv.second->mod && driver().ok) driver().ModuleUnload(kv.second->mod);
-        delete kv.second;
-    }
-}
+LensDevice::LensDevice(int device) : device_(device) {}
 
-void LensDevice::drop_forward_state() {
-    if (!fwd_) return;
-    cudaFree(fwd_->grid);
-    cudaFree(fwd_->status);
-    cudaFree(fwd_->undecided);
-    cudaFree(fwd_->counters);
-    cudaFree(fwd_->owner);
-    cudaFree(fwd_->owner_undecided);
-    delete fwd_;
-    fwd_ = nullptr;
-}
+LensDevice::~LensDevice() = default;
 
 std::string LensDevice::kernel_tail(bool forward, bool globe_plate) {
     if (forward) return globe_plate ? std::string(kForwardKernelSource) + kForwardOwnerKernelSource : std::string(kForwardKernelSource);
@@ -529,7 +589,21 @@ bool LensDevice::compile_unit(const std::string &src, std::vector<char> *cubin, 
 }
 
 LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit, std::string *err) {
+    // per unit (in Unit's order): the letter of its cache keys, the kernel it launches and the tail appended to source
+    static const struct {
+        char key;
+        const char *entry;
+        std::string (*tail)(const std::string &source);
+    } kUnits[] = {
+        {'I', "lt_build", [](const std::string &s) { return kernel_tail(false, source_has_globe_plate(s)); }},
+        {'F', "lt_forward_points", [](const std::string &s) { return kernel_tail(true, source_has_globe_plate(s)); }},
+        {'R', "lt_raymap", [](const std::string &s) { return raymap_tail(source_has_globe_plate(s)); }},
+        {'E', "lt_rays", [](const std::string &) { return rays_tail(); }},
+        {'P', "lt_probe", [](const std::string &) { return probe_tail(); }},
+    };
+    const auto &u = kUnits[unit];
     compile_ms_ = 0;
+    // (since CUDA 12 this also makes the device's primary context current, which cuModuleLoadData needs)
     if (cudaSetDevice(device_) != cudaSuccess) {
         *err = "cudaSetDevice failed";
         return nullptr;
@@ -539,43 +613,29 @@ LensDevice::Module *LensDevice::module_for(const std::string &source, Unit unit,
         *err = "CUDA driver entry points unavailable";
         return nullptr;
     }
-    const std::string cache_key = "IFREP"[unit] + source;
+    const std::string cache_key = u.key + source;
     auto it = cache_.find(cache_key);
-    if (it != cache_.end()) return it->second;
+    if (it != cache_.end()) return it->second.get();
     auto t0 = std::chrono::steady_clock::now();
     std::vector<char> cubin;
     std::string log;
-    const bool compiled = unit == kRaymapUnit ? compile_unit(source + raymap_tail(source_has_globe_plate(source)), &cubin, &log)
-                          : unit == kRaysUnit ? compile_unit(source + rays_tail(), &cubin, &log)
-                          : unit == kProbeUnit ? compile_unit(source + probe_tail(), &cubin, &log)
-                                              : compile(source, unit == kForwardUnit, &cubin, &log);
-    if (!compiled) {
+    if (!compile_unit(source + u.tail(source), &cubin, &log)) {
         *err = log;
         return nullptr;
     }
-    cudaFree(nullptr);  // make sure the primary context is current
-    Module *m = new Module;
+    auto m = std::make_unique<Module>();
     CUresult cr = d.ModuleLoadData(&m->mod, cubin.data());
-    const char *entry = unit == kForwardUnit ? "lt_forward_points" : unit == kRaymapUnit ? "lt_raymap" : unit == kRaysUnit ? "lt_rays"
-                        : unit == kProbeUnit ? "lt_probe" : "lt_build";
-    if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, entry);
+    if (cr == CUDA_SUCCESS) cr = d.ModuleGetFunction(&m->fn, m->mod, u.entry);
     if (cr == CUDA_SUCCESS && unit == kForwardUnit && source_has_globe_plate(source)) cr = d.ModuleGetFunction(&m->owner_fn, m->mod, "lt_forward_owner");
     if (cr != CUDA_SUCCESS) {
-        if (m->mod) d.ModuleUnload(m->mod);
-        delete m;
         *err = "loading the compiled lens failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
         return nullptr;
     }
-    if (cache_.size() >= 16) {  // lenses are few; keep the cache from growing without bound
-        for (auto &kv : cache_) {
-            d.ModuleUnload(kv.second->mod);
-            delete kv.second;
-        }
-        cache_.clear();
-    }
-    cache_[cache_key] = m;
+    if (cache_.size() >= 16) cache_.clear();  // lenses are few; keep the cache from growing without bound
+    Module *loaded = m.get();
+    cache_[cache_key] = std::move(m);
     compile_ms_ = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    return m;
+    return loaded;
 }
 
 bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) {
@@ -586,41 +646,20 @@ bool LensDevice::build(const std::string &lens_source, const LensBuildParams &p,
     }
     Module *m = module_for(lens_source, kInverseUnit, err);
     if (!m) return false;
-    Driver &d = driver();
     const size_t npix = static_cast<size_t>(p.width) * p.height;
-    uint32_t *d_cand = nullptr;
-    cudaError_t ce = cudaMalloc(&d_cand, npix * sizeof(uint32_t));
-    if (ce != cudaSuccess) {
-        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
-        return false;
-    }
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    DeviceBuffer d_cand;
+    if (!checked(allocate(&d_cand, npix * sizeof(uint32_t)), "cudaMalloc", err)) return false;
+    EventTimer timer;
+    if (!checked(timer.start(nullptr), "lens kernel", err)) return false;
     LensBuildParams params = p;
-    void *args[] = {&params, &d_cand};
+    uint32_t *out = d_cand.as<uint32_t>();
+    void *args[] = {&params, &out};
     const unsigned block = 128;
-    cudaEventRecord(e0, nullptr);
-    CUresult cr = d.LaunchKernel(m->fn, (p.width + block - 1) / block, static_cast<unsigned>(p.height), 1, block, 1, 1, 0, nullptr, args, nullptr);
-    cudaEventRecord(e1, nullptr);
-    bool ok = cr == CUDA_SUCCESS;
-    if (!ok) *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
-    if (ok) {
-        ce = cudaMemcpy(cand, d_cand, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost);  // synchronises
-        if (ce != cudaSuccess) {
-            *err = std::string("lens kernel: ") + cudaGetErrorString(ce);
-            ok = false;
-        } else {
-            float ms = 0;
-            cudaEventElapsedTime(&ms, e0, e1);
-            kernel_ms_ = ms;
-            ++launches_;
-        }
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(d_cand);
-    return ok;
+    if (!launch(m->fn, dim3((p.width + block - 1) / block, p.height), block, nullptr, args, err)) return false;
+    timer.stop(nullptr);
+    if (!checked(cudaMemcpy(cand, out, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost), "lens kernel", err)) return false;  // synchronises
+    kernel_ms_ = timer.ms();
+    return true;
 }
 
 bool LensDevice::raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
@@ -635,102 +674,54 @@ bool LensDevice::raymap(const std::string &globe_source, const LensBuildParams &
     if (!m) return false;
     // kept for the context's later ray maps: the look-around loop makes one per frame
     cudaError_t ce = cudaSuccess;
-    if (!ray_flagged_) ce = cudaMalloc(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned));
+    if (!ray_flagged_.get()) ce = allocate(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned));
     if (ce == cudaSuccess && ray_map_pixels_ < npix) {
-        cudaFree(ray_map_);
-        ray_map_ = nullptr;
         ray_map_pixels_ = 0;
-        ce = cudaMalloc(&ray_map_, npix * sizeof(uint32_t));
+        ce = allocate(&ray_map_, npix * sizeof(uint32_t));
         if (ce == cudaSuccess) ray_map_pixels_ = npix;
     }
-    if (ce != cudaSuccess) {
-        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
-        return false;
-    }
-    *d_map = ray_map_;
+    if (!checked(ce, "cudaMalloc", err)) return false;
+    uint32_t *map = ray_map_.as<uint32_t>();
+    *d_map = map;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    EventTimer timer;
     LensBuildParams params = p;
-    unsigned *count = ray_flagged_, *list = ray_flagged_ + 1;
+    unsigned *count = ray_flagged_.as<unsigned>(), *list = count + 1;
     unsigned cap = kUndecidedCap;
-    void *args[] = {&params, &d_rays, &ray_map_, &list, &count, &cap};
+    void *args[] = {&params, &d_rays, &map, &list, &count, &cap};
     const unsigned block = 256;
-    unsigned n = 0;
-    bool ok = true;
     ce = cudaMemsetAsync(count, 0, sizeof(unsigned), s);
+    if (ce == cudaSuccess) ce = timer.start(s);
+    if (!checked(ce, "ray map kernel", err)) return false;
+    if (!launch(m->fn, dim3(static_cast<unsigned>((npix + block - 1) / block)), block, s, args, err)) return false;
+    timer.stop(s);
+    if (!read_list(count, list, s, "ray map kernel", "pixels", flagged, err)) return false;
+    kernel_ms_ = timer.ms();
+    const unsigned n = static_cast<unsigned>(flagged->size());
+    flagged_rays->resize(3 * static_cast<size_t>(n));
+    if (n == 0) return true;
+    // only the flagged pixels' rays come back
+    DeviceBuffer d_gathered;
+    ce = allocate(&d_gathered, flagged_rays->size() * sizeof(float));
     if (ce == cudaSuccess) {
-        cudaEventRecord(e0, s);
-        const CUresult cr = driver().LaunchKernel(m->fn, static_cast<unsigned>((npix + block - 1) / block), 1, 1, block, 1, 1, 0, s, args, nullptr);
-        cudaEventRecord(e1, s);
-        if (cr != CUDA_SUCCESS) {
-            *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
-            ok = false;
-        }
+        gather_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, list, n, d_gathered.as<float>());
+        ce = cudaMemcpyAsync(flagged_rays->data(), d_gathered.get(), flagged_rays->size() * sizeof(float), cudaMemcpyDeviceToHost, s);
     }
-    if (ok) {
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&n, count, sizeof n, cudaMemcpyDeviceToHost, s);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-        if (ce != cudaSuccess) {
-            *err = std::string("ray map kernel: ") + cudaGetErrorString(ce);
-            ok = false;
-        }
-    }
-    if (ok && n > kUndecidedCap) {
-        *err = "too many pixels need the interpreter (" + std::to_string(n) + ")";
-        ok = false;
-    }
-    if (ok) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        kernel_ms_ = ms;
-        ++launches_;
-        flagged->resize(n);
-        flagged_rays->resize(3 * static_cast<size_t>(n));
-    }
-    if (ok && n) {
-        // only the flagged pixels' rays come back
-        float *d_gathered = nullptr;
-        ce = cudaMalloc(&d_gathered, 3 * static_cast<size_t>(n) * sizeof(float));
-        if (ce == cudaSuccess) {
-            gather_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, list, n, d_gathered);
-            ++launches_;
-            ce = cudaMemcpyAsync(flagged->data(), list, n * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
-            if (ce == cudaSuccess) ce = cudaMemcpyAsync(flagged_rays->data(), d_gathered, flagged_rays->size() * sizeof(float), cudaMemcpyDeviceToHost, s);
-            if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-            cudaFree(d_gathered);
-        }
-        if (ce != cudaSuccess) {
-            *err = std::string("ray map gather: ") + cudaGetErrorString(ce);
-            ok = false;
-        }
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    return ok;
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+    return checked(ce, "ray map gather", err);
 }
 
 bool LensDevice::patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) {
     if (patches.empty()) return true;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    RayPatch *d_patches = nullptr;
-    cudaError_t ce = cudaMalloc(&d_patches, patches.size() * sizeof(RayPatch));
+    cudaError_t ce;
+    const DeviceBuffer d_patches = upload(patches, s, &ce);
     if (ce == cudaSuccess) {
-        ce = cudaMemcpyAsync(d_patches, patches.data(), patches.size() * sizeof(RayPatch), cudaMemcpyHostToDevice, s);
-        if (ce == cudaSuccess) {
-            const unsigned n = static_cast<unsigned>(patches.size());
-            scatter_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(ray_map_, d_patches, n);
-            ++launches_;
-            ce = cudaStreamSynchronize(s);  // (patches is pageable host memory the copy may still read)
-        }
-        cudaFree(d_patches);
+        const unsigned n = static_cast<unsigned>(patches.size());
+        scatter_entries_kernel<<<(n + 255) / 256, 256, 0, s>>>(ray_map_.as<uint32_t>(), d_patches.as<RayPatch>(), n);
+        ce = cudaStreamSynchronize(s);  // (patches is pageable host memory the copy may still read)
     }
-    if (ce != cudaSuccess) {
-        *err = std::string("ray map patch: ") + cudaGetErrorString(ce);
-        return false;
-    }
-    return true;
+    return checked(ce, "ray map patch", err);
 }
 
 bool LensDevice::copy_to_host(void *dst, const void *d_src, size_t bytes, void *stream, std::string *err) {
@@ -738,8 +729,7 @@ bool LensDevice::copy_to_host(void *dst, const void *d_src, size_t bytes, void *
     cudaError_t ce = cudaSetDevice(device_);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, s);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-    if (ce != cudaSuccess) *err = std::string("copying the rays to the host: ") + cudaGetErrorString(ce);
-    return ce == cudaSuccess;
+    return checked(ce, "copying the rays to the host", err);
 }
 
 bool LensDevice::copy_to_device(void *d_dst, const void *src, size_t bytes, void *stream, std::string *err) {
@@ -747,8 +737,7 @@ bool LensDevice::copy_to_device(void *d_dst, const void *src, size_t bytes, void
     cudaError_t ce = cudaSetDevice(device_);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_dst, src, bytes, cudaMemcpyHostToDevice, s);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);  // (src is pageable host memory the copy may still read)
-    if (ce != cudaSuccess) *err = std::string("copying the rays to the device: ") + cudaGetErrorString(ce);
-    return ce == cudaSuccess;
+    return checked(ce, "copying the rays to the device", err);
 }
 
 bool LensDevice::capturing(void *stream) {
@@ -765,15 +754,8 @@ bool LensDevice::probe_math(const std::string &prelude, int op, const double *d_
     unsigned long long count = n;
     void *args[] = {&op, &d_a, &d_b, &d_v, &d_e, &count};
     const unsigned block = 256;
-    const CUresult cr = driver().LaunchKernel(m->fn, static_cast<unsigned>((n + block - 1) / block), 1, 1, block, 1, 1, 0, s, args, nullptr);
-    if (cr != CUDA_SUCCESS) {
-        *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
-        return false;
-    }
-    ++launches_;
-    const cudaError_t ce = cudaStreamSynchronize(s);
-    if (ce != cudaSuccess) *err = std::string("math probe: ") + cudaGetErrorString(ce);
-    return ce == cudaSuccess;
+    if (!launch(m->fn, dim3(static_cast<unsigned>((n + block - 1) / block)), block, s, args, err)) return false;
+    return checked(cudaStreamSynchronize(s), "math probe", err);
 }
 
 bool LensDevice::rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
@@ -789,218 +771,130 @@ bool LensDevice::rays(const std::string &lens_source, const LensBuildParams &p, 
     }
     Module *m = module_for(lens_source, kRaysUnit, err);
     if (!m) return false;
-    cudaError_t ce = cudaSuccess;
-    if (!ray_flagged_) ce = cudaMalloc(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned));
-    if (ce != cudaSuccess) {
-        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
+    if (!ray_flagged_.get() && !checked(allocate(&ray_flagged_, (1 + static_cast<size_t>(kUndecidedCap)) * sizeof(unsigned)), "cudaMalloc", err))
         return false;
-    }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    EventTimer timer;
     LensBuildParams params = p;
-    unsigned *count = ray_flagged_, *list = ray_flagged_ + 1;
+    unsigned *count = ray_flagged_.as<unsigned>(), *list = count + 1;
     unsigned cap = kUndecidedCap;
     void *args[] = {&params, &d_rays, &list, &count, &cap};
     const unsigned block = 128;
-    unsigned n = 0;
-    bool ok = true;
-    ce = cudaMemsetAsync(count, 0, sizeof(unsigned), s);
-    if (ce == cudaSuccess) {
-        cudaEventRecord(e0, s);
-        const CUresult cr = driver().LaunchKernel(m->fn, (p.width + block - 1) / block, static_cast<unsigned>(p.height), 1, block, 1, 1, 0, s, args, nullptr);
-        cudaEventRecord(e1, s);
-        if (cr != CUDA_SUCCESS) {
-            *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
-            ok = false;
-        }
-    }
-    if (ok) {
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&n, count, sizeof n, cudaMemcpyDeviceToHost, s);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-        if (ce != cudaSuccess) {
-            *err = std::string("ray export kernel: ") + cudaGetErrorString(ce);
-            ok = false;
-        }
-    }
-    if (ok && n > kUndecidedCap) {
-        *err = "too many pixels need the interpreter (" + std::to_string(n) + ")";
-        ok = false;
-    }
-    if (ok) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        kernel_ms_ = ms;
-        ++launches_;
-        flagged->resize(n);
-        if (n) ce = cudaMemcpyAsync(flagged->data(), list, n * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
-        if (n && ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-        if (ce != cudaSuccess) {
-            *err = std::string("ray export flagged list: ") + cudaGetErrorString(ce);
-            ok = false;
-        }
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    return ok;
+    cudaError_t ce = cudaMemsetAsync(count, 0, sizeof(unsigned), s);
+    if (ce == cudaSuccess) ce = timer.start(s);
+    if (!checked(ce, "ray export kernel", err)) return false;
+    if (!launch(m->fn, dim3((p.width + block - 1) / block, p.height), block, s, args, err)) return false;
+    timer.stop(s);
+    if (!read_list(count, list, s, "ray export kernel", "pixels", flagged, err)) return false;
+    kernel_ms_ = timer.ms();
+    return true;
 }
 
 bool LensDevice::patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) {
     if (samples.empty()) return true;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    RaySample *d_samples = nullptr;
-    cudaError_t ce = cudaMalloc(&d_samples, samples.size() * sizeof(RaySample));
+    cudaError_t ce;
+    const DeviceBuffer d_samples = upload(samples, s, &ce);
     if (ce == cudaSuccess) {
-        ce = cudaMemcpyAsync(d_samples, samples.data(), samples.size() * sizeof(RaySample), cudaMemcpyHostToDevice, s);
-        if (ce == cudaSuccess) {
-            const unsigned n = static_cast<unsigned>(samples.size());
-            scatter_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, d_samples, n);
-            ++launches_;
-            ce = cudaStreamSynchronize(s);  // (samples is pageable host memory the copy may still read)
-        }
-        cudaFree(d_samples);
+        const unsigned n = static_cast<unsigned>(samples.size());
+        scatter_rays_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rays, d_samples.as<RaySample>(), n);
+        ce = cudaStreamSynchronize(s);  // (samples is pageable host memory the copy may still read)
     }
-    if (ce != cudaSuccess) {
-        *err = std::string("ray export patch: ") + cudaGetErrorString(ce);
-        return false;
-    }
-    return true;
+    return checked(ce, "ray export patch", err);
 }
 
 bool LensDevice::forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
                                 std::vector<uint32_t> *undecided_texels, std::string *err) {
     undecided_texels->clear();
     kernel_ms_ = 0;
-    drop_forward_state();
+    fwd_.reset();
     Module *m = module_for(lens_source, kForwardUnit, err);
     if (!m) return false;
-    Driver &d = driver();
     const size_t n1 = static_cast<size_t>(p.platesize) + 1;
     const size_t npoints = static_cast<size_t>(p.numplates) * n1 * n1;
     if (npoints >= 0xFFFFFFFFull) {
         *err = "too many grid points";
         return false;
     }
-    fwd_ = new ForwardState;
-    fwd_->p = p;
-    fwd_->npoints = npoints;
-    cudaError_t ce = cudaMalloc(&fwd_->grid, npoints * sizeof(FwdPoint));
-    if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->status, npoints);
-    if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->undecided, kUndecidedCap * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->counters, 16 * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = cudaMemset(fwd_->counters, 0, 16 * sizeof(unsigned));
+    auto f = std::make_unique<ForwardState>();
+    f->p = p;
+    cudaError_t ce = allocate(&f->grid, npoints * sizeof(FwdPoint));
+    if (ce == cudaSuccess) ce = allocate(&f->status, npoints);
+    if (ce == cudaSuccess) ce = allocate(&f->undecided, kUndecidedCap * sizeof(unsigned));
+    if (ce == cudaSuccess) ce = allocate(&f->counters, 16 * sizeof(unsigned));
+    if (ce == cudaSuccess) ce = cudaMemset(f->counters.get(), 0, 16 * sizeof(unsigned));
     const size_t ntexels = static_cast<size_t>(p.numplates) * p.platesize * p.platesize;
     if (m->owner_fn) {
-        if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->owner, ntexels);
-        if (ce == cudaSuccess) ce = cudaMalloc(&fwd_->owner_undecided, kUndecidedCap * sizeof(unsigned));
+        if (ce == cudaSuccess) ce = allocate(&f->owner, ntexels);
+        if (ce == cudaSuccess) ce = allocate(&f->owner_undecided, kUndecidedCap * sizeof(unsigned));
     }
-    if (ce != cudaSuccess) {
-        *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce);
-        drop_forward_state();
-        return false;
-    }
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    if (!checked(ce, "cudaMalloc", err)) return false;
+    EventTimer timer;
+    if (!checked(timer.start(nullptr), "lens kernel", err)) return false;
     LensBuildParams params = p;
     unsigned cap = kUndecidedCap;
-    void *args[] = {&params, &fwd_->grid, &fwd_->status, &fwd_->undecided, &fwd_->counters, &cap};
+    FwdPoint *grid = f->grid.as<FwdPoint>();
+    unsigned char *status = f->status.as<unsigned char>(), *owner = f->owner.as<unsigned char>();
+    unsigned *counters = f->counters.as<unsigned>(), *points = f->undecided.as<unsigned>(), *texels = f->owner_undecided.as<unsigned>();
+    void *args[] = {&params, &grid, &status, &points, &counters, &cap};
     const unsigned block = 128;
-    cudaEventRecord(e0, nullptr);
-    CUresult cr = d.LaunchKernel(m->fn, static_cast<unsigned>((n1 + block - 1) / block), static_cast<unsigned>(n1), static_cast<unsigned>(p.numplates), block, 1, 1, 0,
-                                 nullptr, args, nullptr);
-    if (cr == CUDA_SUCCESS && m->owner_fn) {
-        unsigned *owner_counter = fwd_->counters + 9;
-        void *oargs[] = {&params, &fwd_->owner, &fwd_->owner_undecided, &owner_counter, &cap};
+    if (!launch(m->fn, dim3(static_cast<unsigned>((n1 + block - 1) / block), static_cast<unsigned>(n1), static_cast<unsigned>(p.numplates)), block,
+                nullptr, args, err))
+        return false;
+    if (m->owner_fn) {
+        unsigned *owner_counter = counters + 9;
+        void *oargs[] = {&params, &owner, &texels, &owner_counter, &cap};
         const unsigned ps = static_cast<unsigned>(p.platesize);
-        cr = d.LaunchKernel(m->owner_fn, (ps + block - 1) / block, ps, static_cast<unsigned>(p.numplates), block, 1, 1, 0, nullptr, oargs, nullptr);
-        if (cr == CUDA_SUCCESS) ++launches_;
+        if (!launch(m->owner_fn, dim3((ps + block - 1) / block, ps, static_cast<unsigned>(p.numplates)), block, nullptr, oargs, err)) return false;
     }
-    cudaEventRecord(e1, nullptr);
-    unsigned counters[16] = {};
-    bool ok = cr == CUDA_SUCCESS;
-    if (!ok) *err = "cuLaunchKernel failed (CUresult " + std::to_string(static_cast<int>(cr)) + ")";
-    if (ok) {
-        ce = cudaMemcpy(counters, fwd_->counters, sizeof counters, cudaMemcpyDeviceToHost);  // synchronises
-        if (ce != cudaSuccess) {
-            *err = std::string("lens kernel: ") + cudaGetErrorString(ce);
-            ok = false;
-        }
-    }
-    if (ok && counters[0] > kUndecidedCap) {
-        *err = "too many grid points need the interpreter (" + std::to_string(counters[0]) + ")";
-        ok = false;
-    }
-    if (ok && counters[9] > kUndecidedCap) {
-        *err = "too many texel owners need the interpreter (" + std::to_string(counters[9]) + ")";
-        ok = false;
-    }
-    if (ok) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        kernel_ms_ = ms;
-        ++launches_;
-        fwd_->nil_count = counters[1];
-        undecided->resize(counters[0]);
-        if (counters[0]) cudaMemcpy(undecided->data(), fwd_->undecided, counters[0] * sizeof(unsigned), cudaMemcpyDeviceToHost);
-        undecided_texels->resize(counters[9]);
-        if (counters[9]) cudaMemcpy(undecided_texels->data(), fwd_->owner_undecided, counters[9] * sizeof(unsigned), cudaMemcpyDeviceToHost);
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    if (!ok) drop_forward_state();
-    return ok;
+    timer.stop(nullptr);
+    if (!read_list(counters, points, nullptr, "lens kernel", "grid points", undecided, err)) return false;
+    if (m->owner_fn && !read_list(counters + 9, texels, nullptr, "lens kernel", "texel owners", undecided_texels, err)) return false;
+    if (!checked(cudaMemcpy(&f->nil_count, counters + 1, sizeof(unsigned), cudaMemcpyDeviceToHost), "lens kernel", err)) return false;
+    kernel_ms_ = timer.ms();
+    fwd_ = std::move(f);
+    return true;
 }
 
 bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
                                 uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) {
-    if (!fwd_) {
+    const std::unique_ptr<ForwardState> f = std::move(fwd_);  // consumed whatever the outcome
+    if (!f) {
         *err = "forward_finish without forward_points";
         return false;
     }
-    const LensBuildParams &p = fwd_->p;
+    const LensBuildParams &p = f->p;
     const size_t npix = static_cast<size_t>(p.width) * p.height;
-    ForwardPatch *d_patches = nullptr;
-    uint32_t *d_owner_patches = nullptr;
-    unsigned *d_keys = nullptr;  // idxkey[npix] then tintkey[npix]
-    FwdMessage *d_messages = nullptr;
-    int32_t *d_idx = nullptr;
-    uint8_t *d_tint = nullptr;
-    cudaError_t ce = cudaMalloc(&d_keys, 2 * npix * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = cudaMemset(d_keys, 0, 2 * npix * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = cudaMalloc(&d_messages, kMessageCap * sizeof(FwdMessage));
-    if (ce == cudaSuccess) ce = cudaMalloc(&d_idx, npix * sizeof(int32_t));
-    if (ce == cudaSuccess) ce = cudaMalloc(&d_tint, npix);
-    bool any_nil = fwd_->nil_count > 0;
+    DeviceBuffer d_keys, d_messages, d_idx, d_tint, d_patches, d_owner_patches;  // d_keys: idxkey[npix] then tintkey[npix]
+    cudaError_t ce = allocate(&d_keys, 2 * npix * sizeof(unsigned));
+    if (ce == cudaSuccess) ce = cudaMemset(d_keys.get(), 0, 2 * npix * sizeof(unsigned));
+    if (ce == cudaSuccess) ce = allocate(&d_messages, kMessageCap * sizeof(FwdMessage));
+    if (ce == cudaSuccess) ce = allocate(&d_idx, npix * sizeof(int32_t));
+    if (ce == cudaSuccess) ce = allocate(&d_tint, npix);
+    FwdPoint *grid = f->grid.as<FwdPoint>();
+    unsigned char *status = f->status.as<unsigned char>(), *owner = f->owner.as<unsigned char>();
+    bool any_nil = f->nil_count > 0;
     if (ce == cudaSuccess && !patches.empty()) {
-        ce = cudaMalloc(&d_patches, patches.size() * sizeof(ForwardPatch));
-        if (ce == cudaSuccess) ce = cudaMemcpy(d_patches, patches.data(), patches.size() * sizeof(ForwardPatch), cudaMemcpyHostToDevice);
+        d_patches = upload(patches, nullptr, &ce);
         if (ce == cudaSuccess) {
             const unsigned n = static_cast<unsigned>(patches.size());
-            fwd_patch_kernel<<<(n + 255) / 256, 256>>>(fwd_->grid, fwd_->status, d_patches, n);
-            ++launches_;
+            fwd_patch_kernel<<<(n + 255) / 256, 256>>>(grid, status, d_patches.as<ForwardPatch>(), n);
         }
         for (const ForwardPatch &pt : patches) any_nil = any_nil || pt.status != 1;
     }
-    if (ce == cudaSuccess && !owner_patches.empty() && fwd_->owner) {
-        ce = cudaMalloc(&d_owner_patches, owner_patches.size() * sizeof(uint32_t));
-        if (ce == cudaSuccess) ce = cudaMemcpy(d_owner_patches, owner_patches.data(), owner_patches.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess && !owner_patches.empty() && owner) {
+        d_owner_patches = upload(owner_patches, nullptr, &ce);
         if (ce == cudaSuccess) {
             const unsigned n = static_cast<unsigned>(owner_patches.size());
-            fwd_owner_patch_kernel<<<(n + 255) / 256, 256>>>(fwd_->owner, d_owner_patches, n);
-            ++launches_;
+            fwd_owner_patch_kernel<<<(n + 255) / 256, 256>>>(owner, d_owner_patches.as<uint32_t>(), n);
         }
     }
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
+    EventTimer timer;
+    if (ce == cudaSuccess) ce = timer.start(nullptr);
     if (ce == cudaSuccess) {
-        cudaEventRecord(e0, nullptr);
         if (any_nil) {
             const int threads = 2 * (p.platesize + 1);
-            fwd_stale_kernel<<<(threads + 63) / 64, 64>>>(fwd_->grid, fwd_->status, p.platesize, p.numplates);
-            ++launches_;
+            fwd_stale_kernel<<<(threads + 63) / 64, 64>>>(grid, status, p.platesize, p.numplates);
         }
         FwdGeom g;
         g.width = p.width;
@@ -1011,43 +905,31 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const 
         g.rubix_pad = p.rubix_pad;
         g.rubix_unit_px = p.rubix_unit_px;
         memcpy(g.plates, p.plates, sizeof g.plates);
-        FwdOut o{d_keys, d_keys + npix, fwd_->counters, d_messages};
-        dim3 grid((p.platesize + 127) / 128, p.platesize, p.numplates);
-        fwd_raster_kernel<<<grid, 128>>>(g, fwd_->grid, o, fwd_->owner);
-        fwd_resolve_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256>>>(d_keys, d_keys + npix, d_idx, d_tint, npix, p.platesize);
-        launches_ += 2;
-        cudaEventRecord(e1, nullptr);
-        ce = cudaMemcpy(idx, d_idx, npix * sizeof(int32_t), cudaMemcpyDeviceToHost);
-        if (ce == cudaSuccess) ce = cudaMemcpy(tint, d_tint, npix, cudaMemcpyDeviceToHost);
+        unsigned *keys = d_keys.as<unsigned>();
+        FwdOut o{keys, keys + npix, f->counters.as<unsigned>(), d_messages.as<FwdMessage>()};
+        dim3 blocks((p.platesize + 127) / 128, p.platesize, p.numplates);
+        fwd_raster_kernel<<<blocks, 128>>>(g, grid, o, owner);
+        fwd_resolve_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256>>>(keys, keys + npix, d_idx.as<int32_t>(), d_tint.as<uint8_t>(), npix, p.platesize);
+        timer.stop(nullptr);
+        ce = cudaMemcpy(idx, d_idx.get(), npix * sizeof(int32_t), cudaMemcpyDeviceToHost);
+        if (ce == cudaSuccess) ce = cudaMemcpy(tint, d_tint.get(), npix, cudaMemcpyDeviceToHost);
     }
     unsigned counters[16] = {};
-    if (ce == cudaSuccess) ce = cudaMemcpy(counters, fwd_->counters, sizeof counters, cudaMemcpyDeviceToHost);
-    bool ok = ce == cudaSuccess;
-    if (!ok) *err = std::string("forward lensmap kernels: ") + cudaGetErrorString(ce);
-    if (ok && counters[2] > kMessageCap) {
+    if (ce == cudaSuccess) ce = cudaMemcpy(counters, f->counters.get(), sizeof counters, cudaMemcpyDeviceToHost);
+    if (!checked(ce, "forward lensmap kernels", err)) return false;
+    if (counters[2] > kMessageCap) {
         *err = "too many 'maxdiff' messages to replay (" + std::to_string(counters[2]) + ")";
-        ok = false;
+        return false;
     }
-    if (ok) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e0, e1);
-        kernel_ms_ += ms;
-        for (int i = 0; i < 6; ++i) display[i] = counters[3 + i] ? 1 : 0;
-        std::vector<FwdMessage> msg(counters[2]);
-        if (counters[2]) cudaMemcpy(msg.data(), d_messages, counters[2] * sizeof(FwdMessage), cudaMemcpyDeviceToHost);
-        messages->clear();
-        for (const FwdMessage &m : msg) messages->emplace_back(m.key, static_cast<int>(m.value));
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(d_patches);
-    cudaFree(d_owner_patches);
-    cudaFree(d_keys);
-    cudaFree(d_messages);
-    cudaFree(d_idx);
-    cudaFree(d_tint);
-    drop_forward_state();
-    return ok;
+    kernel_ms_ += timer.ms();
+    for (int i = 0; i < 6; ++i) display[i] = counters[3 + i] ? 1 : 0;
+    std::vector<FwdMessage> msg(counters[2]);
+    if (counters[2] && !checked(cudaMemcpy(msg.data(), d_messages.get(), counters[2] * sizeof(FwdMessage), cudaMemcpyDeviceToHost),
+                                "forward lensmap kernels", err))
+        return false;
+    messages->clear();
+    for (const FwdMessage &m : msg) messages->emplace_back(m.key, static_cast<int>(m.value));
+    return true;
 }
 
 }  // namespace blinky

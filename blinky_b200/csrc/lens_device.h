@@ -22,9 +22,12 @@
 
 #include <cstdint>
 #include <map>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
+
+#include "device_buffer.h"
 
 namespace blinky {
 
@@ -74,61 +77,43 @@ struct RaySample {
 // True when a translated source defines lt_globe_plate (lua_transpile.h).
 inline bool source_has_globe_plate(const std::string &lens_source) { return lens_source.find("\n#define LT_HAS_GLOBE_PLATE 1\n") != std::string::npos; }
 
-// What FisheyeHost needs from a GPU (implemented by LensDevice).  CPU-only contexts have no
-// builder and take the interpreter.
-class DeviceLensBuilder {
+// Builds lensmaps on the GPU for FisheyeHost; CPU-only contexts have none and take the interpreter.
+class LensDevice {
 public:
-    virtual ~DeviceLensBuilder() {}
-    // inverse lenses: one candidate entry per screen pixel
-    virtual bool build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) = 0;
+    explicit LensDevice(int device);
+    ~LensDevice();
+
+    // inverse lenses: one candidate entry per screen pixel into cand[width*height].
+    // lens_source = transpile_prelude(true) + TranspileResult::source.  Returns false (reason in *err) when NVRTC is
+    // unavailable, the source does not compile, or a CUDA call fails.
+    bool build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err);
     // forward lenses, step 1: screen position of every plate grid point; `undecided` receives
     // the points the host has to evaluate itself.  When the source has a globe_plate, the texel
     // owners are computed too and `undecided_texels` receives the texels the host has to decide.
-    virtual bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
-                                std::vector<uint32_t> *undecided_texels, std::string *err) = 0;
+    bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
+                        std::vector<uint32_t> *undecided_texels, std::string *err);
     // step 2: host results patched in (grid points, texel owners), quads rasterised in the reference's
     // order (last writer wins), map resolved.  messages: (order key, value) of every "%d > maxdiff" the
     // reference prints.
-    virtual bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
-                                uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) = 0;
+    bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx, uint8_t *tint,
+                        int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err);
     // ray maps: the packed lensmap entry of each of the width * height float32 rays at d_rays (unnormalised, three per
     // pixel), on `stream` (a cudaStream_t) after the work already there, into a device map the builder keeps until its
     // next ray map (*d_map).  globe_source: the globe's globe_plate translated alone, or the bare prelude for argmax
     // globes.  Pixels whose plate decision is not provably the host's are written unmapped; *flagged receives them and
     // *flagged_rays their rays, for the host to settle.
-    virtual bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
-                        std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) = 0;
+    bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
+                std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err);
     // writes the settled entries into that map on `stream`; returns once they are there
-    virtual bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) = 0;
+    bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err);
     // ray export: lens_inverse's ray at each of the p.width * p.height pixels of a build at p.scale, narrowed to float and
     // not normalised (zeros for nil), into d_rays (float32[height][width][3], device memory) on `stream` after the work
     // already there.  lens_source: the lens translated alone.  *flagged receives the pixels whose ray is not provably
     // the host's, for the host to evaluate; returns once the kernel has finished.
-    virtual bool rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
-                      std::string *err) = 0;
-    // writes the host's rays into that field on `stream`; returns once they are there
-    virtual bool patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) = 0;
-};
-
-class LensDevice : public DeviceLensBuilder {
-public:
-    explicit LensDevice(int device) : device_(device) {}
-    ~LensDevice() override;
-
-    // lens_source = transpile_prelude(true) + TranspileResult::source.
-    // Fills cand[width*height].  Returns false (reason in *err) when NVRTC is unavailable,
-    // the source does not compile, or a CUDA call fails.
-    bool build(const std::string &lens_source, const LensBuildParams &p, uint32_t *cand, std::string *err) override;
-    bool forward_points(const std::string &lens_source, const LensBuildParams &p, std::vector<uint32_t> *undecided,
-                        std::vector<uint32_t> *undecided_texels, std::string *err) override;
-    bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx, uint8_t *tint,
-                        int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) override;
-    bool raymap(const std::string &globe_source, const LensBuildParams &p, const float *d_rays, void *stream, uint32_t **d_map,
-                std::vector<uint32_t> *flagged, std::vector<float> *flagged_rays, std::string *err) override;
-    bool patch_entries(const std::vector<RayPatch> &patches, void *stream, std::string *err) override;
     bool rays(const std::string &lens_source, const LensBuildParams &p, float *d_rays, void *stream, std::vector<uint32_t> *flagged,
-              std::string *err) override;
-    bool patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err) override;
+              std::string *err);
+    // writes the host's rays into that field on `stream`; returns once they are there
+    bool patch_rays(const std::vector<RaySample> &samples, float *d_rays, void *stream, std::string *err);
     // bytes from device memory on `stream`, after the work already there (a ray map that takes the host path)
     bool copy_to_host(void *dst, const void *d_src, size_t bytes, void *stream, std::string *err);
     // bytes to device memory on `stream`, after the work already there; returns once they are there (a ray export
@@ -162,22 +147,19 @@ public:
 
     double last_compile_ms() const { return compile_ms_; }
     double last_kernel_ms() const { return kernel_ms_; }
-    int64_t launches() const { return launches_; }
 
 private:
     struct Module;
     struct ForwardState;
     enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit, kRaysUnit, kProbeUnit };
     Module *module_for(const std::string &source, Unit unit, std::string *err);
-    void drop_forward_state();
     int device_;
-    std::map<std::string, Module *> cache_;  // by unit + source text
-    ForwardState *fwd_ = nullptr;
-    unsigned *ray_flagged_ = nullptr;  // ray maps: [0] the flagged count, then the flagged pixels
-    uint32_t *ray_map_ = nullptr;      // ray maps: the last map, ray_map_pixels_ entries
+    std::map<std::string, std::unique_ptr<Module>> cache_;  // by unit + source text
+    std::unique_ptr<ForwardState> fwd_;  // between forward_points() and forward_finish()
+    DeviceBuffer ray_flagged_;  // ray maps and exports: [0] the flagged count, then the flagged pixels
+    DeviceBuffer ray_map_;      // ray maps: the last map, ray_map_pixels_ entries
     size_t ray_map_pixels_ = 0;
     double compile_ms_ = 0, kernel_ms_ = 0;
-    int64_t launches_ = 0;
 };
 
 }  // namespace blinky
