@@ -117,6 +117,8 @@ _SIGNATURES = [
                                              c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_device_rays_supersampled", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p, c_size_t,
                                                      c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    ("blinky_warp_device_rays_bilinear", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p, c_size_t,
+                                                 c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_host", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int]),
     ("blinky_upload_bytes_per_frame", c_int64, [_CTX]),
     ("blinky_alloc_pinned", c_int, [_CTX, c_size_t, POINTER(c_void_p)]),
@@ -604,7 +606,8 @@ class Fisheye:
 
     def warp_rays(self, d_faces, d_screen, rays, xforms=None, *, x0: int = 0, y0: int = 0, rowbytes: int | None = None,
                   nframes: int | None = None, keep_unmapped: bool = False, rgba: bool = False, tables=None,
-                  face_stride: int | None = None, screen_stride: int | None = None, stream: int | None = None, supersample: int = 1):
+                  face_stride: int | None = None, screen_stride: int | None = None, stream: int | None = None, supersample: int = 1,
+                  filter: str = "nearest"):
         """warp_view with each pixel's texel computed on the GPU from its view ray, turned by a per-frame 3x3 matrix,
         through the current globe (blinky_warp_device_rays[_rgba]): frame f equals set_raymap of the turned field
         followed by a one-frame warp_view, without changing the installed lensmap, whose size and background it uses.
@@ -613,13 +616,19 @@ class Fisheye:
         defaults to N of whichever is per-frame (else 1).  The other arguments are warp_view's (tables: RGBA only).
         May be captured into a CUDA graph; a replay reads the rays and matrices as they are then.
         supersample=k (2, 3 or 4; RGBA only, blinky_warp_device_rays_supersampled): rays are a k-fold field [k*H, k*W, 3]
-        or [N, k*H, k*W, 3], and each pixel is the rounded mean of the colours of its k x k rays (box filter)."""
+        or [N, k*H, k*W, 3], and each pixel is the rounded mean of the colours of its k x k rays (box filter).
+        filter="bilinear" (RGBA only, blinky_warp_device_rays_bilinear, with any supersample): each ray's colour blends
+        the four texels around where it lands on its plate instead of taking the nearest one."""
         if isinstance(supersample, bool) or not isinstance(supersample, int):
             raise TypeError(f"warp_rays: supersample must be an int (1, 2, 3 or 4), got {supersample!r}")
         if not 1 <= supersample <= 4:
             raise ValueError(f"warp_rays: supersample must be 1, 2, 3 or 4, got {supersample}")
         if supersample > 1 and not rgba:
             raise ValueError("warp_rays: supersample > 1 needs rgba=True (palette indices cannot be averaged)")
+        if filter not in ("nearest", "bilinear"):
+            raise ValueError(f"warp_rays: filter must be 'nearest' or 'bilinear', got {filter!r}")
+        if filter == "bilinear" and not rgba:
+            raise ValueError("warp_rays: filter='bilinear' needs rgba=True (palette indices cannot be blended)")
         if not (hasattr(rays, "is_cuda") and rays.is_cuda):
             raise TypeError("warp_rays: rays must be a CUDA tensor")
         W, H = self.width, self.height
@@ -657,7 +666,9 @@ class Fisheye:
                              else (y0 + H) * rowbytes)
         args = (self._ctx, _ptr(d_faces), face_stride, rays.data_ptr(), ray_stride, d_xforms, xform_stride, _ptr(d_screen), screen_stride,
                 rowbytes, x0, y0, nframes, 1 if keep_unmapped else 0)
-        if k > 1:
+        if filter == "bilinear":
+            self._check(self._lib.blinky_warp_device_rays_bilinear(*args[:7], k, *args[7:], d_tables, table_stride, _warp_stream(stream)))
+        elif k > 1:
             self._check(self._lib.blinky_warp_device_rays_supersampled(*args[:7], k, *args[7:], d_tables, table_stride, _warp_stream(stream)))
         elif rgba:
             self._check(self._lib.blinky_warp_device_rays_rgba(*args, d_tables, table_stride, _warp_stream(stream)))

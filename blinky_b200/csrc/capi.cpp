@@ -670,15 +670,18 @@ int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x
     return rc != BLINKY_OK ? rc : warp_into_view(ctx, r, rowbytes, x0, y0);
 }
 
-// blinky_warp_device_rays[_rgba|_supersampled]: the view warp r with each pixel's texel computed from its ray in q,
-// turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours).  Every refusal launches
-// nothing.
+// blinky_warp_device_rays[_rgba|_supersampled|_bilinear]: the view warp r with each pixel's texel computed from its ray
+// in q, turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours; q.bilinear: RGBA,
+// the mean of q.factor^2 bilinear samples).  Every refusal launches nothing.
 int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRequest &q, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba,
                      bool supersampled = false) {
     NEED_DEVICE(ctx);
     r.keep_unmapped = keep_unmapped != 0;
     r.rgba = rgba;
-    const char *name = supersampled ? "blinky_warp_device_rays_supersampled" : rgba ? "blinky_warp_device_rays_rgba" : "blinky_warp_device_rays";
+    const char *name = q.bilinear      ? "blinky_warp_device_rays_bilinear"
+                       : supersampled  ? "blinky_warp_device_rays_supersampled"
+                       : rgba          ? "blinky_warp_device_rays_rgba"
+                                       : "blinky_warp_device_rays";
     auto refuse = [&](int code, const std::string &why) { return set_err(ctx, code, std::string(name) + ": " + why); };
     const int W = ctx->dev->width(), H = ctx->dev->height(), ps = ctx->dev->platesize();
     if (W <= 0) return refuse(BLINKY_E_STATE, "no lensmap installed (the view's size and background are the installed lensmap's)");
@@ -689,9 +692,10 @@ int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRe
     if (!q.rays) return refuse(BLINKY_E_INVALID, "NULL rays");
     if (reinterpret_cast<uintptr_t>(q.rays) % 4 != 0 || reinterpret_cast<uintptr_t>(q.xforms) % 4 != 0)
         return refuse(BLINKY_E_INVALID, "d_rays and d_xforms must be 4-byte aligned");
-    if (supersampled) {
-        // (factor 1 is blinky_warp_device_rays_rgba)
-        if (q.factor < 2 || q.factor > 4) return refuse(BLINKY_E_INVALID, "factor must be 2, 3 or 4");
+    if (supersampled || q.bilinear) {
+        // (the supersampled factor 1 is blinky_warp_device_rays_rgba; the bilinear one is a sample per pixel)
+        if (q.factor < (q.bilinear ? 1 : 2) || q.factor > 4)
+            return refuse(BLINKY_E_INVALID, q.bilinear ? "factor must be 1, 2, 3 or 4" : "factor must be 2, 3 or 4");
         if (q.ray_stride != 0 && (q.ray_stride < 12 * static_cast<size_t>(q.factor * q.factor) * static_cast<size_t>(W) * static_cast<size_t>(H) ||
                                   q.ray_stride % 4 != 0))
             return refuse(BLINKY_E_INVALID,
@@ -765,6 +769,19 @@ int blinky_warp_device_rays_supersampled(blinky_ctx *ctx, const void *d_faces, s
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
     q.factor = factor;
     return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true, true);
+}
+
+int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
+                                     const float *d_xforms, size_t xform_stride, int factor, void *d_screen_rgba, size_t screen_frame_stride,
+                                     int rowbytes, int x0, int y0, int nframes, int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
+                                     void *stream) {
+    blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
+    r.tables = d_tables;
+    r.table_stride = table_stride;
+    blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
+    q.factor = factor;
+    q.bilinear = true;
+    return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,

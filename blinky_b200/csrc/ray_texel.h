@@ -38,9 +38,9 @@ BLINKY_HD void ray_normalize3(float v[3]) {
 }
 
 // The plate and texel set_raymap gives the unnormalised ray (normalised here, in place) on plates of P.platesize
-// texels: false when the ray maps to nothing.  The plate is the argmax over the globe's P.numplates plates (strict:
-// the lowest index wins ties, NaN never wins).
-BLINKY_HD bool ray_texel(const LensBuildParams &P, float ray[3], int *plate, int *px, int *py) {
+// texels, with the continuous plate coordinates (u, v) the texel truncates: false when the ray maps to nothing.  The
+// plate is the argmax over the globe's P.numplates plates (strict: the lowest index wins ties, NaN never wins).
+BLINKY_HD bool ray_texel_uv(const LensBuildParams &P, float ray[3], int *plate, int *px, int *py, double *pu, double *pv) {
     ray_normalize3(ray);
     int best = 0;
     double best_dp = -2;
@@ -62,7 +62,34 @@ BLINKY_HD bool ray_texel(const LensBuildParams &P, float ray[3], int *plate, int
     *plate = best;
     *px = static_cast<int>(u * ps);
     *py = static_cast<int>(v * ps);
+    *pu = u;
+    *pv = v;
     return *px >= 0 && *px < ps && *py >= 0 && *py < ps;
+}
+
+// ray_texel_uv without (u, v)
+BLINKY_HD bool ray_texel(const LensBuildParams &P, float ray[3], int *plate, int *px, int *py) {
+    double u, v;
+    return ray_texel_uv(P, ray, plate, px, py, &u, &v);
+}
+
+// The bilinear sample of the unnormalised ray (normalised here, in place; blinky_warp_device_rays_bilinear): mapped
+// exactly when ray_texel maps it, on the same plate.  Then, in double, sx = u * ps - 0.5, x0 = floor(sx) and
+// wx = (int)((sx - x0) * 256), and likewise sy, y0 and wy from v.  x0 and y0 lie in [-1, ps - 1] (u * ps < ps because
+// the texel is in range) and wx, wy in [0, 255] (sx - floor(sx) is exact and below 1); the caller clamps the taps x0,
+// x0 + 1, y0, y0 + 1 to [0, ps - 1].
+BLINKY_HD bool ray_bilinear(const LensBuildParams &P, float ray[3], int *plate, int *x0, int *y0, int *wx, int *wy) {
+    int px, py;
+    double u, v;
+    if (!ray_texel_uv(P, ray, plate, &px, &py, &u, &v)) return false;
+    const int ps = P.platesize;
+    const double sx = u * ps - 0.5, sy = v * ps - 0.5;
+    const double fx = floor(sx), fy = floor(sy);
+    *x0 = static_cast<int>(fx);
+    *y0 = static_cast<int>(fy);
+    *wx = static_cast<int>((sx - fx) * 256);
+    *wy = static_cast<int>((sy - fy) * 256);
+    return true;
 }
 
 // on_rubix_grid: texel (px, py) lies in the padding between the rubix cells
@@ -70,6 +97,14 @@ BLINKY_HD bool ray_on_rubix_grid(const LensBuildParams &P, int px, int py) {
     const double ux = static_cast<double>(px) / P.rubix_unit_px;
     const double uy = static_cast<double>(py) / P.rubix_unit_px;
     return fmod(ux, P.rubix_block) < P.rubix_pad || fmod(uy, P.rubix_block) < P.rubix_pad;
+}
+
+// one axis of ray_on_rubix_grid, the same arithmetic: texel column (or row) t lies in the padding between the rubix
+// cells, so that texel (px, py) is on the grid exactly when column px or row py is.  (A separate copy: expressing
+// ray_on_rubix_grid through it changes the machine code of the existing warps.)
+BLINKY_HD bool ray_on_rubix_line(const LensBuildParams &P, int t) {
+    const double ut = static_cast<double>(t) / P.rubix_unit_px;
+    return fmod(ut, P.rubix_block) < P.rubix_pad;
 }
 
 // The packed lensmap entry (BLINKY_LM_*) blinky_set_raymap installs for the ray turned by M (nullptr: the ray as it

@@ -13,6 +13,7 @@ namespace blinky {
 
 struct RayWarpLaunch {
     int factor;                 // 1: ray_warp_kernel; 2-4: ray_supersample_kernel, k x k samples per pixel (RGBA, never quads)
+    bool bilinear;              // ray_bilinear_kernel, factor 1-4: k x k bilinear samples per pixel (RGBA, never quads)
     const float *rays;          // frame 0's field, float32[factor * height][factor * width][3]
     size_t ray_stride;          // bytes between frames' fields (0: one field for every frame)
     const float *xforms;        // frame 0's matrix, 9 floats row-major (nullptr: the rays as they are)
@@ -35,7 +36,7 @@ struct RayWarpLaunch {
     void *stream;               // cudaStream_t
 };
 
-// Launches ray_warp_kernel (factor 1) or ray_supersample_kernel for L.  false with the CUDA error in *cuda_err; *name: the instance and launch shape (last_kernel).
+// Launches ray_warp_kernel (factor 1), ray_supersample_kernel or ray_bilinear_kernel (bilinear) for L.  false with the CUDA error in *cuda_err; *name: the instance and launch shape (last_kernel).
 bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err);
 
 }  // namespace blinky

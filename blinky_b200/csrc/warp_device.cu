@@ -1277,9 +1277,9 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
                " is beyond what a ray map takes (6 * platesize^2 must fit the 28-bit texel index)";
         return false;
     }
-    // (the supersampled kernel indexes the field's pixels in 31 bits)
+    // (the supersampled and bilinear kernels index the field's pixels in 31 bits)
     const uint64_t field_pixels = static_cast<uint64_t>(q.factor) * q.factor * static_cast<uint64_t>(cur_->width) * static_cast<uint64_t>(cur_->height);
-    if (q.factor > 1 && field_pixels > 0x7FFFFFFFu) {
+    if ((q.factor > 1 || q.bilinear) && field_pixels > 0x7FFFFFFFu) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp_rays: a field of factor^2 * width * height = " + std::to_string(field_pixels) + " pixels is beyond the kernel's 31-bit pixel index";
         return false;
@@ -1300,6 +1300,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     if (!capture_info(r.stream, &capturing, &cap_id)) return false;
     RayWarpLaunch L;
     L.factor = q.factor;
+    L.bilinear = q.bilinear;
     L.rays = q.rays;
     L.ray_stride = q.ray_stride;
     L.xforms = q.xforms;
@@ -1316,7 +1317,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     L.width = g.width;
     L.height = g.height;
     L.nframes = r.nframes;
-    L.quads = q.factor == 1 && ray_warp_quads(r, pitch, g.width);
+    L.quads = q.factor == 1 && !q.bilinear && ray_warp_quads(r, pitch, g.width);
     const size_t npix = static_cast<size_t>(g.width) * static_cast<size_t>(g.height);
     L.frames_per_thread = ray_warp_frames_per_thread(q.ray_stride, r.nframes, static_cast<uint32_t>(L.quads ? npix / 4 : npix),
                                                      static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
@@ -1331,7 +1332,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     const bool ok = launch_ray_warp(L, &last_kernel_, &e);
     ++launches_;
     if (capturing) remember_capture(r.stream, cap_id);
-    return ok ? true : fail(q.factor > 1 ? "ray_supersample_kernel" : "ray_warp_kernel", e);
+    return ok ? true : fail(q.bilinear ? "ray_bilinear_kernel" : q.factor > 1 ? "ray_supersample_kernel" : "ray_warp_kernel", e);
 }
 
 bool WarpDevice::release_captures() {

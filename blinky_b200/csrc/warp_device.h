@@ -63,6 +63,7 @@ struct RayRequest {
     const float *xforms;        // frame 0's 3x3 matrix, row-major (nullptr: the rays as they are)
     size_t xform_stride;        // bytes between frames (0: one matrix for every frame)
     int factor = 1;             // 2-4: a [factor * height][factor * width] field, factor^2 samples averaged per RGBA pixel
+    bool bilinear = false;      // each sample bilinear-filtered from four texels (RGBA, factor 1-4)
 };
 
 class WarpDevice {
@@ -103,7 +104,8 @@ public:
     // r (view, rgba, keep_unmapped, tables) with each pixel's texel computed from its ray in q, turned, through the
     // globe `globe` (FisheyeHost::device_params at the resident view's size, no globe_plate script): the resident
     // lensmap gives only the view's size and background.  Every plate of the globe must have an origin in the face
-    // layout.  Capturable like warp().  q.factor > 1: the supersampled RGBA warp (ray_supersample_kernel).
+    // layout.  Capturable like warp().  q.factor > 1: the supersampled RGBA warp (ray_supersample_kernel);
+    // q.bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel).
     bool warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go
     // of the generations held for such graphs and returns every capture counter slot to the pool.

@@ -566,6 +566,45 @@ int blinky_warp_device_rays_supersampled(blinky_ctx *ctx, const void *d_faces, s
                                          int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
                                          void *stream);
 
+/* Bilinear-filtered RGBA warp from a ray field, alone (factor k = 1) or under k x k supersampling
+ * (k = 2, 3 or 4).  Same arguments as blinky_warp_device_rays_supersampled: W, H, ps and the background
+ * are the installed lensmap's, and the field (float32[k*H][k*W][3]), matrices, faces, tables, view
+ * rectangle, keep_unmapped and face layout are read as that call reads them.  Sample s of output pixel
+ * (x, y) is field pixel (k*x + i, k*y + j), turned by M_f exactly as blinky_warp_device_rays turns a ray.
+ *   - Mapping: the sample is mapped exactly when blinky_set_raymap maps the turned ray, on the same
+ *     plate P, with u, v the plate coordinates (in double) whose truncation to u*ps, v*ps is its texel.
+ *   - Position, one IEEE double operation each: sx = u*ps - 0.5, sy = v*ps - 0.5; x0 = floor(sx),
+ *     y0 = floor(sy); wx = (int)((sx - x0) * 256), wy = (int)((sy - y0) * 256), each in 0..255.  The
+ *     taps are (x0 | x0+1, y0 | y0+1), each coordinate clamped to [0, ps-1] on plate P: no filtering
+ *     across plate seams, and no read outside the plate's ps x ps texels.
+ *   - Texel colour: C(tx, ty) = T_f[b'] with b the face byte of (P, tx, ty), b' = LUT_P[b] when f_rubix
+ *     is on and texel (tx, ty) is off the rubix grid, else b' = b: the colour
+ *     blinky_warp_device_rays_rgba draws for a ray that lands on that texel (grid lines are filtered
+ *     like the rest of the image).
+ *   - Blend, per byte n (alpha included), in integers: ((C00*(256-wx) + C10*wx)*(256-wy) +
+ *     (C01*(256-wx) + C11*wx)*wy + 32768) >> 16, with Cab the tap (x0+a, y0+b).  The weights sum to
+ *     65536: a texel centre gives C00 exactly, and a region of one colour stays that colour.  The blend
+ *     is of the tables' gamma-encoded bytes, as the supersampled average is.
+ *   - An unmapped sample's colour is T_f[bg[y][x]], the output pixel's background.
+ * The k^2 sample colours are averaged per byte as (sum + k^2/2) / k^2 (k = 1: the sample's colour).  With
+ * keep_unmapped a pixel none of whose samples is mapped is not written.  Equivalently, frame f is the
+ * k x k box average of this warp at k = 1 over k*W x k*H, whose background is bg with each byte repeated
+ * k x k; at k = 1 with keep_unmapped it writes exactly the pixels blinky_warp_device_rays_rgba writes.
+ * There is no 8-bit form: palette indices cannot be blended.
+ * Sample positions: an exported field (blinky_get_raymap_device at k*W x k*H) places the samples as
+ * blinky_warp_device_rays_supersampled describes.
+ * Refuses everything blinky_warp_device_rays_supersampled refuses, with the same codes, and launches
+ * nothing when it does; BLINKY_E_INVALID for a factor that is not 1, 2, 3 or 4, and for k^2*W*H beyond
+ * the kernel's 31-bit pixel index (2^31 - 1) at every factor, 1 included.  Capturable like
+ * blinky_warp_device_rays_rgba, on the same terms; the context does not change, blinky_launch_count
+ * and blinky_last_kernel do. */
+int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
+                                     const float *d_rays, size_t ray_stride, const float *d_xforms,
+                                     size_t xform_stride, int factor, void *d_screen_rgba,
+                                     size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
+                                     int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
+                                     void *stream);
+
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
 const char *blinky_plan_summary(blinky_ctx *ctx);
