@@ -119,6 +119,9 @@ _SIGNATURES = [
                                                      c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_device_rays_bilinear", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p, c_size_t,
                                                  c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    ("blinky_ray_pyramid_bytes", c_int, [_CTX, POINTER(c_size_t)]),
+    ("blinky_warp_device_rays_trilinear", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t, c_int,
+                                                  c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
     ("blinky_warp_host", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int]),
     ("blinky_upload_bytes_per_frame", c_int64, [_CTX]),
     ("blinky_alloc_pinned", c_int, [_CTX, c_size_t, POINTER(c_void_p)]),
@@ -607,7 +610,7 @@ class Fisheye:
     def warp_rays(self, d_faces, d_screen, rays, xforms=None, *, x0: int = 0, y0: int = 0, rowbytes: int | None = None,
                   nframes: int | None = None, keep_unmapped: bool = False, rgba: bool = False, tables=None,
                   face_stride: int | None = None, screen_stride: int | None = None, stream: int | None = None, supersample: int = 1,
-                  filter: str = "nearest"):
+                  filter: str = "nearest", scratch=None):
         """warp_view with each pixel's texel computed on the GPU from its view ray, turned by a per-frame 3x3 matrix,
         through the current globe (blinky_warp_device_rays[_rgba]): frame f equals set_raymap of the turned field
         followed by a one-frame warp_view, without changing the installed lensmap, whose size and background it uses.
@@ -618,17 +621,26 @@ class Fisheye:
         supersample=k (2, 3 or 4; RGBA only, blinky_warp_device_rays_supersampled): rays are a k-fold field [k*H, k*W, 3]
         or [N, k*H, k*W, 3], and each pixel is the rounded mean of the colours of its k x k rays (box filter).
         filter="bilinear" (RGBA only, blinky_warp_device_rays_bilinear, with any supersample): each ray's colour blends
-        the four texels around where it lands on its plate instead of taking the nearest one."""
+        the four texels around where it lands on its plate instead of taking the nearest one.
+        filter="trilinear" (RGBA only, supersample 1, blinky_warp_device_rays_trilinear): each frame's plates are
+        averaged into a mip pyramid on the GPU, and each pixel blends bilinear colours of the two levels around how far
+        apart its neighbouring rays land.  scratch: a contiguous CUDA tensor of at least nframes * ray_pyramid_bytes()
+        bytes, 16-byte aligned, which the pyramids are written to; None allocates one for the call, which a stream
+        being captured into a graph cannot do (pass a persistent scratch there)."""
         if isinstance(supersample, bool) or not isinstance(supersample, int):
             raise TypeError(f"warp_rays: supersample must be an int (1, 2, 3 or 4), got {supersample!r}")
         if not 1 <= supersample <= 4:
             raise ValueError(f"warp_rays: supersample must be 1, 2, 3 or 4, got {supersample}")
         if supersample > 1 and not rgba:
             raise ValueError("warp_rays: supersample > 1 needs rgba=True (palette indices cannot be averaged)")
-        if filter not in ("nearest", "bilinear"):
-            raise ValueError(f"warp_rays: filter must be 'nearest' or 'bilinear', got {filter!r}")
-        if filter == "bilinear" and not rgba:
-            raise ValueError("warp_rays: filter='bilinear' needs rgba=True (palette indices cannot be blended)")
+        if filter not in ("nearest", "bilinear", "trilinear"):
+            raise ValueError(f"warp_rays: filter must be 'nearest' or 'bilinear' or 'trilinear', got {filter!r}")
+        if filter in ("bilinear", "trilinear") and not rgba:
+            raise ValueError(f"warp_rays: filter={filter!r} needs rgba=True (palette indices cannot be blended)")
+        if filter == "trilinear" and supersample != 1:
+            raise ValueError("warp_rays: filter='trilinear' takes one sample per pixel (supersample=1)")
+        if scratch is not None and filter != "trilinear":
+            raise ValueError("warp_rays: scratch is for filter='trilinear' only")
         if not (hasattr(rays, "is_cuda") and rays.is_cuda):
             raise TypeError("warp_rays: rays must be a CUDA tensor")
         W, H = self.width, self.height
@@ -666,7 +678,9 @@ class Fisheye:
                              else (y0 + H) * rowbytes)
         args = (self._ctx, _ptr(d_faces), face_stride, rays.data_ptr(), ray_stride, d_xforms, xform_stride, _ptr(d_screen), screen_stride,
                 rowbytes, x0, y0, nframes, 1 if keep_unmapped else 0)
-        if filter == "bilinear":
+        if filter == "trilinear":
+            self._warp_rays_trilinear(args, d_tables, table_stride, scratch, nframes, stream)
+        elif filter == "bilinear":
             self._check(self._lib.blinky_warp_device_rays_bilinear(*args[:7], k, *args[7:], d_tables, table_stride, _warp_stream(stream)))
         elif k > 1:
             self._check(self._lib.blinky_warp_device_rays_supersampled(*args[:7], k, *args[7:], d_tables, table_stride, _warp_stream(stream)))
@@ -674,6 +688,40 @@ class Fisheye:
             self._check(self._lib.blinky_warp_device_rays_rgba(*args, d_tables, table_stride, _warp_stream(stream)))
         else:
             self._check(self._lib.blinky_warp_device_rays(*args, _warp_stream(stream)))
+
+    def ray_pyramid_bytes(self) -> int:
+        """bytes of one frame's mip pyramid for warp_rays(filter="trilinear") (blinky_ray_pyramid_bytes): the installed
+        lensmap's plate size and every plate of the current globe"""
+        n = ctypes.c_size_t(0)
+        self._check(self._lib.blinky_ray_pyramid_bytes(self._ctx, ctypes.byref(n)))
+        return n.value
+
+    def _warp_rays_trilinear(self, args, d_tables, table_stride, scratch, nframes, stream):
+        """blinky_warp_device_rays_trilinear with warp_rays' arguments; scratch None: a torch buffer for this call"""
+        own = None
+        if scratch is None:
+            import torch
+
+            size = max(nframes, 0) * self.ray_pyramid_bytes()
+            if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():
+                raise ValueError("warp_rays: filter='trilinear' under graph capture needs a persistent scratch tensor (scratch=, "
+                                 "at least nframes * ray_pyramid_bytes() bytes); allocating one for the call cannot be captured")
+            own = torch.empty(max(size, 1), dtype=torch.uint8, device=f"cuda:{self.device}")
+            d_scratch, scratch_bytes = own.data_ptr(), size
+        else:
+            d_scratch = _ptr(scratch)
+            scratch_bytes = scratch.numel() * scratch.element_size() if hasattr(scratch, "numel") else None
+            if scratch_bytes is None:
+                raise TypeError("warp_rays: scratch must be a CUDA tensor (its size is the scratch_bytes passed on)")
+            if hasattr(scratch, "is_contiguous") and not scratch.is_contiguous():
+                raise ValueError("warp_rays: scratch must be contiguous")
+        stream = _warp_stream(stream)
+        self._check(self._lib.blinky_warp_device_rays_trilinear(*args, d_tables, table_stride, d_scratch, scratch_bytes, stream))
+        if own is not None:
+            import torch
+
+            # the buffer goes back to torch's allocator when this call returns: not to be reused before the warp ran
+            own.record_stream(torch.cuda.ExternalStream(stream) if stream else torch.cuda.default_stream(own.device))
 
     def release_captures(self):
         """No CUDA graph that captured a warp of this context will run again (blinky_release_captures): frees the

@@ -17,6 +17,7 @@
 #include "fisheye_host.h"
 #include "lens_device.h"
 #include "lua_transpile.h"
+#include "ray_texel.h"
 #include "shard.h"
 #include "tile_plan.h"
 #include "tile_plan_device.h"
@@ -670,15 +671,17 @@ int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x
     return rc != BLINKY_OK ? rc : warp_into_view(ctx, r, rowbytes, x0, y0);
 }
 
-// blinky_warp_device_rays[_rgba|_supersampled|_bilinear]: the view warp r with each pixel's texel computed from its ray
-// in q, turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours; q.bilinear: RGBA,
-// the mean of q.factor^2 bilinear samples).  Every refusal launches nothing.
+// blinky_warp_device_rays[_rgba|_supersampled|_bilinear|_trilinear]: the view warp r with each pixel's texel computed
+// from its ray in q, turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours;
+// q.bilinear: RGBA, the mean of q.factor^2 bilinear samples; q.trilinear: RGBA, one sample from the frame's mip pyramid
+// in q.scratch, whose checks are WarpDevice::warp_rays').  Every refusal launches nothing.
 int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRequest &q, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba,
                      bool supersampled = false) {
     NEED_DEVICE(ctx);
     r.keep_unmapped = keep_unmapped != 0;
     r.rgba = rgba;
-    const char *name = q.bilinear      ? "blinky_warp_device_rays_bilinear"
+    const char *name = q.trilinear     ? "blinky_warp_device_rays_trilinear"
+                       : q.bilinear    ? "blinky_warp_device_rays_bilinear"
                        : supersampled  ? "blinky_warp_device_rays_supersampled"
                        : rgba          ? "blinky_warp_device_rays_rgba"
                                        : "blinky_warp_device_rays";
@@ -781,6 +784,37 @@ int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
     q.factor = factor;
     q.bilinear = true;
+    return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
+}
+
+int blinky_ray_pyramid_bytes(blinky_ctx *ctx, size_t *bytes) {
+    NEED_DEVICE(ctx);
+    const char *who = "blinky_ray_pyramid_bytes";
+    if (!bytes) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": NULL bytes");
+    if (ctx->dev->width() <= 0) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": no lensmap installed (its plate size sizes the pyramid)");
+    if (!ctx->host.globe_valid()) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": no valid globe");
+    int size[blinky::kRayMaxLevels];
+    uint64_t off[blinky::kRayMaxLevels], b = 0;
+    const int ps = ctx->dev->platesize();
+    if (static_cast<uint64_t>(ps) * static_cast<uint64_t>(ps) * BLINKY_MAX_PLATES > 0x0FFFFFFFu ||
+        blinky::ray_pyramid_levels(ps, ctx->host.numplates(), size, off, &b) < 0)
+        return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": the installed lensmap's plate size " + std::to_string(ps) +
+                                                " is beyond what the ray warps take (6 * platesize^2 must fit the 28-bit texel index)");
+    *bytes = static_cast<size_t>(b);
+    return BLINKY_OK;
+}
+
+int blinky_warp_device_rays_trilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
+                                      const float *d_xforms, size_t xform_stride, void *d_screen_rgba, size_t screen_frame_stride, int rowbytes,
+                                      int x0, int y0, int nframes, int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
+                                      void *d_scratch, size_t scratch_bytes, void *stream) {
+    blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
+    r.tables = d_tables;
+    r.table_stride = table_stride;
+    blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
+    q.trilinear = true;
+    q.scratch = d_scratch;
+    q.scratch_bytes = scratch_bytes;
     return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
 }
 

@@ -107,6 +107,100 @@ BLINKY_HD bool ray_on_rubix_line(const LensBuildParams &P, int t) {
     return fmod(ut, P.rubix_block) < P.rubix_pad;
 }
 
+// ---- trilinear (blinky_warp_device_rays_trilinear, DESIGN §3g) ------------------------------------------------------
+
+// Levels 0..13 at most: set_raymap's plate size limit (6 * ps^2 < 2^28, ps <= 6688) halves to 1 in 13 steps.
+constexpr int kRayMaxLevels = 14;
+
+// The mip pyramid of one frame, for plates of ps texels on a globe of nplates plates: size[L] = (size[L-1] + 1) >> 1
+// from size[0] = ps down to size[lmax] = 1, and off[L] (L >= 1) the byte offset of level L's plate 0 from the frame's
+// pyramid.  Levels 1..lmax are stored level-major, then plate, then rows [size[L]][size[L]] of uint32 texels (level 0
+// is the faces themselves); *bytes is their total rounded up to 256.  Returns lmax, or -1 when ps < 1 or the pyramid
+// needs more than kRayMaxLevels levels.
+BLINKY_HD int ray_pyramid_levels(int ps, int nplates, int size[kRayMaxLevels], uint64_t off[kRayMaxLevels], uint64_t *bytes) {
+    if (ps < 1) return -1;
+    int lmax = 0;
+    uint64_t at = 0;
+    size[0] = ps;
+    off[0] = 0;
+    while (size[lmax] > 1) {
+        if (lmax + 1 >= kRayMaxLevels) return -1;
+        ++lmax;
+        size[lmax] = (size[lmax - 1] + 1) >> 1;
+        off[lmax] = at;
+        at += 4 * static_cast<uint64_t>(nplates) * static_cast<uint64_t>(size[lmax]) * static_cast<uint64_t>(size[lmax]);
+    }
+    *bytes = (at + 255) / 256 * 256;
+    return lmax;
+}
+
+// The projection of the normalised ray n onto plate `plate`, in level-0 texels: x, y, z are the float dot products
+// with the plate's right, up and forward, widened to double as in ray_texel_uv.  Usable (true) iff z > 0; then, one
+// IEEE double operation each, q = uv_dist * ps / z, a = x * q and b = -y * q.
+BLINKY_HD bool ray_plate_project(const LensBuildParams &P, int plate, const float n[3], double *a, double *b) {
+    const LensBuildParams::PlateF &p = P.plates[plate];
+    const double x = ray_dot3(p.right, n);
+    const double y = ray_dot3(p.up, n);
+    const double z = ray_dot3(p.forward, n);
+    if (!(z > 0)) return false;
+    const double q = P.uv_dist[plate] * P.platesize / z;
+    *a = x * q;
+    *b = -y * q;
+    return true;
+}
+
+// One axis of the footprint: the squared distance da * da + db * db between the projections (a, b) and (a1, b1).
+BLINKY_HD double ray_axis_rho2(double a, double b, double a1, double b1) {
+    const double da = a1 - a, db = b1 - b;
+    return da * da + db * db;
+}
+
+// rho^2, the squared footprint in level-0 texels of a sample on plate `plate` whose normalised ray is n, from the
+// normalised (turned) rays of its field neighbours, nullptr where that field pixel does not exist.  0 when n's own
+// projection is not usable.  Per axis: the forward neighbour (x + 1, or y + 1) when it exists and its projection onto
+// the plate is usable, else the backward one (x - 1, y - 1) on the same terms, else the axis gives 0.  rho^2 is the x
+// axis's value, replaced by the y axis's when that is greater (so a NaN x axis stays; a NaN y axis is ignored).
+BLINKY_HD double ray_footprint2(const LensBuildParams &P, int plate, const float n[3], const float *xf, const float *xb, const float *yf,
+                                const float *yb) {
+    double a, b, a1, b1;
+    if (!ray_plate_project(P, plate, n, &a, &b)) return 0;
+    double rx = 0, ry = 0;
+    if (xf && ray_plate_project(P, plate, xf, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
+    else if (xb && ray_plate_project(P, plate, xb, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
+    if (yf && ray_plate_project(P, plate, yf, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
+    else if (yb && ray_plate_project(P, plate, yb, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
+    return ry > rx ? ry : rx;
+}
+
+// The level and weight of a footprint, by comparisons only: rho = sqrt(rho2), correctly rounded; *L the largest
+// L <= lmax with 2^L <= rho (0 when rho < 1, and for a NaN rho); *w = (int)((rho * 2^-L - 1) * 256) when 1 <= rho
+// and L < lmax, else 0 (rho * 2^-L lies in [1, 2) and every step is exact, so w is in 0..255).
+BLINKY_HD void ray_level(double rho2, int lmax, int *L, int *w) {
+    const double rho = sqrt(rho2);
+    int l = 0;
+    double p = 1, inv = 1;   // 2^l, 2^-l
+    while (l < lmax && 2 * p <= rho) {
+        ++l;
+        p *= 2;
+        inv *= 0.5;
+    }
+    *L = l;
+    *w = rho >= 1 && l < lmax ? static_cast<int>((rho * inv - 1) * 256) : 0;
+}
+
+// ray_bilinear's position arithmetic on a grid of `size` texels per plate side, from the plate coordinates (u, v):
+// sx = u * size - 0.5, x0 = floor(sx), wx = (int)((sx - x0) * 256), and likewise y0, wy; the caller clamps the taps
+// x0, x0 + 1, y0, y0 + 1 to [0, size - 1].  (size = ps gives ray_bilinear's values; a separate copy, so that the
+// bilinear warp's machine code stays as it is.)
+BLINKY_HD void ray_bilinear_level(double u, double v, int size, int *x0, int *y0, int *wx, int *wy) {
+    const double sx = u * size - 0.5, sy = v * size - 0.5;
+    const double fx = floor(sx), fy = floor(sy);
+    *x0 = static_cast<int>(fx);
+    *y0 = static_cast<int>(fy);
+    *wx = static_cast<int>((sx - fx) * 256);
+    *wy = static_cast<int>((sy - fy) * 256);
+}
+
 // The packed lensmap entry (BLINKY_LM_*) blinky_set_raymap installs for the ray turned by M (nullptr: the ray as it
 // is): a map made in one pass gives an on-grid texel no tint.
 BLINKY_HD uint32_t ray_entry(const LensBuildParams &P, const float *M, const float ray[3]) {

@@ -4,7 +4,9 @@
 // blinky_warp_device_view (ray_texel.h holds the per-ray arithmetic).  The supersampled warp
 // (blinky_warp_device_rays_supersampled, ray_supersample_kernel) writes each RGBA pixel as the rounded mean of the
 // colours of k x k such rays; the bilinear warp (blinky_warp_device_rays_bilinear, ray_bilinear_kernel) the mean of k x k
-// bilinear samples, each four texels' colours weighted by where the ray falls between their centres.
+// bilinear samples, each four texels' colours weighted by where the ray falls between their centres; the trilinear warp
+// (blinky_warp_device_rays_trilinear, the pyramid kernels and ray_trilinear_kernel) builds each frame's RGBA mip pyramid
+// in the caller's scratch and blends, per pixel, bilinear colours of the two levels around its footprint.
 //
 // Compiled with --fmad=false: the turn and the globe's float / double arithmetic must round operation by operation
 // as the host's -ffp-contract=off build does.
@@ -13,6 +15,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdio>
+#include <cstring>
 
 #include "ray_texel.h"
 
@@ -390,6 +393,244 @@ __global__ void __launch_bounds__(kRayThreads, 1) ray_bilinear_kernel(const __gr
     }
 }
 
+// --------------------------------------------------------------------------
+// Trilinear RGBA (blinky_warp_device_rays_trilinear): per frame an RGBA mip pyramid of every plate of the globe in the
+// caller's scratch (levels 1..lmax, ray_pyramid_levels' layout), then one sample per pixel blended from two levels.
+// --------------------------------------------------------------------------
+struct RayPyramidParams {
+    uint8_t *scratch;           // frame 0's pyramid
+    size_t stride;              // bytes between frames' pyramids (B)
+    int lmax;
+    uint32_t size[kRayMaxLevels];
+    uint64_t off[kRayMaxLevels];
+};
+
+// per byte, alpha included: (a + b + c + d + 2) >> 2, in two SWAR words of 16-bit lanes (4 * 255 + 2 fits)
+__device__ __forceinline__ uint32_t avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    const uint32_t lo = (a & 0x00ff00ffu) + (b & 0x00ff00ffu) + (c & 0x00ff00ffu) + (d & 0x00ff00ffu) + 0x00020002u;
+    const uint32_t hi = ((a >> 8) & 0x00ff00ffu) + ((b >> 8) & 0x00ff00ffu) + ((c >> 8) & 0x00ff00ffu) + ((d >> 8) & 0x00ff00ffu) + 0x00020002u;
+    return ((lo >> 2) & 0x00ff00ffu) | (((hi >> 2) & 0x00ff00ffu) << 8);
+}
+
+__device__ __forceinline__ uint32_t ld_nc_u32(const uint32_t *p) {
+    uint32_t v;
+    asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+
+// Level 1 from the faces: texel (x, y) of plate blockIdx.y of frame blockIdx.z averages the colours of level-0 texels
+// (min(2x + i, ps - 1), min(2y + j, ps - 1)), each the colour the nearest RGBA warp draws for that texel (through the
+// plate's LUT when f_rubix is on and the texel is off the grid, then the frame's table).
+template <bool RUBIX, bool TABLES>
+__global__ void __launch_bounds__(kRayThreads) ray_pyramid_base_kernel(const __grid_constant__ RayWarpParams p, const __grid_constant__ RayPyramidParams q,
+                                                                       const __grid_constant__ LensBuildParams P, const __grid_constant__ FaceLayoutParams lay) {
+    __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
+    __shared__ uint32_t s_rgba[TABLES ? 1 : 256];
+    if (RUBIX) {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.lut);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(s_lut);
+        for (int i = threadIdx.x; i < 6 * 256 / 4; i += kRayThreads) dst[i] = __ldg(src + i);
+    }
+    if (!TABLES) {
+        for (int i = threadIdx.x; i < 256; i += kRayThreads) s_rgba[i] = __ldg(p.rgba + i);
+    }
+    if (RUBIX || !TABLES) __syncthreads();
+    const uint32_t s = q.size[1], ps = q.size[0];
+    const uint32_t t = blockIdx.x * kRayThreads + threadIdx.x;
+    if (t >= s * s) return;
+    const uint32_t y = t / s, x = t - y * s, plate = blockIdx.y, f = blockIdx.z;
+    const uint8_t *faces = p.faces + static_cast<size_t>(f) * p.face_stride + lay.plate_base[plate];
+    const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : nullptr;
+    const uint32_t x0 = 2 * x, x1 = min(2 * x + 1, ps - 1), y0 = 2 * y, y1 = min(2 * y + 1, ps - 1);
+    bool col[2] = {false, false}, row[2] = {false, false};
+    if (RUBIX) {
+        col[0] = ray_on_rubix_line(P, x0);
+        col[1] = ray_on_rubix_line(P, x1);
+        row[0] = ray_on_rubix_line(P, y0);
+        row[1] = ray_on_rubix_line(P, y1);
+    }
+    uint32_t c[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t tx = k & 1 ? x1 : x0, ty = k & 2 ? y1 : y0;
+        uint32_t b = ld_texel(faces + static_cast<size_t>(ty) * lay.rowbytes + tx);
+        if (RUBIX && !col[k & 1] && !row[k >> 1]) b = s_lut[plate * 256 + b];
+        c[k] = TABLES ? __ldg(table + b) : s_rgba[b];
+    }
+    uint32_t *out = reinterpret_cast<uint32_t *>(q.scratch + static_cast<size_t>(f) * q.stride + q.off[1]) + (static_cast<size_t>(plate) * s + y) * s + x;
+    *out = avg4(c[0], c[1], c[2], c[3]);
+}
+
+// Level `level` >= 2 from level - 1, per plate (blockIdx.y) and frame (blockIdx.z), with the same clamped 2 x 2 average.
+__global__ void __launch_bounds__(kRayThreads) ray_pyramid_reduce_kernel(const __grid_constant__ RayPyramidParams q, int level) {
+    const uint32_t s = q.size[level], sp = q.size[level - 1];
+    const uint32_t t = blockIdx.x * kRayThreads + threadIdx.x;
+    if (t >= s * s) return;
+    const uint32_t y = t / s, x = t - y * s, plate = blockIdx.y;
+    uint8_t *frame = q.scratch + static_cast<size_t>(blockIdx.z) * q.stride;
+    const uint32_t *src = reinterpret_cast<const uint32_t *>(frame + q.off[level - 1]) + static_cast<size_t>(plate) * sp * sp;
+    const uint32_t x0 = 2 * x, x1 = min(2 * x + 1, sp - 1), y0 = 2 * y, y1 = min(2 * y + 1, sp - 1);
+    const uint32_t c = avg4(src[y0 * sp + x0], src[y0 * sp + x1], src[y1 * sp + x0], src[y1 * sp + x1]);
+    reinterpret_cast<uint32_t *>(frame + q.off[level])[(static_cast<size_t>(plate) * s + y) * s + x] = c;
+}
+
+// the blend of the four tap colours 00, 10, 01, 11 with 8-bit weights (ray_bilinear_kernel's arithmetic)
+__device__ __forceinline__ uint32_t blend4(const uint32_t cq[4], uint32_t wx, uint32_t wy) {
+    const uint32_t top_lo = (cq[0] & 0x00ff00ffu) * (256 - wx) + (cq[1] & 0x00ff00ffu) * wx;
+    const uint32_t top_hi = ((cq[0] >> 8) & 0x00ff00ffu) * (256 - wx) + ((cq[1] >> 8) & 0x00ff00ffu) * wx;
+    const uint32_t bot_lo = (cq[2] & 0x00ff00ffu) * (256 - wx) + (cq[3] & 0x00ff00ffu) * wx;
+    const uint32_t bot_hi = ((cq[2] >> 8) & 0x00ff00ffu) * (256 - wx) + ((cq[3] >> 8) & 0x00ff00ffu) * wx;
+    const auto blend = [wy](uint32_t t, uint32_t b) { return (t * (256 - wy) + b * wy + 32768u) >> 16; };
+    return blend(top_lo & 0xffffu, bot_lo & 0xffffu) | blend(top_hi & 0xffffu, bot_hi & 0xffffu) << 8 | blend(top_lo >> 16, bot_lo >> 16) << 16 |
+           blend(top_hi >> 16, bot_hi >> 16) << 24;
+}
+
+// the bilinear colour at (u, v) on level L >= 1 of plate `plate` of a frame's pyramid
+__device__ __forceinline__ uint32_t level_colour(const RayPyramidParams &q, const uint8_t *pyr, int L, int plate, double u, double v) {
+    const int s = static_cast<int>(q.size[L]);
+    int x0, y0, wx, wy;
+    ray_bilinear_level(u, v, s, &x0, &y0, &wx, &wy);
+    const int tx0 = max(x0, 0), tx1 = min(x0 + 1, s - 1), ty0 = max(y0, 0), ty1 = min(y0 + 1, s - 1);
+    const uint32_t *lv = reinterpret_cast<const uint32_t *>(pyr + q.off[L]) + static_cast<size_t>(plate) * s * s;
+    const uint32_t cq[4] = {ld_nc_u32(lv + ty0 * s + tx0), ld_nc_u32(lv + ty0 * s + tx1), ld_nc_u32(lv + ty1 * s + tx0), ld_nc_u32(lv + ty1 * s + tx1)};
+    return blend4(cq, static_cast<uint32_t>(wx), static_cast<uint32_t>(wy));
+}
+
+// One thread per output pixel.  The pixel's ray (field pixel (x, y), turned by M_f) is mapped as ray_bilinear maps a
+// sample; its footprint rho is the larger distance, in level-0 texels on its plate, to where the turned rays of field
+// pixels (x + 1, y) (else (x - 1, y)) and (x, y + 1) (else (x, y - 1)) project onto that plate (ray_footprint2,
+// written out so that a backward neighbour is turned only when the forward one is missing or unusable); ray_level
+// gives L and w.  Level 0's colour is ray_bilinear_kernel's at K = 1; level L >= 1's is the same blend on the
+// pyramid's grid; the output mixes C_L and C_L+1 by w.  With one field and one matrix for every frame of the thread,
+// the plate, (u, v), L, w and the level-0 grid tests are carried.
+template <bool RUBIX, bool KEEP, bool TABLES>
+__global__ void __launch_bounds__(kRayThreads, 1) ray_trilinear_kernel(const __grid_constant__ RayWarpParams p, const __grid_constant__ RayPyramidParams q,
+                                                                    const __grid_constant__ LensBuildParams P, const __grid_constant__ FaceLayoutParams lay) {
+    __shared__ uint8_t s_lut[RUBIX ? 6 * 256 : 4];
+    __shared__ uint32_t s_rgba[TABLES ? 1 : 256];
+    if (RUBIX) {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.lut);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(s_lut);
+        for (int i = threadIdx.x; i < 6 * 256 / 4; i += kRayThreads) dst[i] = __ldg(src + i);
+    }
+    if (!TABLES) {
+        for (int i = threadIdx.x; i < 256; i += kRayThreads) s_rgba[i] = __ldg(p.rgba + i);
+    }
+    if (RUBIX || !TABLES) __syncthreads();
+
+    const uint32_t pix = blockIdx.x * kRayThreads + threadIdx.x;   // y * W + x (WarpDevice::warp_rays: W H < 2^31)
+    if (pix >= p.nitems) return;
+    const uint32_t y = pix / p.width, x = pix - y * p.width;
+    const uint32_t height = p.nitems / p.width;
+    const size_t out_at = static_cast<size_t>(y) * p.pitch + static_cast<size_t>(x) * 4;
+    const int f0 = static_cast<int>(blockIdx.y) * p.frames_per_thread;
+    const int f1 = min(p.nframes, f0 + p.frames_per_thread);
+    const bool carry = p.ray_floats == 0 && p.xform_floats == 0;   // the sample is the same in every frame
+    const int ps = P.platesize;
+
+    bool mapped = false;
+    int plate = 0, L = 0, w = 0;
+    double u = 0, v = 0;
+    uint32_t grid = 0;   // f_rubix, level 0: on-grid bits of columns x0, x0 + 1 (0, 1) and rows y0, y0 + 1 (2, 3)
+    for (int f = f0; f < f1; ++f) {
+        if (f == f0 || !carry) {
+            float M[9] = {};
+            if (p.xforms) {
+                const float *m = p.xforms + static_cast<size_t>(f) * p.xform_floats;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) M[i] = __ldg(m + i);
+            }
+            const float *field = p.rays + static_cast<size_t>(f) * p.ray_floats;
+            // the field pixel pixel + d, turned and normalised
+            const auto ray_at = [&](uint32_t at, float t[3]) {
+                const float *r = field + 3 * static_cast<size_t>(at);
+                const float ray[3] = {__ldg(r), __ldg(r + 1), __ldg(r + 2)};
+                t[0] = ray[0], t[1] = ray[1], t[2] = ray[2];
+                if (p.xforms) turn_ray(M, ray, t);
+            };
+            float n[3];
+            ray_at(pix, n);
+            int px, py;
+            mapped = ray_texel_uv(P, n, &plate, &px, &py, &u, &v);
+            L = 0;
+            w = 0;
+            if (mapped) {
+                double a, b, rx = 0, ry = 0;
+                if (ray_plate_project(P, plate, n, &a, &b)) {
+                    float t[3];
+                    double a1, b1;
+                    bool done = false;
+                    if (x + 1 < p.width) {
+                        ray_at(pix + 1, t);
+                        ray_normalize3(t);
+                        if (ray_plate_project(P, plate, t, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1), done = true;
+                    }
+                    if (!done && x > 0) {
+                        ray_at(pix - 1, t);
+                        ray_normalize3(t);
+                        if (ray_plate_project(P, plate, t, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
+                    }
+                    done = false;
+                    if (y + 1 < height) {
+                        ray_at(pix + p.width, t);
+                        ray_normalize3(t);
+                        if (ray_plate_project(P, plate, t, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1), done = true;
+                    }
+                    if (!done && y > 0) {
+                        ray_at(pix - p.width, t);
+                        ray_normalize3(t);
+                        if (ray_plate_project(P, plate, t, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
+                    }
+                }
+                ray_level(ry > rx ? ry : rx, q.lmax, &L, &w);
+                if (RUBIX && L == 0) {
+                    int x0, y0, wx, wy;
+                    ray_bilinear_level(u, v, ps, &x0, &y0, &wx, &wy);
+                    const int tx = max(x0, 0), ty = max(y0, 0), tx1 = min(x0 + 1, ps - 1), ty1 = min(y0 + 1, ps - 1);
+                    grid = static_cast<uint32_t>(ray_on_rubix_line(P, tx)) | static_cast<uint32_t>(ray_on_rubix_line(P, tx1)) << 1 |
+                           static_cast<uint32_t>(ray_on_rubix_line(P, ty)) << 2 | static_cast<uint32_t>(ray_on_rubix_line(P, ty1)) << 3;
+                }
+            }
+        }
+        if (KEEP && !mapped) continue;
+        const uint32_t *table = TABLES ? p.rgba + static_cast<size_t>(f) * p.table_words : nullptr;
+        uint32_t c;
+        if (mapped) {
+            const uint8_t *pyr = q.scratch + static_cast<size_t>(f) * q.stride;
+            if (L == 0) {
+                int x0, y0, wx, wy;
+                ray_bilinear_level(u, v, ps, &x0, &y0, &wx, &wy);
+                const int tx = max(x0, 0), ty = max(y0, 0), tx1 = min(x0 + 1, ps - 1), ty1 = min(y0 + 1, ps - 1);
+                const uint8_t *base = p.faces + static_cast<size_t>(f) * p.face_stride + lay.plate_base[plate];
+                uint32_t bq[4] = {ld_texel(base + static_cast<size_t>(ty) * lay.rowbytes + tx), ld_texel(base + static_cast<size_t>(ty) * lay.rowbytes + tx1),
+                                  ld_texel(base + static_cast<size_t>(ty1) * lay.rowbytes + tx), ld_texel(base + static_cast<size_t>(ty1) * lay.rowbytes + tx1)};
+                if (RUBIX) {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        if (!((grid >> (k & 1)) & 1u) && !((grid >> (2 + (k >> 1))) & 1u)) bq[k] = s_lut[plate * 256 + bq[k]];
+                }
+                uint32_t cq[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) cq[k] = TABLES ? __ldg(table + bq[k]) : s_rgba[bq[k]];
+                c = blend4(cq, static_cast<uint32_t>(wx), static_cast<uint32_t>(wy));
+            } else {
+                c = level_colour(q, pyr, L, plate, u, v);
+            }
+            if (w > 0) {
+                const uint32_t c1 = level_colour(q, pyr, L + 1, plate, u, v);
+                const uint32_t w1 = static_cast<uint32_t>(w), w0 = 256 - w1;
+                const uint32_t lo = (c & 0x00ff00ffu) * w0 + (c1 & 0x00ff00ffu) * w1 + 0x00800080u;
+                const uint32_t hi = ((c >> 8) & 0x00ff00ffu) * w0 + ((c1 >> 8) & 0x00ff00ffu) * w1 + 0x00800080u;
+                c = ((lo >> 8) & 0x00ff00ffu) | (hi & 0xff00ff00u);
+            }
+        } else {
+            const uint32_t bgb = __ldg(p.bg + pix);
+            c = TABLES ? __ldg(table + bgb) : s_rgba[bgb];
+        }
+        st_cs_u32(p.out + static_cast<size_t>(f) * p.out_stride + out_at, c);
+    }
+}
+
 template <bool QUAD, bool RUBIX, bool RGBA, bool KEEP, bool TABLES>
 void launch_instance(const RayWarpParams &p, const LensBuildParams &P, const FaceLayoutParams &lay, dim3 grid, cudaStream_t st) {
     ray_warp_kernel<QUAD, RUBIX, RGBA, KEEP, TABLES><<<grid, kRayThreads, 0, st>>>(p, P, lay);
@@ -473,6 +714,47 @@ void launch_bilinear(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, 
     else launch_bilinear_rubix<4>(L, p, grid, st);
 }
 
+// the pyramid of every frame (one launch per level 1..lmax), then the trilinear instance of (rubix, keep, tables):
+// 2 x 2 x 2 = 8 instances
+template <bool RUBIX, bool KEEP>
+void launch_trilinear_tables(const RayWarpLaunch &L, const RayWarpParams &p, const RayPyramidParams &q, dim3 grid, cudaStream_t st) {
+    if (L.tables) ray_trilinear_kernel<RUBIX, KEEP, true><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.layout);
+    else ray_trilinear_kernel<RUBIX, KEEP, false><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.layout);
+}
+
+template <bool RUBIX>
+void launch_trilinear_keep(const RayWarpLaunch &L, const RayWarpParams &p, const RayPyramidParams &q, dim3 grid, cudaStream_t st) {
+    if (L.keep) launch_trilinear_tables<RUBIX, true>(L, p, q, grid, st);
+    else launch_trilinear_tables<RUBIX, false>(L, p, q, grid, st);
+}
+
+template <bool RUBIX>
+void launch_pyramid_base(const RayWarpLaunch &L, const RayWarpParams &p, const RayPyramidParams &q, dim3 grid, cudaStream_t st) {
+    if (L.tables) ray_pyramid_base_kernel<RUBIX, true><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.layout);
+    else ray_pyramid_base_kernel<RUBIX, false><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.layout);
+}
+
+void launch_trilinear(const RayWarpLaunch &L, const RayWarpParams &p, dim3 grid, cudaStream_t st) {
+    RayPyramidParams q;
+    memset(&q, 0, sizeof q);
+    q.scratch = static_cast<uint8_t *>(L.scratch);
+    q.stride = L.pyramid_bytes;
+    q.lmax = L.lmax;
+    for (int l = 0; l <= L.lmax; ++l) {
+        q.size[l] = static_cast<uint32_t>(L.level_size[l]);
+        q.off[l] = L.level_off[l];
+    }
+    for (int l = 1; l <= L.lmax; ++l) {
+        const uint32_t s = q.size[l];
+        const dim3 g((s * s + kRayThreads - 1) / kRayThreads, static_cast<unsigned>(L.globe.numplates), static_cast<unsigned>(L.nframes));
+        if (l > 1) ray_pyramid_reduce_kernel<<<g, kRayThreads, 0, st>>>(q, l);
+        else if (L.rubix) launch_pyramid_base<true>(L, p, q, g, st);
+        else launch_pyramid_base<false>(L, p, q, g, st);
+    }
+    if (L.rubix) launch_trilinear_keep<true>(L, p, q, grid, st);
+    else launch_trilinear_keep<false>(L, p, q, grid, st);
+}
+
 }  // namespace
 
 bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
@@ -499,7 +781,11 @@ bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
                     static_cast<unsigned>((L.nframes + L.frames_per_thread - 1) / L.frames_per_thread));
     cudaStream_t st = static_cast<cudaStream_t>(L.stream);
     char buf[192];
-    if (L.bilinear) {
+    if (L.trilinear) {
+        launch_trilinear(L, p, grid, st);
+        snprintf(buf, sizeof buf, "ray_trilinear_kernel<rubix=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d levels=%d", L.rubix, L.keep,
+                 L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread, L.lmax);
+    } else if (L.bilinear) {
         launch_bilinear(L, p, grid, st);
         snprintf(buf, sizeof buf, "ray_bilinear_kernel<k=%d,rubix=%d,keep=%d,tables=%d> grid=(%u,%u) block=%d frames/thread=%d", L.factor, L.rubix,
                  L.keep, L.tables, grid.x, grid.y, kRayThreads, L.frames_per_thread);

@@ -1277,12 +1277,34 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
                " is beyond what a ray map takes (6 * platesize^2 must fit the 28-bit texel index)";
         return false;
     }
-    // (the supersampled and bilinear kernels index the field's pixels in 31 bits)
+    // (the supersampled, bilinear and trilinear kernels index the field's pixels in 31 bits)
     const uint64_t field_pixels = static_cast<uint64_t>(q.factor) * q.factor * static_cast<uint64_t>(cur_->width) * static_cast<uint64_t>(cur_->height);
-    if ((q.factor > 1 || q.bilinear) && field_pixels > 0x7FFFFFFFu) {
+    if ((q.factor > 1 || q.bilinear || q.trilinear) && field_pixels > 0x7FFFFFFFu) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp_rays: a field of factor^2 * width * height = " + std::to_string(field_pixels) + " pixels is beyond the kernel's 31-bit pixel index";
         return false;
+    }
+    // (the trilinear warp's pyramids: every plate of the globe, at the installed plate size)
+    int lsize[kRayMaxLevels] = {};
+    uint64_t loff[kRayMaxLevels] = {}, pyramid = 0;
+    int lmax = 0;
+    if (q.trilinear) {
+        lmax = ray_pyramid_levels(cur_->platesize, globe.numplates, lsize, loff, &pyramid);
+        err_code_ = BLINKY_E_INVALID;
+        if (pyramid > 0 && !q.scratch) {
+            err_ = "warp_rays: NULL scratch (the frames' pyramids need " + std::to_string(pyramid) + " bytes each)";
+            return false;
+        }
+        if (reinterpret_cast<uintptr_t>(q.scratch) % 16 != 0) {
+            err_ = "warp_rays: the scratch must be 16-byte aligned";
+            return false;
+        }
+        if (static_cast<uint64_t>(q.scratch_bytes) < static_cast<uint64_t>(r.nframes) * pyramid) {
+            err_ = "warp_rays: scratch_bytes " + std::to_string(q.scratch_bytes) + " is below nframes * " + std::to_string(pyramid) +
+                   " (blinky_ray_pyramid_bytes)";
+            return false;
+        }
+        err_code_ = BLINKY_E_CUDA;
     }
     size_t pitch = 0;
     if (!check_output(r, &pitch)) return false;
@@ -1301,6 +1323,14 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     RayWarpLaunch L;
     L.factor = q.factor;
     L.bilinear = q.bilinear;
+    L.trilinear = q.trilinear;
+    L.scratch = q.scratch;
+    L.pyramid_bytes = pyramid;
+    L.lmax = lmax;
+    for (int l = 0; l < kRayMaxLevels; ++l) {
+        L.level_size[l] = lsize[l];
+        L.level_off[l] = loff[l];
+    }
     L.rays = q.rays;
     L.ray_stride = q.ray_stride;
     L.xforms = q.xforms;
@@ -1317,7 +1347,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     L.width = g.width;
     L.height = g.height;
     L.nframes = r.nframes;
-    L.quads = q.factor == 1 && !q.bilinear && ray_warp_quads(r, pitch, g.width);
+    L.quads = q.factor == 1 && !q.bilinear && !q.trilinear && ray_warp_quads(r, pitch, g.width);
     const size_t npix = static_cast<size_t>(g.width) * static_cast<size_t>(g.height);
     L.frames_per_thread = ray_warp_frames_per_thread(q.ray_stride, r.nframes, static_cast<uint32_t>(L.quads ? npix / 4 : npix),
                                                      static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
@@ -1330,9 +1360,10 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     L.stream = r.stream;
     int e = 0;
     const bool ok = launch_ray_warp(L, &last_kernel_, &e);
-    ++launches_;
+    launches_ += 1 + lmax;
     if (capturing) remember_capture(r.stream, cap_id);
-    return ok ? true : fail(q.bilinear ? "ray_bilinear_kernel" : q.factor > 1 ? "ray_supersample_kernel" : "ray_warp_kernel", e);
+    return ok ? true
+              : fail(q.trilinear ? "ray_trilinear_kernel" : q.bilinear ? "ray_bilinear_kernel" : q.factor > 1 ? "ray_supersample_kernel" : "ray_warp_kernel", e);
 }
 
 bool WarpDevice::release_captures() {

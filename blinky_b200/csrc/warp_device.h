@@ -64,6 +64,9 @@ struct RayRequest {
     size_t xform_stride;        // bytes between frames (0: one matrix for every frame)
     int factor = 1;             // 2-4: a [factor * height][factor * width] field, factor^2 samples averaged per RGBA pixel
     bool bilinear = false;      // each sample bilinear-filtered from four texels (RGBA, factor 1-4)
+    bool trilinear = false;     // one sample per pixel from the two mip levels around its footprint (RGBA, factor 1)
+    void *scratch = nullptr;    // trilinear: the frames' pyramids, frame f at scratch + f * B (16-byte aligned)
+    size_t scratch_bytes = 0;   // trilinear: at least nframes * B
 };
 
 class WarpDevice {
@@ -105,7 +108,8 @@ public:
     // globe `globe` (FisheyeHost::device_params at the resident view's size, no globe_plate script): the resident
     // lensmap gives only the view's size and background.  Every plate of the globe must have an origin in the face
     // layout.  Capturable like warp().  q.factor > 1: the supersampled RGBA warp (ray_supersample_kernel);
-    // q.bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel).
+    // q.bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel); q.trilinear: the frames' pyramids in
+    // q.scratch, then the trilinear RGBA warp (ray_trilinear_kernel), lmax + 1 launches.
     bool warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go
     // of the generations held for such graphs and returns every capture counter slot to the pool.

@@ -605,6 +605,57 @@ int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_
                                      int keep_unmapped, const uint32_t *d_tables, size_t table_stride,
                                      void *stream);
 
+/* Bytes of one frame's RGBA mip pyramid for blinky_warp_device_rays_trilinear (B below): the installed
+ * lensmap's plate size ps and every plate of the current globe.  BLINKY_E_STATE with no lensmap, no
+ * valid globe, or ps beyond the ray warps' limit (6688); BLINKY_E_NODEVICE on a host-only context.  The
+ * context does not change. */
+int blinky_ray_pyramid_bytes(blinky_ctx *ctx, size_t *bytes);
+
+/* Trilinear-filtered (mip-mapped) RGBA warp from a ray field: one sample per pixel, from the two levels of
+ * a per-frame mip pyramid around the pixel's footprint, so a view that minifies the plates stays steady
+ * as it moves.  W, H, ps and the background are the installed lensmap's; the field (float32[H][W][3]),
+ * matrices, faces, face layout, tables, view rectangle and keep_unmapped are read as
+ * blinky_warp_device_rays_bilinear reads them at factor 1.
+ *   1. Pyramid, per frame, of every plate P of the globe: s_0 = ps, s_L = (s_{L-1} + 1) >> 1 down to
+ *      s_Lmax = 1 (ps = 1: Lmax = 0; 97: 7; 2048: 11).  C_0(P, x, y) = T_f[b'], the texel colour of
+ *      blinky_warp_device_rays_bilinear.  Level L >= 1, per byte, alpha included:
+ *      C_L(x, y) = (sum over i, j in {0, 1} of C_{L-1}(min(2x+i, s_{L-1}-1), min(2y+j, s_{L-1}-1)) + 2) >> 2.
+ *      Levels 1..Lmax are written as uint32 RGBA words at d_scratch + f*B (B = blinky_ray_pyramid_bytes):
+ *      level-major, then plate 0..numplates-1, then rows [s_L][s_L]; level L's plate 0 starts
+ *      4 * numplates * (s_1^2 + ... + s_{L-1}^2) bytes in, and B is the total rounded up to 256.  Level 0
+ *      is never stored: it is the faces.
+ *   2. Footprint: the pixel's ray r (field pixel (x, y) turned by M_f) is mapped on plate P exactly as
+ *      blinky_warp_device_rays_bilinear maps it, with plate coordinates (u, v); unmapped, the pixel is
+ *      T_f[bg[y][x]].  The projection of a normalised ray n onto P: x, y, z the float dot products with
+ *      P's right, up and forward, widened to double; usable iff z > 0; then q = uv_dist_P * ps / z,
+ *      a = x*q, b = -y*q (double, one IEEE operation each).  r's own projection unusable: rho^2 = 0.
+ *      Otherwise the x axis uses field pixel (x+1, y) when it exists and its turned, normalised ray
+ *      projects usably onto P, else (x-1, y) on the same terms, else it gives 0; the y axis likewise with
+ *      (x, y+1) and (x, y-1).  An axis gives da*da + db*db (the differences from r's (a, b)); rho^2 is
+ *      the x axis's value, replaced by the y axis's when that is greater.  rho = sqrt(rho^2), correctly
+ *      rounded.
+ *   3. Level and weight, by comparisons: L the largest L <= Lmax with 2^L <= rho (0 when rho < 1 or NaN);
+ *      w = (int)((rho * 2^-L - 1) * 256) when 1 <= rho and L < Lmax, else 0.
+ *   4. Colour: C_L at (u, v) is blinky_warp_device_rays_bilinear's blend on level L's grid: sx =
+ *      u*s_L - 0.5, x0 = floor(sx), wx = (int)((sx - x0)*256), likewise y, taps clamped to [0, s_L-1]
+ *      on plate P (level 0: exactly that call's colour).  The output is C_Lmax when L = Lmax, else per
+ *      byte (C_L*(256-w) + C_{L+1}*w + 128) >> 8.
+ *   5. With keep_unmapped the pixels blinky_warp_device_rays_rgba skips are skipped.
+ * Where rho < 1 at every pixel the output equals blinky_warp_device_rays_bilinear at factor 1.  The
+ * scratch is the caller's: nothing is allocated, copied or synchronised, and the pyramid bytes are left
+ * in it.  The call adds Lmax + 1 to blinky_launch_count (one launch per pyramid level 1..Lmax, then the
+ * warp); blinky_last_kernel names the warp kernel.
+ * Refuses everything blinky_warp_device_rays_bilinear refuses at factor 1, with the same codes, and
+ * launches nothing when it does; also BLINKY_E_INVALID for a NULL d_scratch while B > 0, a d_scratch
+ * that is not 16-byte aligned, and scratch_bytes < nframes * B.  Capturable like
+ * blinky_warp_device_rays_rgba, on the same terms; the context does not change. */
+int blinky_warp_device_rays_trilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride,
+                                      const float *d_rays, size_t ray_stride, const float *d_xforms,
+                                      size_t xform_stride, void *d_screen_rgba, size_t screen_frame_stride,
+                                      int rowbytes, int x0, int y0, int nframes, int keep_unmapped,
+                                      const uint32_t *d_tables, size_t table_stride, void *d_scratch,
+                                      size_t scratch_bytes, void *stream);
+
 /* one-line description of how the current lensmap was tiled for the TMA kernel
  * (tile counts per class, staged bytes per pixel); "" before a build */
 const char *blinky_plan_summary(blinky_ctx *ctx);
