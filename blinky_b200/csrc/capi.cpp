@@ -673,15 +673,16 @@ int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x
 
 // blinky_warp_device_rays[_rgba|_supersampled|_bilinear|_trilinear]: the view warp r with each pixel's texel computed
 // from its ray in q, turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours;
-// q.bilinear: RGBA, the mean of q.factor^2 bilinear samples; q.trilinear: RGBA, one sample from the frame's mip pyramid
+// Bilinear: RGBA, the mean of q.factor^2 bilinear samples; Trilinear: RGBA, one sample from the frame's mip pyramid
 // in q.scratch, whose checks are WarpDevice::warp_rays').  Every refusal launches nothing.
 int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRequest &q, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba,
                      bool supersampled = false) {
     NEED_DEVICE(ctx);
     r.keep_unmapped = keep_unmapped != 0;
     r.rgba = rgba;
-    const char *name = q.trilinear     ? "blinky_warp_device_rays_trilinear"
-                       : q.bilinear    ? "blinky_warp_device_rays_bilinear"
+    const bool bilinear = q.filter == blinky::RayFilter::Bilinear;
+    const char *name = q.filter == blinky::RayFilter::Trilinear ? "blinky_warp_device_rays_trilinear"
+                       : bilinear      ? "blinky_warp_device_rays_bilinear"
                        : supersampled  ? "blinky_warp_device_rays_supersampled"
                        : rgba          ? "blinky_warp_device_rays_rgba"
                                        : "blinky_warp_device_rays";
@@ -695,10 +696,10 @@ int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRe
     if (!q.rays) return refuse(BLINKY_E_INVALID, "NULL rays");
     if (reinterpret_cast<uintptr_t>(q.rays) % 4 != 0 || reinterpret_cast<uintptr_t>(q.xforms) % 4 != 0)
         return refuse(BLINKY_E_INVALID, "d_rays and d_xforms must be 4-byte aligned");
-    if (supersampled || q.bilinear) {
+    if (supersampled || bilinear) {
         // (the supersampled factor 1 is blinky_warp_device_rays_rgba; the bilinear one is a sample per pixel)
-        if (q.factor < (q.bilinear ? 1 : 2) || q.factor > 4)
-            return refuse(BLINKY_E_INVALID, q.bilinear ? "factor must be 1, 2, 3 or 4" : "factor must be 2, 3 or 4");
+        if (q.factor < (bilinear ? 1 : 2) || q.factor > 4)
+            return refuse(BLINKY_E_INVALID, bilinear ? "factor must be 1, 2, 3 or 4" : "factor must be 2, 3 or 4");
         if (q.ray_stride != 0 && (q.ray_stride < 12 * static_cast<size_t>(q.factor * q.factor) * static_cast<size_t>(W) * static_cast<size_t>(H) ||
                                   q.ray_stride % 4 != 0))
             return refuse(BLINKY_E_INVALID,
@@ -783,7 +784,7 @@ int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_
     r.table_stride = table_stride;
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
     q.factor = factor;
-    q.bilinear = true;
+    q.filter = blinky::RayFilter::Bilinear;
     return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
 }
 
@@ -812,7 +813,7 @@ int blinky_warp_device_rays_trilinear(blinky_ctx *ctx, const void *d_faces, size
     r.tables = d_tables;
     r.table_stride = table_stride;
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
-    q.trilinear = true;
+    q.filter = blinky::RayFilter::Trilinear;
     q.scratch = d_scratch;
     q.scratch_bytes = scratch_bytes;
     return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);

@@ -8,6 +8,7 @@
 #include <cstdint>
 
 #include "face_layout.h"
+#include "ray_warp.h"
 #include "tile_plan.h"
 #include "warp_device.h"
 
@@ -69,6 +70,20 @@ inline int ray_warp_frames_per_thread(size_t ray_stride, int nframes, uint32_t n
     const uint64_t want = (static_cast<uint64_t>(resident_threads) + std::max<uint32_t>(nitems, 1u) - 1) / std::max<uint32_t>(nitems, 1u);
     const uint64_t splits = std::min<uint64_t>(static_cast<uint64_t>(nframes), std::max<uint64_t>(want, 1u));
     return static_cast<int>(static_cast<uint64_t>(nframes) / splits);   // (rounded down: at least `splits` rows of threads)
+}
+
+// The launch shape of the ray warp q of r into a view of width x height: quads only for the nearest filter at factor 1
+// (every other filter writes one RGBA pixel per thread), frames per thread for that item count, and a grid that covers
+// every item and every frame.
+inline RayWarpShape ray_warp_shape(const WarpRequest &r, const RayRequest &q, size_t pitch, int width, int height, uint32_t resident_threads) {
+    RayWarpShape s;
+    s.quads = q.filter == RayFilter::Nearest && q.factor == 1 && ray_warp_quads(r, pitch, width);
+    const size_t npix = static_cast<size_t>(width) * static_cast<size_t>(height);
+    s.nitems = static_cast<uint32_t>(s.quads ? npix / 4 : npix);
+    s.frames_per_thread = ray_warp_frames_per_thread(q.ray_stride, r.nframes, s.nitems, resident_threads);
+    s.grid_x = (s.nitems + kRayThreads - 1) / kRayThreads;
+    s.grid_y = static_cast<uint32_t>((r.nframes + s.frames_per_thread - 1) / s.frames_per_thread);
+    return s;
 }
 
 struct RingGeometry {

@@ -73,39 +73,38 @@ BLINKY_HD bool ray_texel(const LensBuildParams &P, float ray[3], int *plate, int
     return ray_texel_uv(P, ray, plate, px, py, &u, &v);
 }
 
-// The bilinear sample of the unnormalised ray (normalised here, in place; blinky_warp_device_rays_bilinear): mapped
-// exactly when ray_texel maps it, on the same plate.  Then, in double, sx = u * ps - 0.5, x0 = floor(sx) and
-// wx = (int)((sx - x0) * 256), and likewise sy, y0 and wy from v.  x0 and y0 lie in [-1, ps - 1] (u * ps < ps because
-// the texel is in range) and wx, wy in [0, 255] (sx - floor(sx) is exact and below 1); the caller clamps the taps x0,
-// x0 + 1, y0, y0 + 1 to [0, ps - 1].
-BLINKY_HD bool ray_bilinear(const LensBuildParams &P, float ray[3], int *plate, int *x0, int *y0, int *wx, int *wy) {
-    int px, py;
-    double u, v;
-    if (!ray_texel_uv(P, ray, plate, &px, &py, &u, &v)) return false;
-    const int ps = P.platesize;
-    const double sx = u * ps - 0.5, sy = v * ps - 0.5;
+// The bilinear position on a grid of `size` texels per plate side, from the plate coordinates (u, v), in double:
+// sx = u * size - 0.5, x0 = floor(sx), wx = (int)((sx - x0) * 256), and likewise y0, wy; the caller clamps the taps
+// x0, x0 + 1, y0, y0 + 1 to [0, size - 1].
+BLINKY_HD void ray_bilinear_level(double u, double v, int size, int *x0, int *y0, int *wx, int *wy) {
+    const double sx = u * size - 0.5, sy = v * size - 0.5;
     const double fx = floor(sx), fy = floor(sy);
     *x0 = static_cast<int>(fx);
     *y0 = static_cast<int>(fy);
     *wx = static_cast<int>((sx - fx) * 256);
     *wy = static_cast<int>((sy - fy) * 256);
+}
+
+// The bilinear sample of the unnormalised ray (normalised here, in place; blinky_warp_device_rays_bilinear): mapped
+// exactly when ray_texel maps it, on the same plate, at ray_bilinear_level's position on the plate's ps texels.  x0
+// and y0 lie in [-1, ps - 1] (u * ps < ps because the texel is in range) and wx, wy in [0, 255] (sx - floor(sx) is
+// exact and below 1).
+BLINKY_HD bool ray_bilinear(const LensBuildParams &P, float ray[3], int *plate, int *x0, int *y0, int *wx, int *wy) {
+    int px, py;
+    double u, v;
+    if (!ray_texel_uv(P, ray, plate, &px, &py, &u, &v)) return false;
+    ray_bilinear_level(u, v, P.platesize, x0, y0, wx, wy);
     return true;
 }
 
-// on_rubix_grid: texel (px, py) lies in the padding between the rubix cells
-BLINKY_HD bool ray_on_rubix_grid(const LensBuildParams &P, int px, int py) {
-    const double ux = static_cast<double>(px) / P.rubix_unit_px;
-    const double uy = static_cast<double>(py) / P.rubix_unit_px;
-    return fmod(ux, P.rubix_block) < P.rubix_pad || fmod(uy, P.rubix_block) < P.rubix_pad;
-}
-
-// one axis of ray_on_rubix_grid, the same arithmetic: texel column (or row) t lies in the padding between the rubix
-// cells, so that texel (px, py) is on the grid exactly when column px or row py is.  (A separate copy: expressing
-// ray_on_rubix_grid through it changes the machine code of the existing warps.)
+// one axis of on_rubix_grid: texel column (or row) t lies in the padding between the rubix cells
 BLINKY_HD bool ray_on_rubix_line(const LensBuildParams &P, int t) {
     const double ut = static_cast<double>(t) / P.rubix_unit_px;
     return fmod(ut, P.rubix_block) < P.rubix_pad;
 }
+
+// on_rubix_grid: texel (px, py) lies in the padding between the rubix cells, as column px or row py does
+BLINKY_HD bool ray_on_rubix_grid(const LensBuildParams &P, int px, int py) { return ray_on_rubix_line(P, px) || ray_on_rubix_line(P, py); }
 
 // ---- trilinear (blinky_warp_device_rays_trilinear, DESIGN §3g) ------------------------------------------------------
 
@@ -156,20 +155,33 @@ BLINKY_HD double ray_axis_rho2(double a, double b, double a1, double b1) {
 }
 
 // rho^2, the squared footprint in level-0 texels of a sample on plate `plate` whose normalised ray is n, from the
-// normalised (turned) rays of its field neighbours, nullptr where that field pixel does not exist.  0 when n's own
-// projection is not usable.  Per axis: the forward neighbour (x + 1, or y + 1) when it exists and its projection onto
-// the plate is usable, else the backward one (x - 1, y - 1) on the same terms, else the axis gives 0.  rho^2 is the x
+// normalised (turned) rays of its field neighbours: neighbour(k, t) writes neighbour k — 0: (x + 1, y), 1: (x - 1, y),
+// 2: (x, y + 1), 3: (x, y - 1) — to t, or returns false where that field pixel does not exist.  0 when n's own
+// projection is not usable.  Per axis: the forward neighbour when it exists and its projection onto the plate is
+// usable, else the backward one on the same terms (asked for only then), else the axis gives 0.  rho^2 is the x
 // axis's value, replaced by the y axis's when that is greater (so a NaN x axis stays; a NaN y axis is ignored).
-BLINKY_HD double ray_footprint2(const LensBuildParams &P, int plate, const float n[3], const float *xf, const float *xb, const float *yf,
-                                const float *yb) {
+template <class Neighbour>
+BLINKY_HD double ray_footprint2(const LensBuildParams &P, int plate, const float n[3], const Neighbour &neighbour) {
     double a, b, a1, b1;
     if (!ray_plate_project(P, plate, n, &a, &b)) return 0;
+    float t[3];
     double rx = 0, ry = 0;
-    if (xf && ray_plate_project(P, plate, xf, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
-    else if (xb && ray_plate_project(P, plate, xb, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
-    if (yf && ray_plate_project(P, plate, yf, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
-    else if (yb && ray_plate_project(P, plate, yb, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
+    if (neighbour(0, t) && ray_plate_project(P, plate, t, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
+    else if (neighbour(1, t) && ray_plate_project(P, plate, t, &a1, &b1)) rx = ray_axis_rho2(a, b, a1, b1);
+    if (neighbour(2, t) && ray_plate_project(P, plate, t, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
+    else if (neighbour(3, t) && ray_plate_project(P, plate, t, &a1, &b1)) ry = ray_axis_rho2(a, b, a1, b1);
     return ry > rx ? ry : rx;
+}
+
+// ray_footprint2 from neighbour rays already turned and normalised, nullptr where that field pixel does not exist
+BLINKY_HD double ray_footprint2(const LensBuildParams &P, int plate, const float n[3], const float *xf, const float *xb, const float *yf,
+                                const float *yb) {
+    const float *const nb[4] = {xf, xb, yf, yb};
+    return ray_footprint2(P, plate, n, [&](int k, float t[3]) {
+        if (!nb[k]) return false;
+        t[0] = nb[k][0], t[1] = nb[k][1], t[2] = nb[k][2];
+        return true;
+    });
 }
 
 // The level and weight of a footprint, by comparisons only: rho = sqrt(rho2), correctly rounded; *L the largest
@@ -186,19 +198,6 @@ BLINKY_HD void ray_level(double rho2, int lmax, int *L, int *w) {
     }
     *L = l;
     *w = rho >= 1 && l < lmax ? static_cast<int>((rho * inv - 1) * 256) : 0;
-}
-
-// ray_bilinear's position arithmetic on a grid of `size` texels per plate side, from the plate coordinates (u, v):
-// sx = u * size - 0.5, x0 = floor(sx), wx = (int)((sx - x0) * 256), and likewise y0, wy; the caller clamps the taps
-// x0, x0 + 1, y0, y0 + 1 to [0, size - 1].  (size = ps gives ray_bilinear's values; a separate copy, so that the
-// bilinear warp's machine code stays as it is.)
-BLINKY_HD void ray_bilinear_level(double u, double v, int size, int *x0, int *y0, int *wx, int *wy) {
-    const double sx = u * size - 0.5, sy = v * size - 0.5;
-    const double fx = floor(sx), fy = floor(sy);
-    *x0 = static_cast<int>(fx);
-    *y0 = static_cast<int>(fy);
-    *wx = static_cast<int>((sx - fx) * 256);
-    *wy = static_cast<int>((sy - fy) * 256);
 }
 
 // The packed lensmap entry (BLINKY_LM_*) blinky_set_raymap installs for the ray turned by M (nullptr: the ray as it

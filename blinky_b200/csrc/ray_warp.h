@@ -12,10 +12,27 @@
 
 namespace blinky {
 
+constexpr int kRayThreads = 256;   // threads per CTA of every ray-warp kernel
+
+// How each sample of a ray warp takes its colour: the nearest texel (ray_warp_kernel at factor 1,
+// ray_supersample_kernel at 2-4), four texels blended (ray_bilinear_kernel, factor 1-4), or two mip levels' bilinear
+// colours blended (the pyramid launches, then ray_trilinear_kernel, factor 1).  Every filter but Nearest at factor 1
+// writes RGBA.
+enum class RayFilter { Nearest, Bilinear, Trilinear };
+
+// The launch shape of a ray warp (ray_warp_shape, launch_plan.h): one thread per item — a 4-pixel quad of a row
+// (quads) or one output pixel — in grid_x CTAs of kRayThreads per row of threads, and grid_y rows of
+// frames_per_thread frames each.
+struct RayWarpShape {
+    bool quads;
+    uint32_t nitems;            // items per frame: W * H / 4 quads or W * H pixels
+    int frames_per_thread;
+    uint32_t grid_x, grid_y;
+};
+
 struct RayWarpLaunch {
-    int factor;                 // 1: ray_warp_kernel; 2-4: ray_supersample_kernel, k x k samples per pixel (RGBA, never quads)
-    bool bilinear;              // ray_bilinear_kernel, factor 1-4: k x k bilinear samples per pixel (RGBA, never quads)
-    bool trilinear;             // the pyramid launches, then ray_trilinear_kernel (factor 1, RGBA, never quads)
+    RayFilter filter;
+    int factor;                 // k: k x k samples per pixel from a [k * height][k * width] field
     void *scratch;              // trilinear: frame 0's pyramid (16-byte aligned; frame f's at scratch + f * pyramid_bytes)
     size_t pyramid_bytes;       // trilinear: B, one frame's pyramid (ray_pyramid_levels)
     int lmax;                   // trilinear: the top level (0: no pyramid, plates of one texel)
@@ -35,17 +52,23 @@ struct RayWarpLaunch {
     size_t out_stride;          // bytes between frames
     uint32_t pitch;             // bytes between output rows
     int width, height, nframes;
-    int frames_per_thread;      // ray_warp_frames_per_thread (launch_plan.h)
-    bool quads;                 // ray_warp_quads (launch_plan.h)
+    RayWarpShape shape;
     bool rubix, rgba, keep, tables;
     LensBuildParams globe;      // FisheyeHost::device_params of the current globe at the view's size
     FaceLayoutParams layout;    // plate_base and rowbytes address every plate of the globe (dense faces included)
     void *stream;               // cudaStream_t
 };
 
-// Launches ray_warp_kernel (factor 1), ray_supersample_kernel, ray_bilinear_kernel (bilinear) or, for trilinear, one
-// pyramid launch per level 1..lmax and ray_trilinear_kernel for L.  false with the CUDA error in *cuda_err; *name: the
-// instance and launch shape of the warp kernel (last_kernel).
+// The name of the kernel a ray warp launches (last_kernel, and the failure it reports)
+inline const char *ray_warp_kernel_name(RayFilter filter, int factor) {
+    return filter == RayFilter::Trilinear ? "ray_trilinear_kernel"
+           : filter == RayFilter::Bilinear ? "ray_bilinear_kernel"
+           : factor > 1                    ? "ray_supersample_kernel"
+                                           : "ray_warp_kernel";
+}
+
+// Launches the instance of L.filter's kernel in L.shape (for trilinear, one pyramid launch per level 1..lmax first).
+// false with the CUDA error in *cuda_err; *name: the instance and launch shape of the warp kernel (last_kernel).
 bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err);
 
 }  // namespace blinky

@@ -1279,7 +1279,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     }
     // (the supersampled, bilinear and trilinear kernels index the field's pixels in 31 bits)
     const uint64_t field_pixels = static_cast<uint64_t>(q.factor) * q.factor * static_cast<uint64_t>(cur_->width) * static_cast<uint64_t>(cur_->height);
-    if ((q.factor > 1 || q.bilinear || q.trilinear) && field_pixels > 0x7FFFFFFFu) {
+    if ((q.factor > 1 || q.filter != RayFilter::Nearest) && field_pixels > 0x7FFFFFFFu) {
         err_code_ = BLINKY_E_INVALID;
         err_ = "warp_rays: a field of factor^2 * width * height = " + std::to_string(field_pixels) + " pixels is beyond the kernel's 31-bit pixel index";
         return false;
@@ -1288,7 +1288,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     int lsize[kRayMaxLevels] = {};
     uint64_t loff[kRayMaxLevels] = {}, pyramid = 0;
     int lmax = 0;
-    if (q.trilinear) {
+    if (q.filter == RayFilter::Trilinear) {
         lmax = ray_pyramid_levels(cur_->platesize, globe.numplates, lsize, loff, &pyramid);
         err_code_ = BLINKY_E_INVALID;
         if (pyramid > 0 && !q.scratch) {
@@ -1321,9 +1321,8 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     unsigned long long cap_id = 0;
     if (!capture_info(r.stream, &capturing, &cap_id)) return false;
     RayWarpLaunch L;
+    L.filter = q.filter;
     L.factor = q.factor;
-    L.bilinear = q.bilinear;
-    L.trilinear = q.trilinear;
     L.scratch = q.scratch;
     L.pyramid_bytes = pyramid;
     L.lmax = lmax;
@@ -1347,10 +1346,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     L.width = g.width;
     L.height = g.height;
     L.nframes = r.nframes;
-    L.quads = q.factor == 1 && !q.bilinear && !q.trilinear && ray_warp_quads(r, pitch, g.width);
-    const size_t npix = static_cast<size_t>(g.width) * static_cast<size_t>(g.height);
-    L.frames_per_thread = ray_warp_frames_per_thread(q.ray_stride, r.nframes, static_cast<uint32_t>(L.quads ? npix / 4 : npix),
-                                                     static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
+    L.shape = ray_warp_shape(r, q, pitch, g.width, g.height, static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
     L.rubix = rubix_;
     L.rgba = r.rgba;
     L.keep = r.keep_unmapped;
@@ -1362,8 +1358,7 @@ bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const Lens
     const bool ok = launch_ray_warp(L, &last_kernel_, &e);
     launches_ += 1 + lmax;
     if (capturing) remember_capture(r.stream, cap_id);
-    return ok ? true
-              : fail(q.trilinear ? "ray_trilinear_kernel" : q.bilinear ? "ray_bilinear_kernel" : q.factor > 1 ? "ray_supersample_kernel" : "ray_warp_kernel", e);
+    return ok ? true : fail(ray_warp_kernel_name(q.filter, q.factor), e);
 }
 
 bool WarpDevice::release_captures() {

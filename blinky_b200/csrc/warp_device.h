@@ -14,6 +14,7 @@
 
 #include "device_buffer.h"
 #include "face_layout.h"
+#include "ray_warp.h"   // RayFilter
 
 namespace blinky {
 
@@ -63,8 +64,7 @@ struct RayRequest {
     const float *xforms;        // frame 0's 3x3 matrix, row-major (nullptr: the rays as they are)
     size_t xform_stride;        // bytes between frames (0: one matrix for every frame)
     int factor = 1;             // 2-4: a [factor * height][factor * width] field, factor^2 samples averaged per RGBA pixel
-    bool bilinear = false;      // each sample bilinear-filtered from four texels (RGBA, factor 1-4)
-    bool trilinear = false;     // one sample per pixel from the two mip levels around its footprint (RGBA, factor 1)
+    RayFilter filter = RayFilter::Nearest;   // Bilinear: factor 1-4; Trilinear: factor 1, the two mip levels around the footprint
     void *scratch = nullptr;    // trilinear: the frames' pyramids, frame f at scratch + f * B (16-byte aligned)
     size_t scratch_bytes = 0;   // trilinear: at least nframes * B
 };
@@ -108,7 +108,7 @@ public:
     // globe `globe` (FisheyeHost::device_params at the resident view's size, no globe_plate script): the resident
     // lensmap gives only the view's size and background.  Every plate of the globe must have an origin in the face
     // layout.  Capturable like warp().  q.factor > 1: the supersampled RGBA warp (ray_supersample_kernel);
-    // q.bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel); q.trilinear: the frames' pyramids in
+    // Bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel); Trilinear: the frames' pyramids in
     // q.scratch, then the trilinear RGBA warp (ray_trilinear_kernel), lmax + 1 launches.
     bool warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go

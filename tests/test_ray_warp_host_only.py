@@ -36,6 +36,18 @@ extern "C" int quads(int width, size_t opx, uintptr_t out, size_t pitch, size_t 
 extern "C" int frames_per_thread(size_t ray_stride, int nframes, uint32_t nitems, uint32_t resident) {
     return ray_warp_frames_per_thread(ray_stride, nframes, nitems, resident);
 }
+extern "C" void shape(int filter, int factor, int width, int height, int rgba, uintptr_t out, size_t pitch, size_t out_stride, int nframes,
+                      size_t ray_stride, uint32_t resident, uint32_t *o) {
+    WarpRequest r(nullptr, 0, reinterpret_cast<void *>(out), out_stride, nframes, nullptr);
+    r.rgba = rgba != 0;
+    RayRequest q = {nullptr, ray_stride, nullptr, 0};
+    q.factor = factor;
+    q.filter = static_cast<RayFilter>(filter);
+    const RayWarpShape s = ray_warp_shape(r, q, pitch, width, height, resident);
+    const uint32_t v[5] = {s.quads, s.nitems, static_cast<uint32_t>(s.frames_per_thread), s.grid_x, s.grid_y};
+    for (int i = 0; i < 5; ++i) o[i] = v[i];
+}
+extern "C" const char *kernel_name(int filter, int factor) { return ray_warp_kernel_name(static_cast<RayFilter>(filter), factor); }
 """
 
 
@@ -53,6 +65,9 @@ def lib(tmp_path_factory):
     so_lib.entries.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     so_lib.quads.argtypes = [ctypes.c_int, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int]
     so_lib.frames_per_thread.argtypes = [ctypes.c_size_t, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
+    so_lib.shape.argtypes = [ctypes.c_int] * 5 + [ctypes.c_size_t] * 3 + [ctypes.c_int, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_void_p]
+    so_lib.kernel_name.argtypes = [ctypes.c_int, ctypes.c_int]
+    so_lib.kernel_name.restype = ctypes.c_char_p
     return so_lib
 
 
@@ -204,6 +219,43 @@ def test_launch_decision(lib):
             assert 1 <= f <= n
             assert rows * nitems >= min(resident, n * nitems), (nitems, n, f)   # enough threads, when there are enough frames
             assert f == 1 or (rows - 1) * nitems < 2 * resident, (nitems, n, f)   # and not many more
+
+
+NEAREST, BILINEAR, TRILINEAR = 0, 1, 2   # RayFilter
+
+
+def test_launch_shape(lib):
+    """ray_warp_shape over every filter and factor, on aligned and unaligned views: quads only for the nearest filter at
+    factor 1 (a quad instance launched with one item per pixel would read rays and background four times past their
+    end), and a grid that covers every item and every frame"""
+    o = np.zeros(5, np.uint32)
+    resident = 132 * 2048
+    seen = set()
+    for filt, factors in ((NEAREST, (1, 2, 3, 4)), (BILINEAR, (1, 2, 3, 4)), (TRILINEAR, (1,))):
+        for k in factors:
+            for w, h in ((96, 64), (94, 64), (3840, 2160), (640, 480), (1, 1), (5, 3), (4, 1)):
+                for rgba in ((0, 1) if filt == NEAREST and k == 1 else (1,)):
+                    opx = 4 if rgba else 1
+                    pitch = -(-w * opx // 16) * 16
+                    for origin, p in ((4096, pitch), (4096 + opx, pitch), (4096, pitch + opx)):
+                        for ray_stride in (0, 12 * k * k * w * h):
+                            for n in (1, 3, 400):
+                                lib.shape(filt, k, w, h, rgba, origin, p, p * h, n, ray_stride, resident, o.ctypes.data)
+                                quads, nitems, fpt, gx, gy = (int(v) for v in o)
+                                what = (filt, k, w, h, rgba, origin, p, ray_stride, n, o.tolist())
+                                if quads:
+                                    assert filt == NEAREST and k == 1 and w % 4 == 0 and nitems * 4 == w * h, what
+                                else:
+                                    assert nitems == w * h, what
+                                assert gx * 256 >= nitems > (gx - 1) * 256, what
+                                assert 1 <= fpt <= n and gy * fpt >= n > (gy - 1) * fpt, what
+                                assert fpt == 1 or ray_stride == 0, what
+                                seen.add((filt, k, quads))
+    assert (NEAREST, 1, 1) in seen and (NEAREST, 1, 0) in seen
+    assert lib.kernel_name(NEAREST, 1) == b"ray_warp_kernel"
+    assert all(lib.kernel_name(NEAREST, k) == b"ray_supersample_kernel" for k in (2, 3, 4))
+    assert all(lib.kernel_name(BILINEAR, k) == b"ray_bilinear_kernel" for k in (1, 2, 3, 4))
+    assert lib.kernel_name(TRILINEAR, 1) == b"ray_trilinear_kernel"
 
 
 # ---- binding and host-only context -------------------------------------------------------------------------------
