@@ -15,6 +15,7 @@
 #include <string>
 
 #include "fisheye_host.h"
+#include "launch_plan.h"
 #include "lens_device.h"
 #include "lua_transpile.h"
 #include "ray_texel.h"
@@ -629,93 +630,29 @@ int blinky_set_background(blinky_ctx *ctx, const uint8_t *bg) {
 
 namespace {
 
-// The one way into the device-resident warp: frames land in the view rectangle at (x0, y0) of the screens r.out, whose
-// rows are rowbytes bytes apart.  The dense entry points are the rectangle that is the whole screen.
-int warp_into_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0) {
-    const size_t bpp = r.rgba ? 4 : 1;
-    r.out_pitch = static_cast<size_t>(rowbytes);
-    r.out = static_cast<uint8_t *>(r.out) + static_cast<size_t>(y0) * r.out_pitch + static_cast<size_t>(x0) * bpp;
-    return ctx->dev->warp(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
+blinky::GlobeState globe_state(blinky_ctx *ctx) {
+    blinky::GlobeState g;
+    g.valid = ctx->host.globe_valid();
+    g.plate_script = ctx->host.has_globe_plate();
+    g.plates = ctx->host.numplates();
+    return g;
 }
 
-// The checks of the view entry points, r in keep_unmapped / rgba mode into the view rectangle at (x0, y0): BLINKY_OK or
-// the refusal.  with_tables: r.tables / r.table_stride are checked too.
-int check_view(blinky_ctx *ctx, const char *name, const blinky::WarpRequest &r, int rowbytes, int x0, int y0, bool with_tables) {
-    auto invalid = [&](const char *why) { return set_err(ctx, BLINKY_E_INVALID, std::string(name) + ": " + why); };
-    const int64_t W = ctx->dev->width(), H = ctx->dev->height(), bpp = r.rgba ? 4 : 1;
-    if (!r.faces || !r.out) return invalid("NULL buffer");
-    if (x0 < 0 || y0 < 0) return invalid("the view origin (x0, y0) must not be negative");
-    if (static_cast<int64_t>(rowbytes) < (x0 + W) * bpp) return invalid("rowbytes too small for the view rectangle");
-    if (r.nframes > 1 && static_cast<uint64_t>(r.out_stride) < static_cast<uint64_t>((y0 + H) * rowbytes))
-        return invalid("screen_frame_stride too small for the view rectangle");
-    if (r.rgba && ((reinterpret_cast<uintptr_t>(r.out) + static_cast<uintptr_t>(y0) * static_cast<uintptr_t>(rowbytes)) % 4 != 0 || rowbytes % 4 != 0 ||
-                   (r.nframes > 1 && r.out_stride % 4 != 0)))
-        return invalid("the RGBA view origin, rowbytes and screen_frame_stride must be 4-byte aligned");
-    if (with_tables) {
-        // (16 bytes: the ring kernel restages a frame's table with 128-bit loads)
-        if (!r.tables || reinterpret_cast<uintptr_t>(r.tables) % 16 != 0) return invalid("d_tables must be a non-NULL, 16-byte aligned device pointer");
-        if (r.table_stride != 0 && (r.table_stride < 256 * sizeof(uint32_t) || r.table_stride % 16 != 0 || r.table_stride / 4 > UINT32_MAX))
-            return invalid("table_stride must be 0 (one table for every frame) or at least 1024, a multiple of 16 and below 16 GB");
-    }
-    return BLINKY_OK;
-}
-
-// The view entry points: the warp r in keep_unmapped / rgba mode into the view rectangle at (x0, y0), checked first.
-// with_tables: blinky_warp_device_view_rgba_tables (rgba), whose r.tables / r.table_stride are checked here too.
-int warp_device_view(blinky_ctx *ctx, blinky::WarpRequest r, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba, bool with_tables = false) {
+// The view entry points: r into the view rectangle at (x0, y0) of screens whose rows are rowbytes bytes apart, from
+// the faces or, with q, from the rays in q turned through the current globe (WarpDevice::warp_rays).  Every refusal
+// launches nothing.
+int warp_view(blinky_ctx *ctx, blinky::WarpRequest r, blinky::WarpEntry entry, int rowbytes, int x0, int y0, int keep_unmapped,
+              const blinky::RayRequest *q = nullptr) {
     NEED_DEVICE(ctx);
+    r.entry = entry;
+    r.rowbytes = rowbytes;
+    r.x0 = x0;
+    r.y0 = y0;
     r.keep_unmapped = keep_unmapped != 0;
-    r.rgba = rgba;
-    const char *name = with_tables ? "blinky_warp_device_view_rgba_tables" : r.rgba ? "blinky_warp_device_view_rgba" : "blinky_warp_device_view";
-    const int rc = check_view(ctx, name, r, rowbytes, x0, y0, with_tables);
-    return rc != BLINKY_OK ? rc : warp_into_view(ctx, r, rowbytes, x0, y0);
-}
-
-// blinky_warp_device_rays[_rgba|_supersampled|_bilinear|_trilinear]: the view warp r with each pixel's texel computed
-// from its ray in q, turned, through the current globe (supersampled: RGBA, the mean of q.factor^2 rays' colours;
-// Bilinear: RGBA, the mean of q.factor^2 bilinear samples; Trilinear: RGBA, one sample from the frame's mip pyramid
-// in q.scratch, whose checks are WarpDevice::warp_rays').  Every refusal launches nothing.
-int warp_device_rays(blinky_ctx *ctx, blinky::WarpRequest r, const blinky::RayRequest &q, int rowbytes, int x0, int y0, int keep_unmapped, bool rgba,
-                     bool supersampled = false) {
-    NEED_DEVICE(ctx);
-    r.keep_unmapped = keep_unmapped != 0;
-    r.rgba = rgba;
-    const bool bilinear = q.filter == blinky::RayFilter::Bilinear;
-    const char *name = q.filter == blinky::RayFilter::Trilinear ? "blinky_warp_device_rays_trilinear"
-                       : bilinear      ? "blinky_warp_device_rays_bilinear"
-                       : supersampled  ? "blinky_warp_device_rays_supersampled"
-                       : rgba          ? "blinky_warp_device_rays_rgba"
-                                       : "blinky_warp_device_rays";
-    auto refuse = [&](int code, const std::string &why) { return set_err(ctx, code, std::string(name) + ": " + why); };
-    const int W = ctx->dev->width(), H = ctx->dev->height(), ps = ctx->dev->platesize();
-    if (W <= 0) return refuse(BLINKY_E_STATE, "no lensmap installed (the view's size and background are the installed lensmap's)");
-    if (!ctx->host.globe_valid()) return refuse(BLINKY_E_STATE, "no valid globe");
-    if (ctx->host.has_globe_plate())
-        return refuse(BLINKY_E_STATE, "the globe picks its plates with a globe_plate script, whose decisions can need the interpreter: "
-                                      "map such rays with blinky_set_raymap_device and warp the installed lensmap");
-    if (!q.rays) return refuse(BLINKY_E_INVALID, "NULL rays");
-    if (reinterpret_cast<uintptr_t>(q.rays) % 4 != 0 || reinterpret_cast<uintptr_t>(q.xforms) % 4 != 0)
-        return refuse(BLINKY_E_INVALID, "d_rays and d_xforms must be 4-byte aligned");
-    if (supersampled || bilinear) {
-        // (the supersampled factor 1 is blinky_warp_device_rays_rgba; the bilinear one is a sample per pixel)
-        if (q.factor < (bilinear ? 1 : 2) || q.factor > 4)
-            return refuse(BLINKY_E_INVALID, bilinear ? "factor must be 1, 2, 3 or 4" : "factor must be 2, 3 or 4");
-        if (q.ray_stride != 0 && (q.ray_stride < 12 * static_cast<size_t>(q.factor * q.factor) * static_cast<size_t>(W) * static_cast<size_t>(H) ||
-                                  q.ray_stride % 4 != 0))
-            return refuse(BLINKY_E_INVALID,
-                          "ray_stride must be 0 (one field for every frame) or a multiple of 4 of at least 12 * factor^2 * width * height");
-    }
-    if (q.ray_stride != 0 && (q.ray_stride < 12 * static_cast<size_t>(W) * static_cast<size_t>(H) || q.ray_stride % 4 != 0))
-        return refuse(BLINKY_E_INVALID, "ray_stride must be 0 (one field for every frame) or a multiple of 4 of at least 12 * width * height");
-    if (q.xform_stride != 0 && (q.xform_stride < 36 || q.xform_stride % 4 != 0))
-        return refuse(BLINKY_E_INVALID, "xform_stride must be 0 (one matrix for every frame) or a multiple of 4 of at least 36");
-    if (r.nframes > 65535) return refuse(BLINKY_E_INVALID, "at most 65535 frames per launch");
-    const int rc = check_view(ctx, name, r, rowbytes, x0, y0, rgba && r.tables);
-    if (rc != BLINKY_OK) return rc;
-    const blinky::LensBuildParams globe = ctx->host.device_params(W, H, ps);
-    r.out_pitch = static_cast<size_t>(rowbytes);
-    r.out = static_cast<uint8_t *>(r.out) + static_cast<size_t>(y0) * r.out_pitch + static_cast<size_t>(x0) * (rgba ? 4 : 1);
-    return ctx->dev->warp_rays(r, q, globe) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
+    r.rgba = entry != blinky::WarpEntry::View && entry != blinky::WarpEntry::Rays;
+    const bool ok = q ? ctx->dev->warp_rays(r, *q, globe_state(ctx), ctx->host.device_params(ctx->dev->width(), ctx->dev->height(), ctx->dev->platesize()))
+                      : ctx->dev->warp(r);
+    return ok ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 }  // namespace
@@ -725,17 +662,21 @@ extern "C" {
 int blinky_warp_device(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_out, size_t out_stride,
                        int nframes, void *stream) {
     NEED_DEVICE(ctx);
-    return warp_into_view(ctx, blinky::WarpRequest(d_faces, face_stride, d_out, out_stride, nframes, stream), ctx->dev->width(), 0, 0);
+    blinky::WarpRequest r(d_faces, face_stride, d_out, out_stride, nframes, stream);
+    r.entry = blinky::WarpEntry::Dense;
+    return ctx->dev->warp(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int blinky_warp_device_view(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
                             int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
-    return warp_device_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, rowbytes, x0, y0, keep_unmapped, false);
+    return warp_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, blinky::WarpEntry::View, rowbytes, x0, y0,
+                     keep_unmapped);
 }
 
 int blinky_warp_device_view_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen, size_t screen_frame_stride,
                                  int rowbytes, int x0, int y0, int nframes, int keep_unmapped, void *stream) {
-    return warp_device_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, rowbytes, x0, y0, keep_unmapped, true);
+    return warp_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, blinky::WarpEntry::ViewRgba, rowbytes, x0,
+                     y0, keep_unmapped);
 }
 
 int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, size_t face_stride, void *d_screen_rgba,
@@ -744,14 +685,15 @@ int blinky_warp_device_view_rgba_tables(blinky_ctx *ctx, const void *d_faces, si
     blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
     r.tables = d_tables;
     r.table_stride = table_stride;
-    return warp_device_view(ctx, r, rowbytes, x0, y0, keep_unmapped, true, true);
+    return warp_view(ctx, r, blinky::WarpEntry::ViewRgbaTables, rowbytes, x0, y0, keep_unmapped);
 }
 
 int blinky_warp_device_rays(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride, const float *d_xforms,
                             size_t xform_stride, void *d_screen, size_t screen_frame_stride, int rowbytes, int x0, int y0, int nframes,
                             int keep_unmapped, void *stream) {
-    return warp_device_rays(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, {d_rays, ray_stride, d_xforms, xform_stride},
-                            rowbytes, x0, y0, keep_unmapped, false);
+    const blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
+    return warp_view(ctx, {d_faces, face_stride, d_screen, screen_frame_stride, nframes, stream}, blinky::WarpEntry::Rays, rowbytes, x0, y0,
+                     keep_unmapped, &q);
 }
 
 int blinky_warp_device_rays_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
@@ -760,7 +702,8 @@ int blinky_warp_device_rays_rgba(blinky_ctx *ctx, const void *d_faces, size_t fa
     blinky::WarpRequest r(d_faces, face_stride, d_screen_rgba, screen_frame_stride, nframes, stream);
     r.tables = d_tables;
     r.table_stride = table_stride;
-    return warp_device_rays(ctx, r, {d_rays, ray_stride, d_xforms, xform_stride}, rowbytes, x0, y0, keep_unmapped, true);
+    const blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
+    return warp_view(ctx, r, blinky::WarpEntry::RaysRgba, rowbytes, x0, y0, keep_unmapped, &q);
 }
 
 int blinky_warp_device_rays_supersampled(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
@@ -772,7 +715,7 @@ int blinky_warp_device_rays_supersampled(blinky_ctx *ctx, const void *d_faces, s
     r.table_stride = table_stride;
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
     q.factor = factor;
-    return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true, true);
+    return warp_view(ctx, r, blinky::WarpEntry::RaysSupersampled, rowbytes, x0, y0, keep_unmapped, &q);
 }
 
 int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
@@ -785,24 +728,19 @@ int blinky_warp_device_rays_bilinear(blinky_ctx *ctx, const void *d_faces, size_
     blinky::RayRequest q = {d_rays, ray_stride, d_xforms, xform_stride};
     q.factor = factor;
     q.filter = blinky::RayFilter::Bilinear;
-    return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
+    return warp_view(ctx, r, blinky::WarpEntry::RaysBilinear, rowbytes, x0, y0, keep_unmapped, &q);
 }
 
 int blinky_ray_pyramid_bytes(blinky_ctx *ctx, size_t *bytes) {
     NEED_DEVICE(ctx);
     const char *who = "blinky_ray_pyramid_bytes";
     if (!bytes) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": NULL bytes");
-    if (ctx->dev->width() <= 0) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": no lensmap installed (its plate size sizes the pyramid)");
-    if (!ctx->host.globe_valid()) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": no valid globe");
-    int size[blinky::kRayMaxLevels];
-    uint64_t off[blinky::kRayMaxLevels], b = 0;
-    const int ps = ctx->dev->platesize();
-    if (static_cast<uint64_t>(ps) * static_cast<uint64_t>(ps) * BLINKY_MAX_PLATES > 0x0FFFFFFFu ||
-        blinky::ray_pyramid_levels(ps, ctx->host.numplates(), size, off, &b) < 0)
-        return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": the installed lensmap's plate size " + std::to_string(ps) +
-                                                " is beyond what the ray warps take (6 * platesize^2 must fit the 28-bit texel index)");
-    *bytes = static_cast<size_t>(b);
-    return BLINKY_OK;
+    blinky::WarpRequest r(nullptr, 0, nullptr, 0, 0, nullptr);
+    r.entry = blinky::WarpEntry::PyramidBytes;
+    blinky::CheckedWarp c;
+    const int rc = blinky::check_warp(r, blinky::RayRequest(), ctx->dev->state(globe_state(ctx)), &c, &ctx->err);
+    if (rc == BLINKY_OK) *bytes = static_cast<size_t>(c.pyramid_bytes);
+    return rc;
 }
 
 int blinky_warp_device_rays_trilinear(blinky_ctx *ctx, const void *d_faces, size_t face_stride, const float *d_rays, size_t ray_stride,
@@ -816,17 +754,19 @@ int blinky_warp_device_rays_trilinear(blinky_ctx *ctx, const void *d_faces, size
     q.filter = blinky::RayFilter::Trilinear;
     q.scratch = d_scratch;
     q.scratch_bytes = scratch_bytes;
-    return warp_device_rays(ctx, r, q, rowbytes, x0, y0, keep_unmapped, true);
+    return warp_view(ctx, r, blinky::WarpEntry::RaysTrilinear, rowbytes, x0, y0, keep_unmapped, &q);
 }
 
 int blinky_warp_host(blinky_ctx *ctx, const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host,
                      size_t dst_frame_stride, int dst_rowbytes, int x0, int y0, int nframes, int keep_unmapped) {
     NEED_DEVICE(ctx);
-    if (!faces_host || !dst_host) return set_err(ctx, BLINKY_E_INVALID, "NULL buffer");
-    if (dst_rowbytes < ctx->host.width() + x0) return set_err(ctx, BLINKY_E_INVALID, "dst_rowbytes too small for the view rectangle");
-    return ctx->dev->warp_host(faces_host, face_stride, dst_host, dst_frame_stride, dst_rowbytes, x0, y0, nframes, keep_unmapped != 0)
-               ? BLINKY_OK
-               : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
+    blinky::WarpRequest r(faces_host, face_stride, dst_host, dst_frame_stride, nframes, nullptr);
+    r.entry = blinky::WarpEntry::Host;
+    r.rowbytes = dst_rowbytes;
+    r.x0 = x0;
+    r.y0 = y0;
+    r.keep_unmapped = keep_unmapped != 0;
+    return ctx->dev->warp_host(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int64_t blinky_upload_bytes_per_frame(blinky_ctx *ctx) {
@@ -885,8 +825,9 @@ int blinky_warp_device_rgba(blinky_ctx *ctx, const void *d_faces, size_t face_st
                             int nframes, void *stream) {
     NEED_DEVICE(ctx);
     blinky::WarpRequest r(d_faces, face_stride, d_out, out_stride, nframes, stream);
+    r.entry = blinky::WarpEntry::DenseRgba;
     r.rgba = true;
-    return warp_into_view(ctx, r, ctx->dev->width() * 4, 0, 0);
+    return ctx->dev->warp(r) ? BLINKY_OK : set_err(ctx, ctx->dev->last_error_code(), ctx->dev->last_error());
 }
 
 int64_t blinky_launch_count(blinky_ctx *ctx) { return ctx->dev ? ctx->dev->launches() : 0; }

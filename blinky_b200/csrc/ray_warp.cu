@@ -530,25 +530,25 @@ void with_factor(int k, F &&f) {
 RayPyramidParams pyramid_params(const RayWarpLaunch &L) {
     RayPyramidParams q;
     memset(&q, 0, sizeof q);
-    q.scratch = static_cast<uint8_t *>(L.scratch);
-    q.stride = L.pyramid_bytes;
-    q.lmax = L.lmax;
-    for (int l = 0; l <= L.lmax; ++l) {
-        q.size[l] = static_cast<uint32_t>(L.level_size[l]);
-        q.off[l] = L.level_off[l];
+    q.scratch = static_cast<uint8_t *>(L.q.scratch);
+    q.stride = L.c.pyramid_bytes;
+    q.lmax = L.c.lmax;
+    for (int l = 0; l <= L.c.lmax; ++l) {
+        q.size[l] = static_cast<uint32_t>(L.c.level_size[l]);
+        q.off[l] = L.c.level_off[l];
     }
     return q;
 }
 
 // the pyramid of every frame: one launch per level 1..lmax, the base instance of (rubix, tables) first
 void launch_pyramids(const RayWarpLaunch &L, const RayWarpParams &p, const RayPyramidParams &q, cudaStream_t st) {
-    for (int l = 1; l <= L.lmax; ++l) {
+    for (int l = 1; l <= L.c.lmax; ++l) {
         const uint32_t s = q.size[l];
-        const dim3 g((s * s + kRayThreads - 1) / kRayThreads, static_cast<unsigned>(L.globe.numplates), static_cast<unsigned>(L.nframes));
+        const dim3 g((s * s + kRayThreads - 1) / kRayThreads, static_cast<unsigned>(L.globe.numplates), static_cast<unsigned>(L.r.nframes));
         if (l > 1) ray_pyramid_reduce_kernel<<<g, kRayThreads, 0, st>>>(q, l);
         else
             with_flag(L.rubix, [&](auto rubix) {
-                with_flag(L.tables, [&](auto tables) { ray_pyramid_base_kernel<rubix, tables><<<g, kRayThreads, 0, st>>>(p, q, L.globe, L.layout); });
+                with_flag(L.tables(), [&](auto tables) { ray_pyramid_base_kernel<rubix, tables><<<g, kRayThreads, 0, st>>>(p, q, L.globe, L.c.layout); });
             });
     }
 }
@@ -557,43 +557,45 @@ void launch_pyramids(const RayWarpLaunch &L, const RayWarpParams &p, const RayPy
 
 bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
     RayWarpParams p;
-    p.rays = L.rays;
-    p.ray_floats = L.ray_stride / 4;
-    p.xforms = L.xforms;
-    p.xform_floats = L.xform_stride / 4;
-    p.faces = static_cast<const uint8_t *>(L.faces);
-    p.face_stride = L.face_stride;
+    p.rays = L.q.rays;
+    p.ray_floats = L.q.ray_stride / 4;
+    p.xforms = L.q.xforms;
+    p.xform_floats = L.q.xform_stride / 4;
+    p.faces = static_cast<const uint8_t *>(L.r.faces);
+    p.face_stride = L.r.face_stride;
     p.bg = L.bg;
     p.lut = L.lut;
     p.rgba = L.palette;
-    p.table_words = L.table_stride / 4;
-    p.out = static_cast<uint8_t *>(L.out);
-    p.out_stride = L.out_stride;
-    p.pitch = L.pitch;
+    p.table_words = L.r.table_stride / 4;
+    p.out = L.c.view;
+    p.out_stride = L.r.out_stride;
+    p.pitch = static_cast<uint32_t>(L.c.pitch);
     p.width = static_cast<uint32_t>(L.width);
     p.nitems = L.shape.nitems;
-    p.nframes = L.nframes;
+    p.nframes = L.r.nframes;
     p.frames_per_thread = L.shape.frames_per_thread;
     const dim3 grid(L.shape.grid_x, L.shape.grid_y);
-    cudaStream_t st = static_cast<cudaStream_t>(L.stream);
-    const bool trilinear = L.filter == RayFilter::Trilinear;
+    cudaStream_t st = static_cast<cudaStream_t>(L.r.stream);
+    const bool trilinear = L.q.filter == RayFilter::Trilinear;
+    const int factor = L.q.factor;
+    const bool keep = L.r.keep_unmapped, tables = L.tables();
     const RayPyramidParams q = pyramid_params(L);
     if (trilinear) launch_pyramids(L, p, q, st);
     // instances: per-frame tables exist only in RGBA (ray_warp_kernel: 24), supersampled K = 2..4 (24), bilinear
     // K = 1..4 (32), trilinear (8)
     with_flag(L.rubix, [&](auto rubix) {
-        with_flag(L.keep, [&](auto keep) {
-            with_flag(L.tables, [&](auto tables) {
+        with_flag(keep, [&](auto keep) {
+            with_flag(tables, [&](auto tables) {
                 if (trilinear) {
-                    ray_trilinear_kernel<rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.layout);
-                } else if (L.filter == RayFilter::Bilinear) {
-                    with_factor<1, 2, 3, 4>(L.factor, [&](auto k) { ray_bilinear_kernel<k, rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.layout); });
-                } else if (L.factor > 1) {
-                    with_factor<2, 3, 4>(L.factor, [&](auto k) { ray_supersample_kernel<k, rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.layout); });
+                    ray_trilinear_kernel<rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, q, L.globe, L.c.layout);
+                } else if (L.q.filter == RayFilter::Bilinear) {
+                    with_factor<1, 2, 3, 4>(factor, [&](auto k) { ray_bilinear_kernel<k, rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.c.layout); });
+                } else if (factor > 1) {
+                    with_factor<2, 3, 4>(factor, [&](auto k) { ray_supersample_kernel<k, rubix, keep, tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.c.layout); });
                 } else {
                     with_flag(L.shape.quads, [&](auto quad) {
-                        with_flag(L.rgba, [&](auto rgba) {
-                            ray_warp_kernel<quad, rubix, rgba, keep, rgba && tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.layout);
+                        with_flag(L.r.rgba, [&](auto rgba) {
+                            ray_warp_kernel<quad, rubix, rgba, keep, rgba && tables><<<grid, kRayThreads, 0, st>>>(p, L.globe, L.c.layout);
                         });
                     });
                 }
@@ -601,12 +603,12 @@ bool launch_ray_warp(const RayWarpLaunch &L, std::string *name, int *cuda_err) {
         });
     });
     char args[64], buf[192];
-    if (trilinear) snprintf(args, sizeof args, "rubix=%d,keep=%d,tables=%d", L.rubix, L.keep, L.tables);
-    else if (L.filter == RayFilter::Bilinear || L.factor > 1) snprintf(args, sizeof args, "k=%d,rubix=%d,keep=%d,tables=%d", L.factor, L.rubix, L.keep, L.tables);
-    else snprintf(args, sizeof args, "quad=%d,rubix=%d,rgba=%d,keep=%d,tables=%d", L.shape.quads, L.rubix, L.rgba, L.keep, L.tables);
-    const int n = snprintf(buf, sizeof buf, "%s<%s> grid=(%u,%u) block=%d frames/thread=%d", ray_warp_kernel_name(L.filter, L.factor), args, grid.x, grid.y,
+    if (trilinear) snprintf(args, sizeof args, "rubix=%d,keep=%d,tables=%d", L.rubix, keep, tables);
+    else if (L.q.filter == RayFilter::Bilinear || factor > 1) snprintf(args, sizeof args, "k=%d,rubix=%d,keep=%d,tables=%d", factor, L.rubix, keep, tables);
+    else snprintf(args, sizeof args, "quad=%d,rubix=%d,rgba=%d,keep=%d,tables=%d", L.shape.quads, L.rubix, L.r.rgba, keep, tables);
+    const int n = snprintf(buf, sizeof buf, "%s<%s> grid=(%u,%u) block=%d frames/thread=%d", ray_warp_kernel_name(L.q.filter, factor), args, grid.x, grid.y,
                            kRayThreads, L.shape.frames_per_thread);
-    if (trilinear) snprintf(buf + n, sizeof buf - n, " levels=%d", L.lmax);
+    if (trilinear) snprintf(buf + n, sizeof buf - n, " levels=%d", L.c.lmax);
     *name = buf;
     const cudaError_t e = cudaGetLastError();
     *cuda_err = static_cast<int>(e);

@@ -982,8 +982,8 @@ struct WarpDevice::Slot {
     uint8_t *h_faces = nullptr, *h_out = nullptr;  // pinned staging
     bool busy = false;
     // finalize info
-    uint8_t *dst = nullptr;          // the caller's frame
-    int dst_rowbytes = 0, x0 = 0, y0 = 0;
+    uint8_t *dst = nullptr;          // the view origin of the caller's frame
+    int dst_rowbytes = 0;
     bool keep_unmapped = false, direct = false;
 };
 
@@ -1154,69 +1154,26 @@ void WarpDevice::set_face_layout(int rowbytes, const int32_t *origins, int nplat
     layout_origins_.assign(origins && rowbytes > 0 ? origins : nullptr, origins && rowbytes > 0 ? origins + 2 * nplates : nullptr);
 }
 
-// The face layout against the current lensmap (the plate size and the plates it samples change with every build):
-// false, with err_code_ BLINKY_E_INVALID, when it does not fit; otherwise the kernels' view of it in *lay.
-bool WarpDevice::make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay, int globe_plates) {
-    err_code_ = BLINKY_E_INVALID;
-    const int n = static_cast<int>(layout_origins_.size() / 2);
-    const uint64_t rb = static_cast<uint64_t>(layout_rowbytes_), ps = static_cast<uint64_t>(cur_->platesize);
-    memset(lay, 0, sizeof *lay);
-    uint64_t rows = 0;
-    for (int pl = 0; pl < n; ++pl) {
-        const uint64_t x = static_cast<uint64_t>(layout_origins_[2 * pl]), y = static_cast<uint64_t>(layout_origins_[2 * pl + 1]);
-        if (x + ps > rb) {
-            err_ = "face layout: plate " + std::to_string(pl) + " at x = " + std::to_string(x) + " does not fit rowbytes " + std::to_string(rb) +
-                   " with plate size " + std::to_string(ps);
-            return false;
-        }
-        rows = std::max(rows, y + ps);
-        lay->plate_base[pl] = y * rb + x;
-        lay->org_x[pl] = static_cast<int32_t>(x);
-        lay->org_y[pl] = static_cast<int32_t>(y);
+WarpState WarpDevice::state(const GlobeState &globe) const {
+    WarpState s;
+    if (cur_) {
+        s.width = cur_->width;
+        s.height = cur_->height;
+        s.platesize = cur_->platesize;
+        s.display = cur_->display;
+        s.plate_rect = cur_->plate_rect;
     }
-    for (int pl = n; pl < kLayoutPlates; ++pl) {
-        const int *r = cur_->plate_rect[pl];
-        if (globe_plates >= 0 ? pl < globe_plates : cur_->display[pl] || (r[0] <= r[2] && r[1] <= r[3])) {
-            err_ = std::string(globe_plates >= 0 ? "face layout: the globe has plate " : "face layout: the lensmap samples plate ") + std::to_string(pl) +
-                   ", which has no origin (the layout has " + std::to_string(n) + ")";
-            return false;
-        }
-    }
-    if (nframes > 1 && static_cast<uint64_t>(face_stride) < rows * rb) {
-        err_ = "face layout: face_stride " + std::to_string(face_stride) + " is smaller than a frame's surface (" + std::to_string(rows) + " rows of " +
-               std::to_string(rb) + " bytes)";
-        return false;
-    }
-    lay->rowbytes = static_cast<uint32_t>(rb);
-    lay->ps = static_cast<uint32_t>(ps);
-    lay->ps2 = static_cast<uint32_t>(ps * ps);
-    lay->div_ps = make_fastdiv(lay->ps);
-    lay->div_ps2 = make_fastdiv(lay->ps2);
-    layout_rows_ = static_cast<uint32_t>(rows);
-    err_code_ = BLINKY_E_CUDA;
-    return true;
+    s.globe = globe;
+    s.layout_rowbytes = layout_rowbytes_;
+    s.layout_origins = layout_origins_.data();
+    s.layout_plates = static_cast<int>(layout_origins_.size() / 2);
+    return s;
 }
 
-bool WarpDevice::check_output(const WarpRequest &r, size_t *pitch) {
-    if (r.nframes > 65535) {
-        err_code_ = BLINKY_E_INVALID;
-        err_ = "warp: at most 65535 frames per launch";
-        return false;
-    }
-    const size_t opx = r.rgba ? 4 : 1;
-    if (r.rgba && (reinterpret_cast<uintptr_t>(r.out) % 4 != 0 || r.out_pitch % 4 != 0 || (r.nframes > 1 && r.out_stride % 4 != 0))) {
-        err_code_ = BLINKY_E_INVALID;
-        err_ = "warp (RGBA): the output buffer, the row pitch and the frame stride must be 4-byte aligned";
-        return false;
-    }
-    const Generation &g = *cur_;
-    *pitch = r.out_pitch ? r.out_pitch : static_cast<size_t>(g.width) * opx;
-    if (*pitch < static_cast<size_t>(g.width) * opx || *pitch > (size_t{1} << 26)) {   // (the kernels step 32 rows in 32-bit offsets)
-        err_code_ = BLINKY_E_INVALID;
-        err_ = "warp: the output row pitch must hold a row of the view and be at most 64 MB";
-        return false;
-    }
-    return true;
+bool WarpDevice::check(const WarpRequest &r, const RayRequest &q, const GlobeState &globe, CheckedWarp *c) {
+    const int rc = check_warp(r, q, state(globe), c, &err_);
+    err_code_ = rc != BLINKY_OK ? rc : BLINKY_E_CUDA;
+    return rc == BLINKY_OK;
 }
 
 bool WarpDevice::capture_info(void *stream, bool *capturing, unsigned long long *id) {
@@ -1238,125 +1195,43 @@ void WarpDevice::remember_capture(void *stream, unsigned long long id) {
 }
 
 bool WarpDevice::warp(const WarpRequest &r) {
-    err_code_ = BLINKY_E_CUDA;
-    if (!cur_) {
-        err_ = "warp: no lensmap on the device (call blinky_build_lensmap)";
-        return false;
-    }
-    if (r.nframes <= 0) return true;
-    size_t pitch = 0;
-    if (!check_output(r, &pitch)) return false;
+    CheckedWarp c;
+    if (!check(r, RayRequest(), GlobeState(), &c)) return false;
+    if (!c.launch) return true;
     const Generation &g = *cur_;
-    const bool use_layout = layout_rowbytes_ > 0 && !r.dense_faces;
-    FaceLayoutParams lay = {};   // (dense: the kernels' last argument, never read)
-    if (use_layout && !make_layout(r.face_stride, r.nframes, &lay)) return false;
-    const KernelVariant v = {rubix_, r.rgba, r.keep_unmapped, r.rgba && r.tables && r.table_stride != 0, use_layout};
-    const WarpKernel k = choose_kernel(r, pitch, use_layout ? &lay : nullptr, g.width, g.height, g.have_plan, g.plan_has_box,
+    const KernelVariant v = {rubix_, r.rgba, r.keep_unmapped, r.rgba && r.tables && r.table_stride != 0, c.use_layout};
+    const WarpKernel k = choose_kernel(r, c.pitch, c.use_layout ? &c.layout : nullptr, g.width, g.height, g.have_plan, g.plan_has_box,
                                        variant_ == BLINKY_KERNEL_GATHER);
     bool capturing = false;
     unsigned long long cap_id = 0;
     if (!capture_info(r.stream, &capturing, &cap_id)) return false;
-    const bool ok = k == WarpKernel::Ring ? launch_ring(r, static_cast<uint32_t>(pitch), v, lay, capturing)
-                                          : launch_flat(r, static_cast<uint32_t>(pitch), v, lay, k);
+    const bool ok = k == WarpKernel::Ring ? launch_ring(r, c, v, capturing) : launch_flat(r, c, v, k);
     if (capturing) remember_capture(r.stream, cap_id);
     return ok;
 }
 
-bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe) {
-    err_code_ = BLINKY_E_CUDA;
-    if (!cur_) {
-        err_code_ = BLINKY_E_STATE;
-        err_ = "warp_rays: no lensmap on the device (its view size and background are the warp's)";
-        return false;
-    }
-    if (r.nframes <= 0) return true;
-    // (the kernel packs a texel's px and py into 13 bits each: set_raymap's own limit, 6 * ps^2 < 2^28, keeps ps <= 6688)
-    if (static_cast<uint64_t>(cur_->platesize) * static_cast<uint64_t>(cur_->platesize) * kLayoutPlates > 0x0FFFFFFFu) {
-        err_code_ = BLINKY_E_STATE;
-        err_ = "warp_rays: the installed lensmap's plate size " + std::to_string(cur_->platesize) +
-               " is beyond what a ray map takes (6 * platesize^2 must fit the 28-bit texel index)";
-        return false;
-    }
-    // (the supersampled, bilinear and trilinear kernels index the field's pixels in 31 bits)
-    const uint64_t field_pixels = static_cast<uint64_t>(q.factor) * q.factor * static_cast<uint64_t>(cur_->width) * static_cast<uint64_t>(cur_->height);
-    if ((q.factor > 1 || q.filter != RayFilter::Nearest) && field_pixels > 0x7FFFFFFFu) {
-        err_code_ = BLINKY_E_INVALID;
-        err_ = "warp_rays: a field of factor^2 * width * height = " + std::to_string(field_pixels) + " pixels is beyond the kernel's 31-bit pixel index";
-        return false;
-    }
-    // (the trilinear warp's pyramids: every plate of the globe, at the installed plate size)
-    int lsize[kRayMaxLevels] = {};
-    uint64_t loff[kRayMaxLevels] = {}, pyramid = 0;
-    int lmax = 0;
-    if (q.filter == RayFilter::Trilinear) {
-        lmax = ray_pyramid_levels(cur_->platesize, globe.numplates, lsize, loff, &pyramid);
-        err_code_ = BLINKY_E_INVALID;
-        if (pyramid > 0 && !q.scratch) {
-            err_ = "warp_rays: NULL scratch (the frames' pyramids need " + std::to_string(pyramid) + " bytes each)";
-            return false;
-        }
-        if (reinterpret_cast<uintptr_t>(q.scratch) % 16 != 0) {
-            err_ = "warp_rays: the scratch must be 16-byte aligned";
-            return false;
-        }
-        if (static_cast<uint64_t>(q.scratch_bytes) < static_cast<uint64_t>(r.nframes) * pyramid) {
-            err_ = "warp_rays: scratch_bytes " + std::to_string(q.scratch_bytes) + " is below nframes * " + std::to_string(pyramid) +
-                   " (blinky_ray_pyramid_bytes)";
-            return false;
-        }
-        err_code_ = BLINKY_E_CUDA;
-    }
-    size_t pitch = 0;
-    if (!check_output(r, &pitch)) return false;
+bool WarpDevice::warp_rays(const WarpRequest &r, const RayRequest &q, const GlobeState &globe, const LensBuildParams &params) {
+    CheckedWarp c;
+    if (!check(r, q, globe, &c)) return false;
+    if (!c.launch) return true;
     const Generation &g = *cur_;
-    FaceLayoutParams lay = {};
-    if (layout_rowbytes_ > 0) {
-        if (!make_layout(r.face_stride, r.nframes, &lay, globe.numplates)) return false;
-    } else {   // dense [plate][ps][ps] frames: the layout with rowbytes = ps
-        const uint64_t ps = static_cast<uint64_t>(g.platesize);
-        for (int i = 0; i < kLayoutPlates; ++i) lay.plate_base[i] = static_cast<uint64_t>(i) * ps * ps;
-        lay.rowbytes = static_cast<uint32_t>(ps);
-    }
     bool capturing = false;
     unsigned long long cap_id = 0;
     if (!capture_info(r.stream, &capturing, &cap_id)) return false;
-    RayWarpLaunch L;
-    L.filter = q.filter;
-    L.factor = q.factor;
-    L.scratch = q.scratch;
-    L.pyramid_bytes = pyramid;
-    L.lmax = lmax;
-    for (int l = 0; l < kRayMaxLevels; ++l) {
-        L.level_size[l] = lsize[l];
-        L.level_off[l] = loff[l];
-    }
-    L.rays = q.rays;
-    L.ray_stride = q.ray_stride;
-    L.xforms = q.xforms;
-    L.xform_stride = q.xform_stride;
-    L.faces = r.faces;
-    L.face_stride = r.face_stride;
-    L.bg = g.bg->as<const uint8_t>();
-    L.lut = d_lut_.as<const uint8_t>();
-    L.palette = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
-    L.table_stride = r.table_stride;
-    L.out = r.out;
-    L.out_stride = r.out_stride;
-    L.pitch = static_cast<uint32_t>(pitch);
-    L.width = g.width;
-    L.height = g.height;
-    L.nframes = r.nframes;
-    L.shape = ray_warp_shape(r, q, pitch, g.width, g.height, static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_));
-    L.rubix = rubix_;
-    L.rgba = r.rgba;
-    L.keep = r.keep_unmapped;
-    L.tables = r.rgba && r.tables && r.table_stride != 0;
-    L.globe = globe;
-    L.layout = lay;
-    L.stream = r.stream;
+    const RayWarpLaunch L = {r,
+                             q,
+                             c,
+                             g.bg->as<const uint8_t>(),
+                             d_lut_.as<const uint8_t>(),
+                             r.tables ? r.tables : d_rgba_.as<const uint32_t>(),
+                             g.width,
+                             g.height,
+                             ray_warp_shape(r, q, c.pitch, g.width, g.height, static_cast<uint32_t>(sm_count_) * static_cast<uint32_t>(threads_per_sm_)),
+                             rubix_,
+                             params};
     int e = 0;
     const bool ok = launch_ray_warp(L, &last_kernel_, &e);
-    launches_ += 1 + lmax;
+    launches_ += 1 + c.lmax;
     if (capturing) remember_capture(r.stream, cap_id);
     return ok ? true : fail(ray_warp_kernel_name(q.filter, q.factor), e);
 }
@@ -1451,7 +1326,7 @@ WarpDevice::TmapSet *WarpDevice::get_tmaps(const void *d_faces, size_t face_stri
 // warps only spread the faces' L2 footprint; the registers left over go to the gather CTAs.
 constexpr int kRingWarpsDefault = 12;
 
-bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, bool capturing) {
+bool WarpDevice::launch_ring(const WarpRequest &r, const CheckedWarp &c, const KernelVariant &v, bool capturing) {
     cudaStream_t st = static_cast<cudaStream_t>(r.stream);
     const Generation &g = *cur_;
     RingParams p;
@@ -1460,7 +1335,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
     static const RingTmaps kNoTmaps = {};
     const RingTmaps *tm = &kNoTmaps;
     if (g.plan_has_box) {
-        TmapSet *t = get_tmaps(r.faces, r.face_stride, r.nframes, lay.rowbytes, v.layout ? layout_rows_ : 0u);
+        TmapSet *t = get_tmaps(r.faces, r.face_stride, r.nframes, c.layout.rowbytes, v.layout ? c.layout_rows : 0u);
         if (!t) return false;
         tm = &t->table;
     }
@@ -1470,9 +1345,9 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
     p.lut = d_lut_.as<const uint8_t>();
     p.rgba = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
     p.table_words = static_cast<uint32_t>(r.table_stride / 4);
-    p.out = r.out;
+    p.out = c.view;
     p.out_stride = r.out_stride;
-    p.out_pitch = pitch / (v.rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
+    p.out_pitch = static_cast<uint32_t>(c.pitch) / (v.rgba ? 4u : 1u);   // (whole pixels: an RGBA pitch is a multiple of 4 bytes)
     p.nbox = g.nbox_tiles;
     p.ngather = g.ngather_tiles;
     p.ntiles = g.ntiles;
@@ -1561,7 +1436,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
         dim3 g2(g.ngather_tiles, static_cast<unsigned>((r.nframes + kGatherFramesPerCta - 1) / kGatherFramesPerCta));
         with_variant(vi, [&](auto vt) {
             using V = decltype(vt);
-            warp_tile_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<g2, kThreads, 0, st>>>(p, g.nbox_tiles, lay);
+            warp_tile_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<g2, kThreads, 0, st>>>(p, g.nbox_tiles, c.layout);
         });
         ++launches_;
         snprintf(buf, sizeof buf, "warp_tile_gather_kernel<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", v.rubix, v.rgba, v.tags(), g2.x, g2.y, kThreads);
@@ -1574,7 +1449,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
         const uint32_t extra = merged_gather ? gather_items(g.ngather_tiles, r.nframes) : 0u;
         with_variant(vi, [&](auto vt) {
             using V = decltype(vt);
-            warp_ring_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid + extra, 32, smem, st>>>(p, *tm, lay);
+            warp_ring_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid + extra, 32, smem, st>>>(p, *tm, c.layout);
         });
         ++launches_;
         nbuf = static_cast<int>(strlen(buf));
@@ -1589,7 +1464,7 @@ bool WarpDevice::launch_ring(const WarpRequest &r, uint32_t pitch, const KernelV
     return true;
 }
 
-bool WarpDevice::launch_flat(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, WarpKernel k) {
+bool WarpDevice::launch_flat(const WarpRequest &r, const CheckedWarp &c, const KernelVariant &v, WarpKernel k) {
     // NULL is CUDA's default stream (what torch.cuda.current_stream() hands out unless the caller made its own)
     cudaStream_t st = static_cast<cudaStream_t>(r.stream);
     const Generation &g = *cur_;
@@ -1601,19 +1476,19 @@ bool WarpDevice::launch_flat(const WarpRequest &r, uint32_t pitch, const KernelV
     p.lut = d_lut_.as<const uint8_t>();
     p.rgba = r.tables ? r.tables : d_rgba_.as<const uint32_t>();
     p.table_words = static_cast<uint32_t>(r.table_stride / 4);
-    p.out = r.out;
+    p.out = c.view;
     p.out_stride = r.out_stride;
     p.nquads = static_cast<uint32_t>((g.npix + 3) / 4);
     p.npix = static_cast<uint32_t>(g.npix);
     p.width = static_cast<uint32_t>(g.width);
-    p.out_pitch = pitch;
-    p.pitched = pitch != static_cast<size_t>(g.width) * (v.rgba ? 4 : 1);
+    p.out_pitch = static_cast<uint32_t>(c.pitch);
+    p.pitched = c.pitch != static_cast<size_t>(g.width) * (v.rgba ? 4 : 1);
     const bool vector = k == WarpKernel::Vector;
     const dim3 grid(static_cast<unsigned>(vector ? g.npix_pad / kPixelsPerBlock : (g.npix + kThreads - 1) / kThreads), static_cast<unsigned>(r.nframes));
     with_variant(v.index(), [&](auto vt) {
         using V = decltype(vt);
-        if (vector) warp_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, lay);
-        else warp_scalar_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, lay);
+        if (vector) warp_gather_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, c.layout);
+        else warp_scalar_kernel<V::rubix, V::rgba, V::keep, V::tables, V::layout><<<grid, kThreads, 0, st>>>(p, c.layout);
     });
     char buf[160];
     snprintf(buf, sizeof buf, "%s<rubix=%d,rgba=%d%s> grid=(%u,%u) block=%d", vector ? "warp_gather_kernel" : "warp_scalar_kernel", v.rubix, v.rgba,
@@ -1650,7 +1525,7 @@ void WarpDevice::finalize_slot(Slot &s) {
     if (s.direct) return;  // the copy engine already wrote the caller's buffer
     const Generation &g = *cur_;
     const int W = g.width, H = g.height;
-    uint8_t *dst = s.dst + static_cast<size_t>(s.y0) * s.dst_rowbytes + s.x0;
+    uint8_t *dst = s.dst;
     if (s.keep_unmapped) {
         // only mapped pixels are written, like `if (*lmap)` in render_lensmap (:2413)
         for (int y = 0; y < H; ++y) {
@@ -1678,18 +1553,18 @@ static bool is_pinned(const void *p) {
     return a.type == cudaMemoryTypeHost;
 }
 
-bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
-                           int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped) {
-    err_code_ = BLINKY_E_CUDA;
-    if (!cur_) {
-        err_ = "warp_host: no lensmap on the device (call blinky_build_lensmap)";
-        return false;
-    }
+bool WarpDevice::warp_host(const WarpRequest &r) {
+    CheckedWarp c;
+    if (!check(r, RayRequest(), GlobeState(), &c)) return false;
     const Generation &g = *cur_;
+    const uint8_t *faces_host = static_cast<const uint8_t *>(r.faces);
+    const uint8_t *dst_host = static_cast<const uint8_t *>(r.out);
+    const size_t face_stride = r.face_stride;
+    const int dst_rowbytes = r.rowbytes, nframes = r.nframes;
+    const bool keep_unmapped = r.keep_unmapped;
     // with a face layout the plates' rectangles are read out of each frame's surface; the device copy stays dense
-    FaceLayoutParams lay;
-    const bool layout = layout_rowbytes_ > 0;
-    if (layout && !make_layout(face_stride, nframes, &lay)) return false;
+    const FaceLayoutParams &lay = c.layout;
+    const bool layout = c.use_layout;
     const size_t ps = static_cast<size_t>(g.platesize);
     const size_t src_pitch = layout ? lay.rowbytes : ps;
     CK(cudaSetDevice(device_));
@@ -1757,16 +1632,14 @@ bool WarpDevice::warp_host(const uint8_t *faces_host, size_t face_stride, uint8_
             if (e != cudaSuccess) ok = fail("cudaMemcpy2DAsync(H2D faces)", e);
         }
         if (!ok) break;
-        s.dst = dst_host + static_cast<size_t>(f) * dst_frame_stride;
-        WarpRequest r(s.d_faces.get(), slot_face_bytes_, s.d_out.get(), slot_out_bytes_, 1, s.stream);
-        r.dense_faces = true;   // the device copy is dense whatever the face layout
-        if (!warp(r)) { ok = false; break; }
+        s.dst = c.view + static_cast<size_t>(f) * r.out_stride;
+        WarpRequest frame_r(s.d_faces.get(), slot_face_bytes_, s.d_out.get(), slot_out_bytes_, 1, s.stream);
+        frame_r.dense_faces = true;   // the device copy is dense whatever the face layout
+        if (!warp(frame_r)) { ok = false; break; }
         s.dst_rowbytes = dst_rowbytes;
-        s.x0 = x0;
-        s.y0 = y0;
         s.keep_unmapped = keep_unmapped;
         s.direct = direct;
-        uint8_t *to = s.dst + static_cast<size_t>(y0) * dst_rowbytes + x0;
+        uint8_t *to = s.dst;
         cudaError_t e = !direct              ? cudaMemcpyAsync(s.h_out, s.d_out.get(), frame, cudaMemcpyDeviceToHost, s.stream)
                         : dst_rowbytes == W ? cudaMemcpyAsync(to, s.d_out.get(), frame, cudaMemcpyDeviceToHost, s.stream)
                                             : cudaMemcpy2DAsync(to, static_cast<size_t>(dst_rowbytes), s.d_out.get(), static_cast<size_t>(W),

@@ -14,13 +14,12 @@
 
 #include "device_buffer.h"
 #include "face_layout.h"
-#include "ray_warp.h"   // RayFilter
+#include "ray_texel.h"   // kRayMaxLevels
 
 namespace blinky {
 
 struct DevicePlan;     // tile_plan_device.h
 struct KernelVariant;  // launch_plan.h
-struct LensBuildParams;  // lens_device.h
 enum class WarpKernel;
 
 // What WarpDevice::install keeps of a lensmap beside its device buffers (DevicePlan).
@@ -35,6 +34,17 @@ struct LensmapUpload {
     size_t nspans = 0;
 };
 
+// The entry point a warp request comes from (warp_entry_name): it decides which checks the request gets, in which
+// order, and how its refusals read (check_warp, launch_plan.h).
+enum class WarpEntry {
+    Internal,                                 // blinky_warp_host's frames and the sharded batches
+    Dense, DenseRgba,                         // blinky_warp_device[_rgba]: the view is the whole of out
+    View, ViewRgba, ViewRgbaTables,           // blinky_warp_device_view*: the view rectangle at (x0, y0) of out
+    Rays, RaysRgba, RaysSupersampled, RaysBilinear, RaysTrilinear,   // blinky_warp_device_rays*: likewise
+    PyramidBytes,                             // blinky_ray_pyramid_bytes: the ray warps' checks of the state alone
+    Host,                                     // blinky_warp_host: the view rectangle at (x0, y0) of a host buffer
+};
+
 // One device-resident batch (WarpDevice::warp), asynchronous on `stream` (nullptr = CUDA's default stream).  May be
 // captured into a CUDA graph: see WarpDevice::release_captures.
 struct WarpRequest {
@@ -42,11 +52,13 @@ struct WarpRequest {
         : faces(faces), face_stride(face_stride), out(out), out_stride(out_stride), nframes(nframes), stream(stream) {}
     const void *faces;                 // frame 0's faces, in the face layout (WarpDevice::set_face_layout)
     size_t face_stride;                // bytes between frames
-    void *out;                         // view origin of frame 0
+    void *out;                         // frame 0's screen, whose view rectangle at (x0, y0) the warp writes
     size_t out_stride;                 // bytes between frames
-    size_t out_pitch = 0;              // bytes between rows (0: dense, W * bytes per pixel)
     int nframes;
     void *stream;                      // cudaStream_t
+    WarpEntry entry = WarpEntry::Internal;
+    int rowbytes = 0, x0 = 0, y0 = 0;  // the screen's bytes between rows and the view's origin in it (view entry points
+                                       // and Host; otherwise 0: the view is the whole screen, rows W * bytes per pixel apart)
     bool rgba = false;
     bool keep_unmapped = false;        // only mapped pixels are written, the others keep what the caller's buffer holds
     // RGBA: frame f is expanded through the 256-entry device table at tables + f * table_stride bytes (table_stride 0:
@@ -55,18 +67,58 @@ struct WarpRequest {
     const uint32_t *tables = nullptr;
     size_t table_stride = 0;
     bool dense_faces = false;          // the faces are dense [plate][ps][ps] frames whatever the face layout
+
+    // frame 0's view origin, in screens whose rows are `pitch` bytes apart
+    uint8_t *view(size_t pitch) const { return static_cast<uint8_t *>(out) + static_cast<size_t>(y0) * pitch + static_cast<size_t>(x0) * (rgba ? 4 : 1); }
 };
+
+// How each sample of a ray warp takes its colour: the nearest texel (ray_warp_kernel at factor 1,
+// ray_supersample_kernel at 2-4), four texels blended (ray_bilinear_kernel, factor 1-4), or two mip levels' bilinear
+// colours blended (the pyramid launches, then ray_trilinear_kernel, factor 1).  Every filter but Nearest at factor 1
+// writes RGBA.
+enum class RayFilter { Nearest, Bilinear, Trilinear };
 
 // The ray field and matrices of a warp from rays (WarpDevice::warp_rays), device memory read when the launch runs.
 struct RayRequest {
-    const float *rays;          // frame 0's field, float32[height][width][3] as blinky_set_raymap reads it
-    size_t ray_stride;          // bytes between frames (0: one field for every frame)
-    const float *xforms;        // frame 0's 3x3 matrix, row-major (nullptr: the rays as they are)
-    size_t xform_stride;        // bytes between frames (0: one matrix for every frame)
+    const float *rays = nullptr;   // frame 0's field, float32[height][width][3] as blinky_set_raymap reads it
+    size_t ray_stride = 0;         // bytes between frames (0: one field for every frame)
+    const float *xforms = nullptr; // frame 0's 3x3 matrix, row-major (nullptr: the rays as they are)
+    size_t xform_stride = 0;       // bytes between frames (0: one matrix for every frame)
     int factor = 1;             // 2-4: a [factor * height][factor * width] field, factor^2 samples averaged per RGBA pixel
     RayFilter filter = RayFilter::Nearest;   // Bilinear: factor 1-4; Trilinear: factor 1, the two mip levels around the footprint
     void *scratch = nullptr;    // trilinear: the frames' pyramids, frame f at scratch + f * B (16-byte aligned)
     size_t scratch_bytes = 0;   // trilinear: at least nframes * B
+};
+
+// What the checks of a warp read besides the call (check_warp): the installed lensmap, the globe and the face layout.
+struct GlobeState {
+    bool valid = false;
+    bool plate_script = false;         // the globe picks its plates with a globe_plate script
+    int plates = 0;
+};
+struct WarpState {
+    int width = 0, height = 0, platesize = 0;   // the installed view (0 before the first install)
+    const int *display = nullptr;               // [6]: with plate_rect, the plates the lensmap samples
+    const int (*plate_rect)[4] = nullptr;       // [6] texel rectangles (x0, y0, x1, y1)
+    GlobeState globe;
+    int layout_rowbytes = 0;                    // face layout: 0 = dense
+    const int32_t *layout_origins = nullptr;    // (x, y) per plate
+    int layout_plates = 0;
+};
+
+// What check_warp derives for an accepted call.
+struct CheckedWarp {
+    bool launch = false;         // false: nframes <= 0, nothing to do
+    uint8_t *view = nullptr;     // frame 0's view origin, WarpRequest::view(pitch)
+    size_t pitch = 0;            // bytes between the view's rows
+    bool use_layout = false;     // the faces are read through `layout` (ray warps: always, dense faces included)
+    FaceLayoutParams layout = {};
+    uint32_t layout_rows = 0;    // rows of a frame's surface in the face layout
+    // trilinear (and blinky_ray_pyramid_bytes): the frames' pyramids, ray_pyramid_levels
+    int lmax = 0;
+    int level_size[kRayMaxLevels] = {};
+    uint64_t level_off[kRayMaxLevels] = {};
+    uint64_t pyramid_bytes = 0;
 };
 
 class WarpDevice {
@@ -103,22 +155,24 @@ public:
     size_t plan_tiles() const;
     size_t plan_entry_bytes() const;
 
+    // what the checks of a warp read of this object, with the globe `globe`
+    WarpState state(const GlobeState &globe = {}) const;
+    // r, checked (check_warp) and launched: nothing is launched when it is refused
     bool warp(const WarpRequest &r);
     // r (view, rgba, keep_unmapped, tables) with each pixel's texel computed from its ray in q, turned, through the
-    // globe `globe` (FisheyeHost::device_params at the resident view's size, no globe_plate script): the resident
+    // globe `params` (FisheyeHost::device_params at the resident view's size) described by `globe`: the resident
     // lensmap gives only the view's size and background.  Every plate of the globe must have an origin in the face
     // layout.  Capturable like warp().  q.factor > 1: the supersampled RGBA warp (ray_supersample_kernel);
     // Bilinear: the bilinear RGBA warp at any factor (ray_bilinear_kernel); Trilinear: the frames' pyramids in
     // q.scratch, then the trilinear RGBA warp (ray_trilinear_kernel), lmax + 1 launches.
-    bool warp_rays(const WarpRequest &r, const RayRequest &q, const LensBuildParams &globe);
+    bool warp_rays(const WarpRequest &r, const RayRequest &q, const GlobeState &globe, const LensBuildParams &params);
     // The caller will not run again any graph that captured a warp of this object: synchronises the device, lets go
     // of the generations held for such graphs and returns every capture counter slot to the pool.
     bool release_captures();
     // BLINKY_E_* code of the last failure (BLINKY_E_CUDA unless the call was refused for another reason)
     int last_error_code() const { return err_code_; }
-    // end to end from host buffers (synchronous)
-    bool warp_host(const uint8_t *faces_host, size_t face_stride, uint8_t *dst_host, size_t dst_frame_stride,
-                   int dst_rowbytes, int x0, int y0, int nframes, bool keep_unmapped);
+    // end to end from host buffers (synchronous): r.faces and r.out in host memory, 8-bit, entry Host
+    bool warp_host(const WarpRequest &r);
 
     bool alloc_device(size_t bytes, void **out);
     bool free_device(void *p);
@@ -137,11 +191,8 @@ private:
     struct Slot;
     bool ensure_slots();
     bool fail(const char *what, int cuda_err);
-    // globe_plates >= 0: the plates 0..globe_plates-1 need an origin (a warp from rays may sample any of them), instead
-    // of the plates the lensmap samples
-    bool make_layout(size_t face_stride, int nframes, FaceLayoutParams *lay, int globe_plates = -1);
-    // the checks every warp makes of its output; *pitch: the bytes between output rows
-    bool check_output(const WarpRequest &r, size_t *pitch);
+    // check_warp of r (and q) on state(globe): false, with the refusal in err_code_ / err_, or the derived values in *c
+    bool check(const WarpRequest &r, const RayRequest &q, const GlobeState &globe, CheckedWarp *c);
     // whether r.stream is capturing (and which capture); remember_capture: a warp was captured into it
     bool capture_info(void *stream, bool *capturing, unsigned long long *id);
     void remember_capture(void *stream, unsigned long long id);
@@ -165,7 +216,6 @@ private:
     int variant_ = 0;
     int layout_rowbytes_ = 0;              // face layout: 0 = dense
     std::vector<int32_t> layout_origins_;  // (x, y) per plate
-    uint32_t layout_rows_ = 0;             // rows of a frame's surface (set by make_layout)
 
     // tiled layout (ring kernel)
     struct TmapSet;
@@ -186,10 +236,9 @@ private:
     int ring_ctas_per_sm_[32] = {};      // per ring kernel instance (KernelVariant::index)
     size_t ring_smem_[32] = {};
     TmapSet *get_tmaps(const void *d_faces, size_t face_stride, int nframes, uint32_t rowbytes, uint32_t rows);
-    // what warp() derived from the request: pitch, the output's bytes between rows; lay, the face layout when v.layout
-    // (zero otherwise)
-    bool launch_ring(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, bool capturing);
-    bool launch_flat(const WarpRequest &r, uint32_t pitch, const KernelVariant &v, const FaceLayoutParams &lay, WarpKernel k);
+    // r as check_warp accepted it, with what it derived in c
+    bool launch_ring(const WarpRequest &r, const CheckedWarp &c, const KernelVariant &v, bool capturing);
+    bool launch_flat(const WarpRequest &r, const CheckedWarp &c, const KernelVariant &v, WarpKernel k);
 
     // CUDA graph capture.  A captured ring launch gets a work counter of its own out of a pool allocated (zeroed) with
     // the object, because its graph may be replayed on any stream, beside eager launches and other graphs; slots are

@@ -288,3 +288,30 @@ def test_view_argument_errors_launch_nothing(bb, fe, torch_mod):
     fe.warp_view(d_faces, base, **ok4)
     torch.cuda.synchronize()
     assert fe.launch_count > before
+
+
+def test_dense_null_buffers_and_negative_host_origin_launch_nothing(bb, fe, torch_mod):
+    """the dense entry points refuse a NULL buffer as the view entry points do, and blinky_warp_host a negative view
+    origin: nothing is launched and nothing is written"""
+    torch = torch_mod
+    W, H, PS = 128, 96, 48
+    setup(fe, "cube", "panini", W, H, PS)
+    lib = bb.load_library()
+    faces = np.stack([bb.synthetic_faces(6, PS, i) for i in range(2)])
+    d_faces = torch.from_numpy(faces).cuda()
+    out = torch.full((2 * W * H * 4,), 0xA5, dtype=torch.uint8, device="cuda")
+    before = fe.launch_count
+    for fn, name, bpp in ((lib.blinky_warp_device, "blinky_warp_device", 1), (lib.blinky_warp_device_rgba, "blinky_warp_device_rgba", 4)):
+        for f, o in ((None, out.data_ptr()), (d_faces.data_ptr(), None)):
+            assert fn(fe._ctx, f, faces[0].nbytes, o, bpp * W * H, 2, None) == bb.E_INVALID
+            assert lib.blinky_last_error(fe._ctx).decode() == f"{name}: NULL buffer"
+    torch.cuda.synchronize()
+    assert bool((out == 0xA5).all())
+    rowbytes, guard = W + 16, 4096
+    dst = np.full(guard + 2 * (H + 8) * rowbytes + guard, 0xA5, np.uint8)
+    for x0, y0 in ((-1, 0), (0, -1), (-1, -1)):
+        rc = lib.blinky_warp_host(fe._ctx, faces.ctypes.data, faces[0].nbytes, dst.ctypes.data + guard, (H + 8) * rowbytes, rowbytes, x0, y0, 2, 0)
+        assert rc == bb.E_INVALID, (x0, y0)
+        assert lib.blinky_last_error(fe._ctx).decode() == "the view origin (x0, y0) must not be negative"
+    assert (dst == 0xA5).all()
+    assert fe.launch_count == before
