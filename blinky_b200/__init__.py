@@ -65,6 +65,8 @@ _SIGNATURES = [
     ("blinky_set_raymap_device", c_int, [_CTX, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_get_raymap", c_int, [_CTX, c_int, c_int, c_void_p]),
     ("blinky_get_raymap_device", c_int, [_CTX, c_int, c_int, c_void_p, c_void_p]),
+    ("blinky_get_raymap_forward", c_int, [_CTX, c_int, c_int, c_int, c_void_p]),
+    ("blinky_get_raymap_forward_device", c_int, [_CTX, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("blinky_build_info", c_char_p, [_CTX]),
     ("blinky_plan_digest", ctypes.c_uint64, [_CTX, c_int]),
     ("blinky_get_tile_plan", c_int, [_CTX, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
@@ -317,21 +319,30 @@ class Fisheye:
             raise ValueError(f"set_raymap: expected a contiguous [H, W, 3] float32 tensor, got {rays.dtype} {tuple(rays.shape)}")
         self._check(self._lib.blinky_set_raymap_device(self._ctx, rays.shape[1], rays.shape[0], platesize, rays.data_ptr(), stream))
 
-    def raymap(self, width: int, height: int, out=None, stream: int | None = None):
+    def raymap(self, width: int, height: int, out=None, stream: int | None = None, *, forward: bool = False, platesize: int = 0):
         """The view rays a width x height build of the current lens evaluates, as set_raymap reads them: [height,
         width, 3] float32, lens_inverse at ((lx - width//2) * scale, -(ly - height//2) * scale) narrowed to float and not
         normalised, the zero vector for nil.  No `out`: a new numpy array (blinky_get_raymap, on the worker threads).
         `out`, a contiguous CUDA float32 [height, width, 3] tensor: filled on `stream` after the work already there
-        (blinky_get_raymap_device, evaluated on the GPU) and returned once complete."""
+        (blinky_get_raymap_device, evaluated on the GPU) and returned once complete.
+        forward=True: the rays of the forward build at width x height on plates of `platesize` texels (0: min(width,
+        height)), interpolated through each pixel's winning quad and normalised (blinky_get_raymap_forward[_device],
+        DESIGN §3h), for any lens with a lens_forward function; platesize is ignored without it."""
         if out is None:
             rays = np.empty((height, width, 3), np.float32)
-            self._check(self._lib.blinky_get_raymap(self._ctx, width, height, rays.ctypes.data))
+            if forward:
+                self._check(self._lib.blinky_get_raymap_forward(self._ctx, width, height, platesize, rays.ctypes.data))
+            else:
+                self._check(self._lib.blinky_get_raymap(self._ctx, width, height, rays.ctypes.data))
             return rays
         if not (hasattr(out, "is_cuda") and out.is_cuda):
             raise TypeError("raymap: out must be a CUDA tensor")
         if tuple(out.shape) != (height, width, 3) or str(out.dtype) != "torch.float32" or not out.is_contiguous():
             raise ValueError(f"raymap: expected a contiguous [{height}, {width}, 3] float32 tensor, got {out.dtype} {tuple(out.shape)}")
-        self._check(self._lib.blinky_get_raymap_device(self._ctx, width, height, out.data_ptr(), stream))
+        if forward:
+            self._check(self._lib.blinky_get_raymap_forward_device(self._ctx, width, height, platesize, out.data_ptr(), stream))
+        else:
+            self._check(self._lib.blinky_get_raymap_device(self._ctx, width, height, out.data_ptr(), stream))
         return out
 
     @property

@@ -326,6 +326,29 @@ int get_raymap_host(blinky_ctx *ctx, const char *who, int width, int height, dou
     return BLINKY_OK;
 }
 
+// the checks both forward ray-export entry points make before anything runs; *platesize: the build's, *scale: its zoom
+int check_export_forward(blinky_ctx *ctx, const char *who, int width, int height, int *platesize, const float *rays, double *scale) {
+    if (!rays || reinterpret_cast<uintptr_t>(rays) % 4 != 0) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": rays must be a non-NULL, 4-byte aligned pointer");
+    if (width <= 0 || height <= 0) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": width and height must be positive");
+    std::string why;
+    const int rc = ctx->host.check_rays_forward(width, height, platesize, scale, &why);
+    if (rc == -1) return set_err(ctx, BLINKY_E_INVALID, std::string(who) + ": " + why);
+    if (rc == -7) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": " + why);
+    if (rc != 0) return set_err(ctx, BLINKY_E_ZOOM, std::string(who) + ": zoom could not be computed for this lens: " + ctx->host.log());
+    return BLINKY_OK;
+}
+
+// blinky_get_raymap_forward and the host path of blinky_get_raymap_forward_device: the serial forward builder into host memory
+int get_raymap_forward_host(blinky_ctx *ctx, const char *who, int width, int height, int platesize, double scale, float *rays, const std::string &path) {
+    auto t0 = std::chrono::steady_clock::now();
+    if (ctx->host.export_rays_forward(width, height, platesize, scale, rays) != 0)
+        return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": lens_forward failed: " + ctx->host.log());
+    char t[64];
+    snprintf(t, sizeof t, "; rays %.1f ms", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+    ctx->build_info = "ray export (forward), " + path + t;
+    return BLINKY_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -341,6 +364,13 @@ int blinky_get_raymap(blinky_ctx *ctx, int width, int height, float *rays) {
     double scale;
     const int rc = check_export(ctx, who, width, height, rays, &scale);
     return rc != BLINKY_OK ? rc : get_raymap_host(ctx, who, width, height, scale, rays, "host");
+}
+
+int blinky_get_raymap_forward(blinky_ctx *ctx, int width, int height, int platesize, float *rays) {
+    const char *who = "blinky_get_raymap_forward";
+    double scale;
+    const int rc = check_export_forward(ctx, who, width, height, &platesize, rays, &scale);
+    return rc != BLINKY_OK ? rc : get_raymap_forward_host(ctx, who, width, height, platesize, scale, rays, "host");
 }
 
 const char *blinky_build_info(blinky_ctx *ctx) { return ctx->build_info.c_str(); }
@@ -617,6 +647,32 @@ int blinky_get_raymap_device(blinky_ctx *ctx, int width, int height, float *d_ra
     char t[192];
     snprintf(t, sizeof t, "ray export, device: %zu of %zu pixels settled by the interpreter; NVRTC %.0f ms, kernel %.3f ms", settled, npix,
              ctx->lens_dev->last_compile_ms(), ctx->lens_dev->last_kernel_ms());
+    ctx->build_info = t;
+    return BLINKY_OK;
+}
+
+int blinky_get_raymap_forward_device(blinky_ctx *ctx, int width, int height, int platesize, float *d_rays, void *stream) {
+    NEED_DEVICE(ctx);
+    const char *who = "blinky_get_raymap_forward_device";
+    double scale;
+    int rc = check_export_forward(ctx, who, width, height, &platesize, d_rays, &scale);
+    if (rc != BLINKY_OK) return rc;
+    // the host settles grid points between the kernels and the call returns with the field complete: nothing here can be captured
+    if (LensDevice::capturing(stream)) return set_err(ctx, BLINKY_E_STATE, std::string(who) + ": the stream is capturing a graph");
+    const size_t npix = static_cast<size_t>(width) * height;
+    std::string why;
+    size_t settled = 0;
+    rc = ctx->host.export_rays_forward_device(width, height, platesize, scale, d_rays, stream, &settled, &why);
+    if (rc == -2) return set_err(ctx, BLINKY_E_SCRIPT, std::string(who) + ": lens_forward failed: " + ctx->host.log());
+    if (rc == 1) {
+        std::vector<float> rays(3 * npix);
+        rc = get_raymap_forward_host(ctx, who, width, height, platesize, scale, rays.data(), "host (" + why + ")");
+        if (rc != BLINKY_OK) return rc;
+        return ctx->lens_dev->copy_to_device(d_rays, rays.data(), rays.size() * sizeof(float), stream, &ctx->err) ? BLINKY_OK : BLINKY_E_CUDA;
+    }
+    char t[256];
+    snprintf(t, sizeof t, "ray export (forward), device: %zu grid points settled by the interpreter; NVRTC %.0f ms, kernels %.3f ms (rays %.3f ms)",
+             settled, ctx->lens_dev->last_compile_ms(), ctx->lens_dev->last_kernel_ms(), ctx->lens_dev->last_ray_kernel_ms());
     ctx->build_info = t;
     return BLINKY_OK;
 }

@@ -6,6 +6,7 @@
 // float expressions are evaluated in float (x86-64, FLT_EVAL_METHOD 0) and this
 // file is compiled with -ffp-contract=off and never with -ffast-math.
 #include "fisheye_host.h"
+#include "forward_raster.h"
 #include "lua_transpile.h"
 #include "parallel.h"
 
@@ -1296,18 +1297,21 @@ int FisheyeHost::build_inverse(int threads) {
 // forward builder (fisheye.c:2126-2338)
 // ---------------------------------------------------------------------------
 
-int FisheyeHost::uv_to_screen(Worker &w, int plate, double u, double v, int *lx, int *ly) {
+int FisheyeHost::uv_to_screen(Worker &w, const ForwardView &fv, int plate, double u, double v, int *lx, int *ly) {
     float ray[3];
     plate_uv_to_ray(plate, u, v, ray);
     double x, y;
     int status = call_forward(w, ray, &x, &y);
     if (status != 1) return status;
-    *lx = static_cast<int>(x / scale_ + width_px_ / 2);
-    *ly = static_cast<int>(-y / scale_ + height_px_ / 2);
+    *lx = static_cast<int>(x / fv.scale + fv.width / 2);
+    *ly = static_cast<int>(-y / fv.scale + fv.height / 2);
     return 1;
 }
 
-void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const int *br, int plate, int px, int py, int *display) {
+// sink.pixel(x, y, quad) for every pixel the quad covers (before the screen check), sink.too_wide(n) where the
+// reference prints "%d > maxdiff"; quad: the corners {tl, tr, br, bl}
+template <class Sink>
+void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const int *br, Sink &sink) {
     const int *corner[4] = {tl, tr, br, bl};  // clockwise
     int x = tl[0], y = tl[1];
     int minx = x, maxx = x, miny = y, maxy = y;
@@ -1319,15 +1323,15 @@ void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const i
     const int maxdiff = 20;  // wrap-around guard, :2271
     if (std::abs(minx - maxx) > maxdiff || std::abs(miny - maxy) > maxdiff) return;
     if (miny == maxy && minx == maxx) {
-        set_from_plate(x, y, px, py, plate, display);
+        sink.pixel(x, y, corner);
         return;
     }
     if (miny == maxy) {
-        for (int tx = minx; tx <= maxx; ++tx) set_from_plate(tx, miny, px, py, plate, display);
+        for (int tx = minx; tx <= maxx; ++tx) sink.pixel(tx, miny, corner);
         return;
     }
     if (minx == maxx) {
-        for (int ty = miny; ty <= maxy; ++ty) set_from_plate(x, ty, px, py, plate, display);
+        for (int ty = miny; ty <= maxy; ++ty) sink.pixel(x, ty, corner);
         return;
     }
     for (y = miny; y <= maxy; ++y) {
@@ -1347,102 +1351,24 @@ void FisheyeHost::draw_quad(const int *tl, const int *tr, const int *bl, const i
         }
         if (tx[0] > tx[1]) std::swap(tx[0], tx[1]);
         if (tx[1] - tx[0] > maxdiff) {
-            print("%d > maxdiff\n", tx[1] - tx[0]);
+            sink.too_wide(tx[1] - tx[0]);
             return;
         }
-        for (x = tx[0]; x <= tx[1]; ++x) set_from_plate(x, y, px, py, plate, display);
+        for (x = tx[0]; x <= tx[1]; ++x) sink.pixel(x, y, corner);
     }
 }
 
-// Forward lenses on the GPU: lens_forward is evaluated at every plate grid point by the translated
-// kernel, the interpreter settles the points the device could not decide, then the quads are
-// rasterised on the device in the reference's writer order (lens_device.cu).
-int FisheyeHost::build_forward_device(std::string *why) {
-    std::string src;
-    if (!lens_device_source(true, &src, why, true, true)) return 1;
-    const LensBuildParams p = device_params(width_px_, height_px_, platesize_);
-    std::vector<uint32_t> undecided, undecided_texels;
-    if (!device_builder_->forward_points(src, p, &undecided, &undecided_texels, why)) return 1;
-    std::vector<ForwardPatch> patches(undecided.size());
-    const int n1 = platesize_ + 1;
-    int display_unused[kMaxPlates] = {0, 0, 0, 0, 0, 0};
-    std::atomic<int> bad(0);
-    // the workers only need lens_forward; the generic worker setup parks lens_inverse (may be nil: fine)
-    lua_->set_global("__blinky_forward", fn_forward_);
-    int rc = settle_flagged(undecided.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
-        if (!w.forward.is_function()) w.forward = w.L->get_global("__blinky_forward");
-        for (size_t k = b; k < e; ++k) {
-            const uint32_t pt = undecided[k];
-            const int i = static_cast<int>(pt % n1), j = static_cast<int>(pt / n1 % n1), plate = static_cast<int>(pt / n1 / n1);
-            ForwardPatch &out = patches[k];
-            out.point = pt;
-            out.lx = out.ly = 0;
-            out.status = uv_to_screen(w, plate, (i - 0.5) / platesize_, (j - 0.5) / platesize_, &out.lx, &out.ly);
-            if (out.status < 0) bad.store(1);
-        }
-        w.forward = Value();
-        return 0;
-    });
-    lua_->set_global("__blinky_forward", Value());
-    if (rc != 0 || bad.load()) return -1;
-    // with a globe_plate script: the texel owners the device could not decide, from ray_to_plate_index on
-    // the very ray build_forward makes for the texel
-    std::vector<uint32_t> owner_patches(undecided_texels.size());
-    if (!undecided_texels.empty()) {
-        const int ps = platesize_;
-        rc = settle_flagged(undecided_texels.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
-            for (size_t k = b; k < e; ++k) {
-                const uint32_t t = undecided_texels[k];
-                const int px = static_cast<int>(t % ps), py = static_cast<int>(t / ps % ps), plate = static_cast<int>(t / ps / ps);
-                float ray[3];
-                plate_uv_to_ray(plate, static_cast<double>(px) / ps, static_cast<double>(py) / ps, ray);
-                owner_patches[k] = t | (ray_to_plate_index(w, ray) == plate ? kOwnerPatchOwned : 0u);
-            }
-            return 0;
-        });
-        if (rc != 0) return -1;
-    }
-    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
-    std::vector<std::pair<uint32_t, int>> messages;
-    if (!device_builder_->forward_finish(patches, owner_patches, idx_.data(), tint_.data(), display, &messages, why)) {
-        std::fill(idx_.begin(), idx_.end(), -1);
-        std::fill(tint_.begin(), tint_.end(), 255);
-        return 1;
-    }
-    std::sort(messages.begin(), messages.end());
-    for (auto &m : messages) print("%d > maxdiff\n", m.second);
-    for (int i = 0; i < kMaxPlates; ++i) plates_[i].display = display[i];
-    char info[200];
-    if (fn_globe_plate_.is_function()) {
-        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points and %zu of %zu texel owners re-evaluated by the interpreter",
-                 undecided.size(), static_cast<size_t>(numplates_) * n1 * n1, undecided_texels.size(),
-                 static_cast<size_t>(numplates_) * platesize_ * platesize_);
-    } else {
-        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points re-evaluated by the interpreter", undecided.size(),
-                 static_cast<size_t>(numplates_) * n1 * n1);
-    }
-    build_info_ = info;
-    return 0;
-}
-
-int FisheyeHost::build_forward(int threads) {
-    if (!fn_forward_.is_function()) {
-        print("lens_forward is not a function\n");
-        return -2;
-    }
-    if (threads == 0) {
-        std::string why = "no GPU lens builder installed";
-        int rc = device_builder_ ? build_forward_device(&why) : 1;
-        if (rc != 1) return rc;
-        build_info_ = "host (forward lens; " + why + ")";
-    }
+// The serial forward builder (resume_lensmap_forward, fisheye.c:2126-2243) at the geometry fv: every texel's quad,
+// in the reference's order, to draw_quad with sink.texel(plate, px, py) called first.  0 ok; -1 when lens_forward
+// or globe_plate fails.
+template <class Sink>
+int FisheyeHost::forward_loop(const ForwardView &fv, Sink &sink) {
     Worker w;
     w.L = lua_.get();
     w.forward = fn_forward_;
     w.globe_plate = fn_globe_plate_;
     w.has_globe_plate = fn_globe_plate_.is_function();
-    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
-    const int ps = platesize_;
+    const int ps = fv.ps;
     // two rows of (ps+1) screen points; zero-initialised (the reference leaves
     // them uninitialised, which only matters if lens_forward returns nil)
     std::vector<int> rowa(static_cast<size_t>(ps + 1) * 2, 0), rowb(static_cast<size_t>(ps + 1) * 2, 0);
@@ -1454,12 +1380,12 @@ int FisheyeHost::build_forward(int threads) {
                 auto fill_row = [&](int *row, double v) -> int {
                     for (int px = 0; px < ps; ++px) {
                         if (px == 0) {
-                            int st = uv_to_screen(w, plate, (px - 0.5) / ps, v, &row[0], &row[1]);
+                            int st = uv_to_screen(w, fv, plate, (px - 0.5) / ps, v, &row[0], &row[1]);
                             if (st == 0) continue;
                             if (st == -1) return -1;
                         }
                         int at = 2 * (px + 1);
-                        int st = uv_to_screen(w, plate, (px + 0.5) / ps, v, &row[at], &row[at + 1]);
+                        int st = uv_to_screen(w, fv, plate, (px + 0.5) / ps, v, &row[at], &row[at + 1]);
                         if (st == 0) continue;
                         if (st == -1) return -1;
                     }
@@ -1477,7 +1403,8 @@ int FisheyeHost::build_forward(int threads) {
                     plate_uv_to_ray(plate, static_cast<double>(px) / ps, v, ray);
                     if (plate != ray_to_plate_index(w, ray)) continue;  // texel owned by another plate
                     int at = 2 * px;
-                    draw_quad(&top[at], &top[at + 2], &bot[at], &bot[at + 2], plate, px, py, display);
+                    sink.texel(plate, px, py);
+                    draw_quad(&top[at], &top[at + 2], &bot[at], &bot[at + 2], sink);
                 }
             }
         }
@@ -1485,7 +1412,116 @@ int FisheyeHost::build_forward(int threads) {
         print("%s\n", e.what());
         rc = -1;
     }
+    return rc;
+}
+
+// Forward lenses on the GPU, step 1 at the geometry fv: lens_forward is evaluated at every plate grid point by the
+// translated kernel, and the interpreter settles the points (and, with a globe_plate script, the texel owners) the
+// device could not decide.  0 ok, -1 script failure, 1 = not possible on the device (why).
+int FisheyeHost::forward_device_points(const ForwardView &fv, std::vector<ForwardPatch> *patches, std::vector<uint32_t> *owner_patches,
+                                       std::string *why) {
+    std::string src;
+    if (!lens_device_source(true, &src, why, true, true)) return 1;
+    LensBuildParams p = device_params(fv.width, fv.height, fv.ps);
+    p.scale = fv.scale;
+    std::vector<uint32_t> undecided, undecided_texels;
+    if (!device_builder_->forward_points(src, p, &undecided, &undecided_texels, why)) return 1;
+    patches->assign(undecided.size(), ForwardPatch{});
+    const int n1 = fv.ps + 1;
+    int display_unused[kMaxPlates] = {0, 0, 0, 0, 0, 0};
+    std::atomic<int> bad(0);
+    // the workers only need lens_forward; the generic worker setup parks lens_inverse (may be nil: fine)
+    lua_->set_global("__blinky_forward", fn_forward_);
+    int rc = settle_flagged(undecided.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
+        if (!w.forward.is_function()) w.forward = w.L->get_global("__blinky_forward");
+        for (size_t k = b; k < e; ++k) {
+            const uint32_t pt = undecided[k];
+            const int i = static_cast<int>(pt % n1), j = static_cast<int>(pt / n1 % n1), plate = static_cast<int>(pt / n1 / n1);
+            ForwardPatch &out = (*patches)[k];
+            out.point = pt;
+            out.lx = out.ly = 0;
+            out.status = uv_to_screen(w, fv, plate, (i - 0.5) / fv.ps, (j - 0.5) / fv.ps, &out.lx, &out.ly);
+            if (out.status < 0) bad.store(1);
+        }
+        w.forward = Value();
+        return 0;
+    });
+    lua_->set_global("__blinky_forward", Value());
+    if (rc != 0 || bad.load()) return -1;
+    // with a globe_plate script: the texel owners the device could not decide, from ray_to_plate_index on
+    // the very ray build_forward makes for the texel
+    owner_patches->assign(undecided_texels.size(), 0u);
+    if (!undecided_texels.empty()) {
+        const int ps = fv.ps;
+        rc = settle_flagged(undecided_texels.size(), display_unused, [&](Worker &w, size_t b, size_t e, int *) {
+            for (size_t k = b; k < e; ++k) {
+                const uint32_t t = undecided_texels[k];
+                const int px = static_cast<int>(t % ps), py = static_cast<int>(t / ps % ps), plate = static_cast<int>(t / ps / ps);
+                float ray[3];
+                plate_uv_to_ray(plate, static_cast<double>(px) / ps, static_cast<double>(py) / ps, ray);
+                (*owner_patches)[k] = t | (ray_to_plate_index(w, ray) == plate ? kOwnerPatchOwned : 0u);
+            }
+            return 0;
+        });
+        if (rc != 0) return -1;
+    }
+    return 0;
+}
+
+// Forward lenses on the GPU: step 1 (forward_device_points), then the quads are rasterised on the device in the
+// reference's writer order (lens_device.cu).
+int FisheyeHost::build_forward_device(std::string *why) {
+    const ForwardView fv{width_px_, height_px_, platesize_, scale_};
+    std::vector<ForwardPatch> patches;
+    std::vector<uint32_t> owner_patches;
+    const int rc = forward_device_points(fv, &patches, &owner_patches, why);
+    if (rc != 0) return rc;
+    const int n1 = platesize_ + 1;
+    int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
+    std::vector<std::pair<uint32_t, int>> messages;
+    if (!device_builder_->forward_finish(patches, owner_patches, idx_.data(), tint_.data(), display, &messages, why)) {
+        std::fill(idx_.begin(), idx_.end(), -1);
+        std::fill(tint_.begin(), tint_.end(), 255);
+        return 1;
+    }
+    std::sort(messages.begin(), messages.end());
+    for (auto &m : messages) print("%d > maxdiff\n", m.second);
     for (int i = 0; i < kMaxPlates; ++i) plates_[i].display = display[i];
+    char info[200];
+    if (fn_globe_plate_.is_function()) {
+        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points and %zu of %zu texel owners re-evaluated by the interpreter",
+                 patches.size(), static_cast<size_t>(numplates_) * n1 * n1, owner_patches.size(),
+                 static_cast<size_t>(numplates_) * platesize_ * platesize_);
+    } else {
+        snprintf(info, sizeof info, "device (forward): %zu of %zu grid points re-evaluated by the interpreter", patches.size(),
+                 static_cast<size_t>(numplates_) * n1 * n1);
+    }
+    build_info_ = info;
+    return 0;
+}
+
+int FisheyeHost::build_forward(int threads) {
+    if (!fn_forward_.is_function()) {
+        print("lens_forward is not a function\n");
+        return -2;
+    }
+    if (threads == 0) {
+        std::string why = "no GPU lens builder installed";
+        int rc = device_builder_ ? build_forward_device(&why) : 1;
+        if (rc != 1) return rc;
+        build_info_ = "host (forward lens; " + why + ")";
+    }
+    // the lensmap: set_lensmap_from_plate (fisheye.c:1963-1982) for every pixel a quad covers
+    struct MapSink {
+        FisheyeHost *h;
+        int display[kMaxPlates] = {0, 0, 0, 0, 0, 0};
+        int plate = 0, px = 0, py = 0;
+        void texel(int p, int x, int y) { plate = p, px = x, py = y; }
+        void pixel(int lx, int ly, const int *const *) { h->set_from_plate(lx, ly, px, py, plate, display); }
+        void too_wide(int n) { h->print("%d > maxdiff\n", n); }
+    } sink{this};
+    const int rc = forward_loop(ForwardView{width_px_, height_px_, platesize_, scale_}, sink);
+    for (int i = 0; i < kMaxPlates; ++i) plates_[i].display = sink.display[i];
     return rc;
 }
 
@@ -1918,6 +1954,84 @@ int FisheyeHost::export_rays_device(int width, int height, double scale, float *
     if (rc != 0) return -2;
     if (!device_builder_->patch_rays(samples, d_rays, stream, why)) return 1;
     *settled = samples.size();
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// ray export of a forward lens (DESIGN §3h): the forward build's winning quads, interpolated
+// ---------------------------------------------------------------------------
+
+int FisheyeHost::check_rays_forward(int width, int height, int *platesize, double *scale, std::string *why) {
+    if (*platesize <= 0) *platesize = width < height ? width : height;
+    if (static_cast<int64_t>(*platesize) * *platesize * kMaxPlates > 0x0FFFFFFF) {
+        *why = "platesize too large: 6 * platesize^2 must stay below 2^28";
+        return -1;
+    }
+    if (!lens_valid_) {
+        *why = "no valid lens";
+        return -7;
+    }
+    if (!fn_forward_.is_function()) {
+        *why = "the lens has no lens_forward";
+        return -7;
+    }
+    if (!globe_valid_) {
+        *why = "no valid globe";
+        return -7;
+    }
+    return calc_zoom(width, height, scale) ? 0 : -3;
+}
+
+namespace {
+
+// the plate as the device kernels read it (LensBuildParams::PlateF)
+LensBuildParams::PlateF plate_f(const Plate &pl) {
+    LensBuildParams::PlateF f;
+    for (int k = 0; k < 3; ++k) {
+        f.forward[k] = pl.forward[k];
+        f.right[k] = pl.right[k];
+        f.up[k] = pl.up[k];
+    }
+    f.dist = pl.dist;
+    return f;
+}
+
+}  // namespace
+
+int FisheyeHost::export_rays_forward(int width, int height, int platesize, double scale, float *rays) {
+    const size_t npix = static_cast<size_t>(width) * height;
+    std::fill(rays, rays + 3 * npix, 0.0f);
+    // the build's last writer of each pixel leaves its ray: the same rule the device applies to the winning key
+    struct RaySink {
+        const FisheyeHost *h;
+        int width, height, ps;
+        float *rays;
+        int plate = 0, px = 0, py = 0;
+        void texel(int p, int x, int y) { plate = p, px = x, py = y; }
+        void pixel(int lx, int ly, const int *const *corner) {
+            if (lx < 0 || lx >= width || ly < 0 || ly >= height) return;  // set_lensmap_from_plate's screen check
+            const int cx[4] = {corner[0][0], corner[1][0], corner[2][0], corner[3][0]};
+            const int cy[4] = {corner[0][1], corner[1][1], corner[2][1], corner[3][1]};
+            fwd_quad_ray(plate_f(h->plates_[plate]), ps, px, py, cx, cy, lx, ly, rays + 3 * (static_cast<size_t>(ly) * width + lx));
+        }
+        void too_wide(int) {}  // the export prints nothing
+    } sink{this, width, height, platesize, rays};
+    return forward_loop(ForwardView{width, height, platesize, scale}, sink) == 0 ? 0 : -2;
+}
+
+int FisheyeHost::export_rays_forward_device(int width, int height, int platesize, double scale, float *d_rays, void *stream, size_t *settled,
+                                            std::string *why) {
+    *settled = 0;
+    if (!device_builder_) {
+        *why = "no GPU lens builder installed";
+        return 1;
+    }
+    std::vector<ForwardPatch> patches;
+    std::vector<uint32_t> owner_patches;
+    const int rc = forward_device_points(ForwardView{width, height, platesize, scale}, &patches, &owner_patches, why);
+    if (rc != 0) return rc == -1 ? -2 : 1;
+    if (!device_builder_->forward_rays(patches, owner_patches, d_rays, stream, why)) return 1;
+    *settled = patches.size() + owner_patches.size();
     return 0;
 }
 

@@ -129,6 +129,22 @@ public:
     // export_rays.
     int export_rays_device(int width, int height, double scale, float *d_rays, void *stream, size_t *settled, std::string *why);
 
+    // ---- ray export of a forward lens (DESIGN §3h) ------------------------------------------------------------------
+    // The view rays of a width x height forward build on plates of platesize texels, at the scale calc_zoom gives:
+    // each pixel the build maps gets the ray through the point of its winning texel's quad where the pixel lies
+    // (forward_raster.h: fwd_quad_ray), normalised; the others get (0, 0, 0).  Same layout as export_rays.  The build's
+    // grid points, stale slots, texel owners and maxdiff guard apply; nothing is printed and nothing of the context
+    // changes.  check_rays_forward: platesize <= 0 becomes min(width, height); 0 with the scale in *scale; -1 for a
+    // platesize beyond the 28-bit texel index; -7 without a valid lens, a lens_forward function or a valid globe
+    // (reason in *why); -3 when the zoom fails (the build's console message is printed).
+    int check_rays_forward(int width, int height, int *platesize, double *scale, std::string *why);
+    // the host path: the serial forward builder; 0 ok, -2 when lens_forward or globe_plate fails
+    int export_rays_forward(int width, int height, int platesize, double scale, float *rays);
+    // the device path: the rays into d_rays (device memory) on `stream`, with *settled grid points and texel owners
+    // settled by the interpreter.  0 ok; 1 = not possible on the device (why): take the host path; -2 as the host path.
+    int export_rays_forward_device(int width, int height, int platesize, double scale, float *d_rays, void *stream, size_t *settled,
+                                   std::string *why);
+
     // ---- results -------------------------------------------------------------
     int width() const { return width_px_; }
     int height() const { return height_px_; }
@@ -236,8 +252,16 @@ private:
     int build_inverse_device(int *display, std::string *why);  // 0 ok, -1 script failure, 1 = not possible (why)
     int build_forward_device(std::string *why);                // same convention
     int build_forward(int threads);
-    int uv_to_screen(Worker &w, int plate, double u, double v, int *lx, int *ly);
-    void draw_quad(const int *tl, const int *tr, const int *bl, const int *br, int plate, int px, int py, int *display);
+    struct ForwardView {  // the geometry of a forward build
+        int width, height, ps;
+        double scale;
+    };
+    int forward_device_points(const ForwardView &fv, std::vector<ForwardPatch> *patches, std::vector<uint32_t> *owner_patches, std::string *why);
+    template <class Sink>
+    int forward_loop(const ForwardView &fv, Sink &sink);
+    int uv_to_screen(Worker &w, const ForwardView &fv, int plate, double u, double v, int *lx, int *ly);
+    template <class Sink>
+    void draw_quad(const int *tl, const int *tr, const int *bl, const int *br, Sink &sink);
     void finish_build();
     void unpack_map(const uint32_t *packed);
 

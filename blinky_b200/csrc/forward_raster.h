@@ -92,6 +92,27 @@ FWD_HD void fwd_stale_chain(FwdPoint *grid, const unsigned char *status, int ps,
 
 FWD_HD float fwd_dot3(const float *a, const float *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
+// plate_uv_to_ray (fisheye.c:1198-1214) in the host's float operations (FisheyeHost::plate_uv_to_ray): the
+// normalised ray through (u, v) of plate P
+FWD_HD void fwd_plate_uv_to_ray(const LensBuildParams::PlateF &P, double u, double v, float r[3]) {
+    u -= 0.5;
+    v -= 0.5;
+    v = -v;
+    r[0] = r[1] = r[2] = 0.0f;
+    const float fu = static_cast<float>(u), fv = static_cast<float>(v);
+    for (int k = 0; k < 3; ++k) r[k] = r[k] + P.dist * P.forward[k];
+    for (int k = 0; k < 3; ++k) r[k] = r[k] + fu * P.right[k];
+    for (int k = 0; k < 3; ++k) r[k] = r[k] + fv * P.up[k];
+    float len = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
+    len = static_cast<float>(sqrt(static_cast<double>(len)));
+    if (len) {
+        const float inv = 1 / len;
+        r[0] *= inv;
+        r[1] *= inv;
+        r[2] *= inv;
+    }
+}
+
 FWD_HD void fwd_set(const FwdGeom &g, const FwdOut &o, int lx, int ly, unsigned key, bool ongrid, int plate) {
     if (lx < 0 || lx >= g.width || ly < 0 || ly >= g.height) return;  // set_lensmap_from_plate's screen check
     o.counters[3 + plate] = 1u;                                         // display flag (benign race: all writers store 1)
@@ -115,24 +136,8 @@ FWD_HD void fwd_raster_texel(const FwdGeom &g, const FwdPoint *grid, const FwdOu
         if (!(owner[(static_cast<size_t>(plate) * ps + py) * ps + px] & kOwnerOwned)) return;
     } else {
         // the texel belongs to this plate only if the plate wins the ray's argmax (:2193-2199)
-        const LensBuildParams::PlateF &P = g.plates[plate];
-        double u = static_cast<double>(px) / ps, v = static_cast<double>(py) / ps;
-        u -= 0.5;
-        v -= 0.5;
-        v = -v;
-        float r[3] = {0.0f, 0.0f, 0.0f};
-        const float fu = static_cast<float>(u), fv = static_cast<float>(v);
-        for (int k = 0; k < 3; ++k) r[k] = r[k] + P.dist * P.forward[k];
-        for (int k = 0; k < 3; ++k) r[k] = r[k] + fu * P.right[k];
-        for (int k = 0; k < 3; ++k) r[k] = r[k] + fv * P.up[k];
-        float len = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
-        len = static_cast<float>(sqrt(static_cast<double>(len)));
-        if (len) {
-            const float inv = 1 / len;
-            r[0] *= inv;
-            r[1] *= inv;
-            r[2] *= inv;
-        }
+        float r[3];
+        fwd_plate_uv_to_ray(g.plates[plate], static_cast<double>(px) / ps, static_cast<double>(py) / ps, r);
         int best = 0;
         double best_dp = -2;
         for (int k = 0; k < g.numplates; ++k) {
@@ -215,6 +220,80 @@ FWD_HD void fwd_resolve_pixel(const unsigned *idxkey, const unsigned *tintkey, i
     }
     const unsigned tk = tintkey[at];
     tint[at] = tk ? static_cast<uint8_t>((tk - 1) / ps / ps) : 255;
+}
+
+// ---- ray export of a forward lens (DESIGN §3h) -------------------------------------------------------------------
+
+// Where pixel (X, Y) lies in a quad the raster drew it with: (s, t) in [0, 1]^2 with tl = (0, 0), tr = (1, 0),
+// br = (1, 1) and bl = (0, 1); cx, cy: the corners in the raster's order {tl, tr, br, bl}.  A corner c came from
+// (int)(x / scale + W/2) and the pixel sits at X, so both are measured in half pixels: 2c + 1 and 2X.  The quad is
+// split into A = (tl, tr, br) and B = (tl, br, bl); the first non-degenerate triangle that contains the pixel (its
+// boundary included) gives (s, t) by exact integer signed areas, one double division each.  When neither contains
+// it, the first non-degenerate one does, with s and t clamped.  Both degenerate, or a corner further than the
+// raster's maxdiff from tl (corners wrapped at INT_MIN / INT_MAX that its 32-bit bounding box lets through): the
+// quad's centre.
+FWD_HD void fwd_quad_st(const int cx[4], const int cy[4], int X, int Y, double *s, double *t) {
+    *s = *t = 0.5;
+    long long qx[4], qy[4];  // corner offsets from tl, in half pixels
+    for (int i = 0; i < 4; ++i) {
+        const long long dx = static_cast<long long>(cx[i]) - cx[0], dy = static_cast<long long>(cy[i]) - cy[0];
+        if (dx > 20 || dx < -20 || dy > 20 || dy < -20) return;
+        qx[i] = 2 * dx;
+        qy[i] = 2 * dy;
+    }
+    const long long pxo = 2 * (static_cast<long long>(X) - cx[0]) - 1, pyo = 2 * (static_cast<long long>(Y) - cy[0]) - 1;
+    int use = -1;       // the triangle (s, t) comes from: 0 = A, 1 = B
+    bool clamp = true;  // it does not contain the pixel
+    long long use_a1 = 0, use_a2 = 0, use_area = 0;
+    for (int tri = 0; tri < 2 && clamp; ++tri) {
+        const int i1 = tri == 0 ? 1 : 2, i2 = tri == 0 ? 2 : 3;  // V0 = tl, V1, V2
+        const long long area = qx[i1] * qy[i2] - qy[i1] * qx[i2];
+        if (area == 0) continue;
+        const long long a1 = pxo * qy[i2] - pyo * qx[i2];  // area(V0, p, V2)
+        const long long a2 = qx[i1] * pyo - qy[i1] * pxo;  // area(V0, V1, p)
+        const long long a0 = area - a1 - a2;
+        const bool inside = area > 0 ? (a0 >= 0 && a1 >= 0 && a2 >= 0) : (a0 <= 0 && a1 <= 0 && a2 <= 0);
+        if (use < 0 || inside) {
+            use = tri;
+            use_a1 = a1;
+            use_a2 = a2;
+            use_area = area;
+        }
+        if (inside) clamp = false;
+    }
+    if (use < 0) return;
+    // with l1, l2 the weights of V1, V2: A gives s = l1 + l2, t = l2; B gives s = l1, t = l1 + l2
+    const double area = static_cast<double>(use_area);
+    double ss = static_cast<double>(use == 0 ? use_a1 + use_a2 : use_a1) / area;
+    double tt = static_cast<double>(use == 0 ? use_a2 : use_a1 + use_a2) / area;
+    if (clamp) {
+        ss = ss < 0 ? 0 : (ss > 1 ? 1 : ss);
+        tt = tt < 0 ? 0 : (tt > 1 ? 1 : tt);
+    }
+    *s = ss;
+    *t = tt;
+}
+
+// the ray of pixel (X, Y) drawn by the texel (px, py) of plate P through the quad (cx, cy): the plate point at
+// ((px - 1/2 + s) / ps, (py - 1/2 + t) / ps), grid point i lying at (i - 1/2) / ps
+FWD_HD void fwd_quad_ray(const LensBuildParams::PlateF &P, int ps, int px, int py, const int cx[4], const int cy[4], int X, int Y, float r[3]) {
+    double s, t;
+    fwd_quad_st(cx, cy, X, Y, &s, &t);
+    const double u = ((px - 0.5) + s) / ps, v = ((py - 0.5) + t) / ps;
+    fwd_plate_uv_to_ray(P, u, v, r);
+}
+
+// the exported ray of pixel (X, Y) from its highest writer key k (idxkey): the zero vector when no texel drew it
+FWD_HD void fwd_ray_pixel(const FwdGeom &g, const FwdPoint *grid, unsigned k, int X, int Y, float r[3]) {
+    if (!k) {
+        r[0] = r[1] = r[2] = 0.0f;
+        return;
+    }
+    const unsigned ps = static_cast<unsigned>(g.ps), key = k - 1, px = key % ps, q = key / ps, py = ps - 1 - q % ps, plate = q / ps;
+    const size_t n1 = ps + 1, top = (static_cast<size_t>(plate) * n1 + py) * n1, bot = top + n1;
+    const FwdPoint c0 = grid[top + px], c1 = grid[top + px + 1], c2 = grid[bot + px + 1], c3 = grid[bot + px];
+    const int cx[4] = {c0.x, c1.x, c2.x, c3.x}, cy[4] = {c0.y, c1.y, c2.y, c3.y};
+    fwd_quad_ray(g.plates[plate], g.ps, static_cast<int>(px), static_cast<int>(py), cx, cy, X, Y, r);
 }
 
 }  // namespace blinky

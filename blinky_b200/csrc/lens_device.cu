@@ -396,6 +396,11 @@ struct LensDevice::ForwardState {
     unsigned nil_count = 0;
     DeviceBuffer owner;            // [numplates * ps * ps] texel owners; empty: the plate argmax decides
     DeviceBuffer owner_undecided;  // unsigned[kUndecidedCap]
+    // from patch_forward on
+    DeviceBuffer keys;             // idxkey[npix] then tintkey[npix]
+    DeviceBuffer messages;         // FwdMessage[kFwdMessageCap]
+    DeviceBuffer patches, owner_patches;  // the host's grid points and texel owners
+    bool any_nil = false;          // a grid point is nil: the stale slots need replaying
 };
 
 namespace {
@@ -453,6 +458,19 @@ __global__ void fwd_resolve_kernel(const unsigned *__restrict__ idxkey, const un
                                    uint8_t *__restrict__ tint, size_t npix, int ps) {
     const size_t at = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (at < npix) fwd_resolve_pixel(idxkey, tintkey, idx, tint, at, ps);
+}
+
+// the exported ray of each pixel from the forward build's winning texel (ray export of a forward lens, DESIGN §3h)
+__global__ void __launch_bounds__(256) fwd_ray_kernel(const __grid_constant__ FwdGeom g, const FwdPoint *__restrict__ grid,
+                                                      const unsigned *__restrict__ idxkey, float *__restrict__ rays, size_t npix) {
+    const size_t at = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (at >= npix) return;
+    const int y = static_cast<int>(at / static_cast<unsigned>(g.width)), x = static_cast<int>(at - static_cast<size_t>(y) * g.width);
+    float r[3];
+    fwd_ray_pixel(g, grid, idxkey[at], x, y, r);
+    rays[3 * at] = r[0];
+    rays[3 * at + 1] = r[1];
+    rays[3 * at + 2] = r[2];
 }
 
 // true when ce is cudaSuccess; otherwise false with "what: <CUDA error>" in *err
@@ -856,6 +874,67 @@ bool LensDevice::forward_points(const std::string &lens_source, const LensBuildP
     return true;
 }
 
+bool LensDevice::patch_forward(ForwardState &f, const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches,
+                               void *stream, std::string *err) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const size_t npix = static_cast<size_t>(f.p.width) * f.p.height;
+    cudaError_t ce = allocate(&f.keys, 2 * npix * sizeof(unsigned));
+    if (ce == cudaSuccess) ce = cudaMemsetAsync(f.keys.get(), 0, 2 * npix * sizeof(unsigned), s);
+    if (ce == cudaSuccess) ce = allocate(&f.messages, kMessageCap * sizeof(FwdMessage));
+    FwdPoint *grid = f.grid.as<FwdPoint>();
+    unsigned char *status = f.status.as<unsigned char>(), *owner = f.owner.as<unsigned char>();
+    f.any_nil = f.nil_count > 0;
+    if (ce == cudaSuccess && !patches.empty()) {
+        f.patches = upload(patches, s, &ce);
+        if (ce == cudaSuccess) {
+            const unsigned n = static_cast<unsigned>(patches.size());
+            fwd_patch_kernel<<<(n + 255) / 256, 256, 0, s>>>(grid, status, f.patches.as<ForwardPatch>(), n);
+        }
+        for (const ForwardPatch &pt : patches) f.any_nil = f.any_nil || pt.status != 1;
+    }
+    if (ce == cudaSuccess && !owner_patches.empty() && owner) {
+        f.owner_patches = upload(owner_patches, s, &ce);
+        if (ce == cudaSuccess) {
+            const unsigned n = static_cast<unsigned>(owner_patches.size());
+            fwd_owner_patch_kernel<<<(n + 255) / 256, 256, 0, s>>>(owner, f.owner_patches.as<uint32_t>(), n);
+        }
+    }
+    return checked(ce, "forward lensmap kernels", err);
+}
+
+namespace {
+
+FwdGeom forward_geom(const LensBuildParams &p) {
+    FwdGeom g;
+    g.width = p.width;
+    g.height = p.height;
+    g.ps = p.platesize;
+    g.numplates = p.numplates;
+    g.rubix_block = p.rubix_block;
+    g.rubix_pad = p.rubix_pad;
+    g.rubix_unit_px = p.rubix_unit_px;
+    memcpy(g.plates, p.plates, sizeof g.plates);
+    return g;
+}
+
+}  // namespace
+
+void LensDevice::raster_forward(ForwardState &f, void *stream) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const LensBuildParams &p = f.p;
+    const size_t npix = static_cast<size_t>(p.width) * p.height;
+    FwdPoint *grid = f.grid.as<FwdPoint>();
+    unsigned char *status = f.status.as<unsigned char>(), *owner = f.owner.as<unsigned char>();
+    if (f.any_nil) {
+        const int threads = 2 * (p.platesize + 1);
+        fwd_stale_kernel<<<(threads + 63) / 64, 64, 0, s>>>(grid, status, p.platesize, p.numplates);
+    }
+    unsigned *keys = f.keys.as<unsigned>();
+    FwdOut o{keys, keys + npix, f.counters.as<unsigned>(), f.messages.as<FwdMessage>()};
+    dim3 blocks((p.platesize + 127) / 128, p.platesize, p.numplates);
+    fwd_raster_kernel<<<blocks, 128, 0, s>>>(forward_geom(p), grid, o, owner);
+}
+
 bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx,
                                 uint8_t *tint, int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err) {
     const std::unique_ptr<ForwardState> f = std::move(fwd_);  // consumed whatever the outcome
@@ -865,50 +944,15 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const 
     }
     const LensBuildParams &p = f->p;
     const size_t npix = static_cast<size_t>(p.width) * p.height;
-    DeviceBuffer d_keys, d_messages, d_idx, d_tint, d_patches, d_owner_patches;  // d_keys: idxkey[npix] then tintkey[npix]
-    cudaError_t ce = allocate(&d_keys, 2 * npix * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = cudaMemset(d_keys.get(), 0, 2 * npix * sizeof(unsigned));
-    if (ce == cudaSuccess) ce = allocate(&d_messages, kMessageCap * sizeof(FwdMessage));
-    if (ce == cudaSuccess) ce = allocate(&d_idx, npix * sizeof(int32_t));
+    DeviceBuffer d_idx, d_tint;
+    if (!patch_forward(*f, patches, owner_patches, nullptr, err)) return false;
+    cudaError_t ce = allocate(&d_idx, npix * sizeof(int32_t));
     if (ce == cudaSuccess) ce = allocate(&d_tint, npix);
-    FwdPoint *grid = f->grid.as<FwdPoint>();
-    unsigned char *status = f->status.as<unsigned char>(), *owner = f->owner.as<unsigned char>();
-    bool any_nil = f->nil_count > 0;
-    if (ce == cudaSuccess && !patches.empty()) {
-        d_patches = upload(patches, nullptr, &ce);
-        if (ce == cudaSuccess) {
-            const unsigned n = static_cast<unsigned>(patches.size());
-            fwd_patch_kernel<<<(n + 255) / 256, 256>>>(grid, status, d_patches.as<ForwardPatch>(), n);
-        }
-        for (const ForwardPatch &pt : patches) any_nil = any_nil || pt.status != 1;
-    }
-    if (ce == cudaSuccess && !owner_patches.empty() && owner) {
-        d_owner_patches = upload(owner_patches, nullptr, &ce);
-        if (ce == cudaSuccess) {
-            const unsigned n = static_cast<unsigned>(owner_patches.size());
-            fwd_owner_patch_kernel<<<(n + 255) / 256, 256>>>(owner, d_owner_patches.as<uint32_t>(), n);
-        }
-    }
     EventTimer timer;
     if (ce == cudaSuccess) ce = timer.start(nullptr);
     if (ce == cudaSuccess) {
-        if (any_nil) {
-            const int threads = 2 * (p.platesize + 1);
-            fwd_stale_kernel<<<(threads + 63) / 64, 64>>>(grid, status, p.platesize, p.numplates);
-        }
-        FwdGeom g;
-        g.width = p.width;
-        g.height = p.height;
-        g.ps = p.platesize;
-        g.numplates = p.numplates;
-        g.rubix_block = p.rubix_block;
-        g.rubix_pad = p.rubix_pad;
-        g.rubix_unit_px = p.rubix_unit_px;
-        memcpy(g.plates, p.plates, sizeof g.plates);
-        unsigned *keys = d_keys.as<unsigned>();
-        FwdOut o{keys, keys + npix, f->counters.as<unsigned>(), d_messages.as<FwdMessage>()};
-        dim3 blocks((p.platesize + 127) / 128, p.platesize, p.numplates);
-        fwd_raster_kernel<<<blocks, 128>>>(g, grid, o, owner);
+        raster_forward(*f, nullptr);
+        unsigned *keys = f->keys.as<unsigned>();
         fwd_resolve_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256>>>(keys, keys + npix, d_idx.as<int32_t>(), d_tint.as<uint8_t>(), npix, p.platesize);
         timer.stop(nullptr);
         ce = cudaMemcpy(idx, d_idx.get(), npix * sizeof(int32_t), cudaMemcpyDeviceToHost);
@@ -924,11 +968,44 @@ bool LensDevice::forward_finish(const std::vector<ForwardPatch> &patches, const 
     kernel_ms_ += timer.ms();
     for (int i = 0; i < 6; ++i) display[i] = counters[3 + i] ? 1 : 0;
     std::vector<FwdMessage> msg(counters[2]);
-    if (counters[2] && !checked(cudaMemcpy(msg.data(), d_messages.get(), counters[2] * sizeof(FwdMessage), cudaMemcpyDeviceToHost),
+    if (counters[2] && !checked(cudaMemcpy(msg.data(), f->messages.get(), counters[2] * sizeof(FwdMessage), cudaMemcpyDeviceToHost),
                                 "forward lensmap kernels", err))
         return false;
     messages->clear();
     for (const FwdMessage &m : msg) messages->emplace_back(m.key, static_cast<int>(m.value));
+    return true;
+}
+
+bool LensDevice::forward_rays(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, float *d_rays, void *stream,
+                              std::string *err) {
+    const std::unique_ptr<ForwardState> f = std::move(fwd_);  // consumed whatever the outcome
+    ray_kernel_ms_ = 0;
+    if (!f) {
+        *err = "forward_rays without forward_points";
+        return false;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const LensBuildParams &p = f->p;
+    const size_t npix = static_cast<size_t>(p.width) * p.height;
+    if (!patch_forward(*f, patches, owner_patches, stream, err)) return false;
+    EventTimer timer, ray_timer;
+    cudaError_t ce = timer.start(s);
+    if (ce == cudaSuccess) {
+        raster_forward(*f, stream);
+        ce = ray_timer.start(s);
+    }
+    if (ce == cudaSuccess) {
+        const unsigned block = 256;
+        fwd_ray_kernel<<<static_cast<unsigned>((npix + block - 1) / block), block, 0, s>>>(forward_geom(p), f->grid.as<FwdPoint>(), f->keys.as<unsigned>(),
+                                                                                          d_rays, npix);
+        ce = cudaGetLastError();
+        ray_timer.stop(s);
+        timer.stop(s);
+    }
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);  // (the patches are pageable host memory the copies may still read)
+    if (!checked(ce, "forward ray export kernels", err)) return false;
+    kernel_ms_ += timer.ms();
+    ray_kernel_ms_ = ray_timer.ms();
     return true;
 }
 

@@ -97,6 +97,12 @@ public:
     // reference prints.
     bool forward_finish(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, int32_t *idx, uint8_t *tint,
                         int display[6], std::vector<std::pair<uint32_t, int>> *messages, std::string *err);
+    // step 2 for a ray export instead (DESIGN §3h): the same patches, stale slots and rasterised quads, then each
+    // pixel's ray from its winning texel's quad (forward_raster.h: fwd_ray_pixel), normalised, the zero vector where no
+    // texel draws, into d_rays (float32[height][width][3], device memory).  Everything runs on `stream` (a cudaStream_t)
+    // after the work already there; returns once the field is written.  Nothing is printed or kept.
+    bool forward_rays(const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, float *d_rays, void *stream,
+                      std::string *err);
     // ray maps: the packed lensmap entry of each of the width * height float32 rays at d_rays (unnormalised, three per
     // pixel), on `stream` (a cudaStream_t) after the work already there, into a device map the builder keeps until its
     // next ray map (*d_map).  globe_source: the globe's globe_plate translated alone, or the bare prelude for argmax
@@ -147,19 +153,25 @@ public:
 
     double last_compile_ms() const { return compile_ms_; }
     double last_kernel_ms() const { return kernel_ms_; }
+    double last_ray_kernel_ms() const { return ray_kernel_ms_; }  // forward_rays: fwd_ray_kernel alone
 
 private:
     struct Module;
     struct ForwardState;
     enum Unit { kInverseUnit, kForwardUnit, kRaymapUnit, kRaysUnit, kProbeUnit };
     Module *module_for(const std::string &source, Unit unit, std::string *err);
+    // forward steps 2-3 on `stream`: the host's grid points and texel owners patched in, then (raster_forward) the
+    // stale slots replayed and every texel's quad rasterised into f.keys
+    bool patch_forward(ForwardState &f, const std::vector<ForwardPatch> &patches, const std::vector<uint32_t> &owner_patches, void *stream,
+                       std::string *err);
+    void raster_forward(ForwardState &f, void *stream);
     int device_;
     std::map<std::string, std::unique_ptr<Module>> cache_;  // by unit + source text
     std::unique_ptr<ForwardState> fwd_;  // between forward_points() and forward_finish()
     DeviceBuffer ray_flagged_;  // ray maps and exports: [0] the flagged count, then the flagged pixels
     DeviceBuffer ray_map_;      // ray maps: the last map, ray_map_pixels_ entries
     size_t ray_map_pixels_ = 0;
-    double compile_ms_ = 0, kernel_ms_ = 0;
+    double compile_ms_ = 0, kernel_ms_ = 0, ray_kernel_ms_ = 0;
 };
 
 }  // namespace blinky

@@ -254,6 +254,44 @@ int blinky_set_raymap_device(blinky_ctx *ctx, int width, int height, int platesi
 int blinky_get_raymap(blinky_ctx *ctx, int width, int height, float *rays);
 int blinky_get_raymap_device(blinky_ctx *ctx, int width, int height, float *d_rays, void *stream);
 
+/* Ray export of a forward lens (DESIGN section 3h): the view rays of any lens whose lens_forward is a
+ * function, whatever its `map`, so that lenses without lens_inverse (sinusoidal, winkel1, ...) can feed
+ * the ray warps too.  Same layout as blinky_get_raymap: float32[height][width][3], dense, ly = 0 the top
+ * row.  The rays come from the forward build of the current lens and globe at width x height on plates
+ * of platesize texels (platesize <= 0: min(width, height), as blinky_build_lensmap; 6 * platesize^2 must
+ * stay below 2^28, so a 4K export wants an explicit platesize), at the scale the current zoom gives for
+ * width x height.  That build's grid points, stale slots, texel owners (plate argmax or globe_plate) and
+ * maxdiff guard apply, and:
+ *   - a pixel is non-zero exactly when that build's lensmap maps it; the others are (0, 0, 0);
+ *   - the texel (P, px, py) that last wrote the pixel drew it with a quad of integer screen corners
+ *     tl, tr (grid row py, v = (py - 1/2) / ps) and bl, br (row py + 1), grid point i at u = (i - 1/2) / ps;
+ *   - measured in half pixels (a corner c came from (int)(x / scale + width/2) and sits at 2c + 1, pixel
+ *     X at 2X), the pixel's (s, t) in the quad (tl = (0,0), tr = (1,0), br = (1,1), bl = (0,1)) comes
+ *     from the first non-degenerate triangle of A = (tl, tr, br), B = (tl, br, bl) that contains it
+ *     (boundary included), by exact integer areas and one double division each; when neither contains it,
+ *     from the first non-degenerate one, clamped to [0, 1]; when both are degenerate, or a corner lies
+ *     further than the raster's maxdiff (20) from tl, s = t = 1/2;
+ *   - the ray is plate_uv_to_ray(P, ((px - 1/2) + s) / ps, ((py - 1/2) + t) / ps), normalised.
+ * It is a function of the build's integer state, so the host and the GPU write the same bits.  Each
+ * corner is within half a pixel of where lens_forward puts its grid point, so away from seams a ray
+ * projects back to within about a pixel of its pixel (DESIGN 3h gives the measured bounds).  Nothing is
+ * printed (no "> maxdiff" lines) and the context does not change, as for blinky_get_raymap;
+ * blinky_build_info reports the export ("ray export (forward), device: ..." or "... host ...").
+ * blinky_get_raymap keeps refusing lenses that map with lens_forward.  On failure the buffer's contents
+ * are unspecified: BLINKY_E_INVALID for NULL or misaligned rays, width / height <= 0 or a platesize
+ * beyond the limit; BLINKY_E_STATE without a valid lens, a lens_forward function or a valid globe;
+ * BLINKY_E_ZOOM when the zoom cannot be computed; BLINKY_E_SCRIPT when lens_forward or globe_plate fails.
+ * blinky_get_raymap_forward runs the serial forward builder on the host and works on host-only contexts.
+ * blinky_get_raymap_forward_device evaluates the grid points on the GPU (the unit blinky_build_lensmap
+ * compiles for this lens), settles the points it cannot prove on the host, and rasterises and writes
+ * d_rays (4-byte aligned device memory) on `stream` (a cudaStream_t, NULL = the default stream) after the
+ * work already there; when that is not possible (no NVRTC, a lens outside the translatable subset) the
+ * host path runs and the field is copied in stream order.  It returns once d_rays holds the field.
+ * BLINKY_E_STATE while `stream` is capturing a graph (nothing is launched); BLINKY_E_NODEVICE on a
+ * host-only context. */
+int blinky_get_raymap_forward(blinky_ctx *ctx, int width, int height, int platesize, float *rays);
+int blinky_get_raymap_forward_device(blinky_ctx *ctx, int width, int height, int platesize, float *d_rays, void *stream);
+
 /* ---- state queries ------------------------------------------------------ */
 int blinky_fisheye_enabled(blinky_ctx *ctx);          /* fisheye_enabled, :293 */
 int blinky_lens_valid(blinky_ctx *ctx);
